@@ -2,15 +2,19 @@
 """bench.py — the BASELINE.json metric: queries/sec (+ decoded-postings/sec) on the synthetic Zipfian index.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload and2|or10|tree8|and2l] [--sub or10,tree8,and2l|none]
+                  [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic queries.  Default workload (BASELINE.json configs[1]): a batch of
 1000 2-term AND queries on the 100M-doc Zipfian synthetic index, GOOGLE codec, DocumentsOnly.  The same run also measures configs[2]
 (10-term OR, BM25 top-100, LUCENE) and configs[3] (8-term AND/OR/NOT trees) at a reduced step count and reports them under
-`workloads` (value, e2e, roofline, parity), so every driver record carries all three at every N.
+`workloads` (value, e2e, roofline, parity), so every record carries all three at every N.
 
   value      whole-job queries/s with the index resident in HBM and results left in HBM (kernels only), CUDA events, max over ranks
   e2e        the same through the public C-ABI call (trn_exec_batch) with HOST buffers: plans H2D + every matched docID (or top-k) D2H
              — the number to quote as throughput
+  --dump-outputs DIR   after the timed steps, what the last end-to-end step returned to its caller, per workload, as DIR/<workload>_<name>.npy
+             (see dump_outputs); the index and the queries are generated from fixed seeds, so two builds run with the same arguments can be
+             compared output for output
   roofline   of the fused exec kernel: SURVEY 8(d) algorithmic bytes (sum of the queries' term chunks + emitted bytes) / event time
   cpu_baseline / parity   the reference's own exec_query (oracle/_ref) on the host cores over a bounded sample of the same batch; its
              results double as the full-size checker of the GPU batch (N = 1: this rank's results; N > 1: per-query match counts and
@@ -81,8 +85,8 @@ def synth_dfs(ndocs: int, nterms: int, min_df: int = 1000) -> np.ndarray:
 def config_of(args, wl, world: int) -> dict:
     """what the job measures — identical in the product arm and the reference arm (no measured quantities in here)"""
     est = float(synth_dfs(args.ndocs, args.nterms).sum()) * BYTES_PER_POSTING[wl["codec"]] / max(1, world)
-    l2 = (f"inputs larger than L2: ~{est / 1e6:.0f} MB of index per GPU vs 126 MB L2, no flush between steps" if est > 126e6
-          else f"TEST SIZE: ~{est / 1e6:.0f} MB of index per GPU fits the 126 MB L2")
+    l2 = (f"inputs larger than L2: ~{est / 1e6:.0f} MB of index per GPU vs 50 MB L2, no flush between steps" if est > 50e6
+          else f"TEST SIZE: ~{est / 1e6:.0f} MB of index per GPU fits the 50 MB L2")
     return {"workload": f"{wl['desc']}; {args.ndocs} docs, {args.nterms} terms, Zipf(1) df, batch {args.nq}, seed 0xC0FFEE",
             "codec": "GOOGLE" if wl["codec"] == 0 else "LUCENE",
             "docid_sharding": f"{world} x contiguous docID range" if world > 1 else "none", "l2": l2}
@@ -109,7 +113,7 @@ def host_info() -> dict:
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md clocks line)"""
+    """nvidia-smi clocks + throttle reasons DURING the timed region"""
 
     def __init__(self, device: int):
         self.device, self.rows, self.proc = device, [], None
@@ -152,25 +156,13 @@ def measured_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(kernel: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel per 1000-query batch, from the committed ncu --set full capture
-    of this same command (profiles/traffic.json, values copied from the ncu summaries it names); None if not captured"""
-    p = ROOT / "profiles" / "traffic.json"
-    if p.exists():
-        try:
-            return json.loads(p.read_text()).get(kernel)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not measured"
 
 
 def numa_bind(local_rank: int, world: int) -> dict:
     """pin this rank's threads (and with them its first-touch pinned allocations) to the NUMA node its GPU hangs off; the node's cores
     are split between the ranks that share it.  Eight unbound ranks on a two-socket host had their result copies cross the socket link
-    (SCALE_r01: e2e at 8 GPUs below 4 GPUs)."""
+    and end-to-end throughput at 8 GPUs fell below that at 4."""
     out = {"bound": False}
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=pci.bus_id", "--format=csv,noheader"], capture_output=True, text=True, timeout=20).stdout.split()
@@ -237,6 +229,47 @@ def sharded_parity(mode, k, n, counts, sums, tsc, g_counts, g_sums, merged_score
         out["topk_scores_max_rel_err"] = worst
         out["topk_scores_within_1e-5"] = bool(worst <= 1e-5)
     return out
+
+
+DUMP_SAMPLE_DOCIDS = 1 << 20  # DocumentsOnly: docIDs kept per workload (16 MB with their positions), at most 1024 per query
+DUMP_SEED = 0xD0C5
+
+
+def dump_outputs(res, mode, k, nq, out_dir: Path, prefix: str) -> int:
+    """Writes what the caller of exec_batch received in `res` as float64 / float32 .npy files, returns the bytes written:
+      <prefix>match_counts          [nq]     matches per query
+      DocumentsOnly (plain or compact):
+      <prefix>docid_sums_mod2p52    [nq]     sum of each query's matched docIDs modulo 2^52 (exact in float64)
+      <prefix>docid_sample          [nq, S]  a seeded sample of each query's docIDs, in result order (-1 = fewer than S matches)
+      <prefix>docid_sample_pos      [nq, S]  the positions in the query's result the sample was taken at (-1 likewise)
+      top-k: <prefix>topk_docids, <prefix>topk_scores  [nq, k]  (score desc, docID asc), -1 past the query's last entry
+    Set results are exact and repeat bit for bit. BM25 scores are fp32 sums accumulated in no fixed order, so they can differ in the last
+    bits from run to run, and two docIDs whose scores are that close can trade places: compare top-k dumps with a tolerance."""
+    import trinity_b200 as tb
+    out_dir.mkdir(parents=True, exist_ok=True)
+    counts = np.asarray(res.match_counts[:nq], np.uint64)
+    arrays = {"match_counts": counts.astype(np.float64)}
+    if mode == tb.MODE_SCORED_TOPK:
+        ids, sc = np.full((nq, k), -1.0), np.full((nq, k), -1.0, np.float32)
+        for q in range(nq):
+            d, s = res.query(q)
+            ids[q, : len(d)], sc[q, : len(s)] = d, s
+        arrays.update(topk_docids=ids, topk_scores=sc)
+    else:
+        S = max(1, min(1024, DUMP_SAMPLE_DOCIDS // max(1, nq)))
+        sums, sample, pos = np.zeros(nq), np.full((nq, S), -1.0), np.full((nq, S), -1.0)
+        for q in range(nq):
+            d = np.asarray(res.query(q)[0])
+            sums[q] = int(d.sum(dtype=np.uint64)) % (1 << 52)
+            n = len(d)
+            at = np.arange(n) if n <= S else np.sort(np.random.default_rng([DUMP_SEED, q]).choice(n, S, replace=False))
+            sample[q, : len(at)], pos[q, : len(at)] = d[at], at
+        arrays.update(docid_sums_mod2p52=sums, docid_sample=sample, docid_sample_pos=pos)
+    total = 0
+    for name, a in arrays.items():
+        np.save(out_dir / f"{prefix}{name}.npy", a)
+        total += a.nbytes
+    return total
 
 
 def reference_sample(r, texts, scored, k, cores, budget_s):
@@ -308,7 +341,7 @@ class Job:
                                                     a.ndocs, synth.sum_hits), synth)
         return self.refs[codec][0]
 
-    def run(self, workload: str, K: int, W: int, cpu_budget_s: float, with_clocks: bool) -> dict:
+    def run(self, workload: str, K: int, W: int, cpu_budget_s: float, with_clocks: bool, dump_dir: Path | None = None) -> dict:
         import trinity_b200 as tb
         from trinity_b200.sharded import device_view
         torch, dist, args, world, rank = self.torch, self.dist, self.args, self.world, self.rank
@@ -388,6 +421,8 @@ class Job:
         torch.cuda.synchronize()
         e2e_s = time.perf_counter() - t0
         clocks = sampler.stop() if sampler else None
+        # read before the next exec call: with copy=False `res` views buffers the engine reuses
+        dumped = dump_outputs(res, mode, args.k, args.nq, dump_dir, f"{workload}_") if dump_dir is not None and rank == 0 else None
         # the same end-to-end step with plain 32-bit docIDs out (TRN_MODE_DOCS_ONLY), for comparison with the compact encoding
         plain = None
         if emode != mode:
@@ -427,9 +462,6 @@ class Job:
         nlaunch = max(1, int(round(float(np.mean([t.get("chunks", 1.0) for t in tms]))))) if tms else 1
         k_ms_step = float(np.mean(kern_ms)) if kern_ms else None          # all fused-kernel launches of one step
         k_ms = k_ms_step / nlaunch if k_ms_step else None                 # average duration of ONE launch
-        traffic = ncu_traffic(f"{kernel_name}:{workload}") if (world == 1 and args.ndocs == 100_000_000 and args.nq == 1000) else None
-        if traffic is not None:
-            traffic = int(traffic) // nlaunch  # the capture is per 1000-query batch; the line reports per launch, like `achieved`
         algo_bytes = (int(res.index_bytes_touched) + out_bytes_per_batch) // nlaunch   # algorithmic bytes of ONE launch
         achieved = algo_bytes / (k_ms * 1e-3) / 1e9 if k_ms else None
 
@@ -459,12 +491,14 @@ class Job:
                     "matched_docids_per_step": matches_per_batch, "plain_u32": plain},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": traffic, "peak_source": peak_src,
+                         "frac": (achieved / peak) if achieved else None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": k_ms, "launches_per_step": nlaunch,
                          "note": "achieved = SURVEY 8(d) algorithmic bytes (every referenced list once per query, skipped blocks included) / kernel time: an EFFECTIVE rate, not HBM utilisation (the kernels skip blocks and are instruction-issue bound); see DESIGN.md section 4"},
         }
         if clocks is not None:
             line["clocks"] = clocks
+        if dumped is not None:
+            line["dumped_bytes"] = dumped
 
         # ---------------- reference leg: CPU baseline + full-size parity (rank 0 runs the reference; every rank contributes its results)
         if not args.no_cpu_baseline:
@@ -527,6 +561,8 @@ def main():
                          "replayed by trn_result_decode) or plain 32-bit docIDs (TRN_MODE_DOCS_ONLY)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-numa-bind", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", type=Path, default=None,
+                    help="write what the last timed end-to-end step returned, per workload, as DIR/<workload>_<name>.npy (at N > 1: rank 0's shard)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -537,7 +573,7 @@ def main():
         return reference_arm(args, rank, world, K, W)
 
     job = Job(args)
-    line = job.run(args.workload, K, W, cpu_budget_s=30.0, with_clocks=True)
+    line = job.run(args.workload, K, W, cpu_budget_s=30.0, with_clocks=True, dump_dir=args.dump_outputs)
     line["numa"] = job.numa
     subs = []
     if args.sub == "auto":
@@ -551,8 +587,9 @@ def main():
             for c in list(job.indexes):
                 if c != WORKLOADS[w]["codec"]:
                     job.drop_index(c)
-            sub = job.run(w, min(K, 3), 3, cpu_budget_s=12.0, with_clocks=False)
-            keep = ("value", "unit", "ms_per_step", "steps", "warmup", "config", "e2e", "roofline", "decoded_postings_per_s", "gpu_launches", "parity", "cpu_baseline")
+            sub = job.run(w, K, 3, cpu_budget_s=12.0, with_clocks=False, dump_dir=args.dump_outputs)
+            keep = ("value", "unit", "ms_per_step", "steps", "warmup", "config", "e2e", "roofline", "decoded_postings_per_s", "gpu_launches", "parity", "cpu_baseline",
+                    "dumped_bytes")
             line["workloads"][w] = {k2: sub[k2] for k2 in keep if k2 in sub}
     if rank == 0:
         print(json.dumps(line))

@@ -1,5 +1,5 @@
 /*
- * trinity_b200 — C ABI of the B200-native execution engine for Trinity's inverted-index hot path
+ * trinity_b200 — C ABI of the GPU-native (H100, sm_90a) execution engine for Trinity's inverted-index hot path
  * (postings-block decode -> docset AND/OR/NOT -> per-doc BM25 -> top-k).
  *
  * This is the drop-in boundary: plain pointers and sizes, int return codes (0 = ok, <0 = error; the message is

@@ -1,7 +1,7 @@
 #!/usr/bin/env bash
 # TEST INFRASTRUCTURE — builds the *reference's own* hot-path code (read in place from
 # /root/reference, never copied into this repo) plus oracle/ref_harness.cpp into
-# oracle/_ref/libtrinity_ref.so.  Outputs ONLY under oracle/_ref/ (git-ignored, travels via gpurun).
+# oracle/_ref/libtrinity_ref.so.  Outputs ONLY under oracle/_ref/ (git-ignored; reused as is where the reference tree is absent).
 #
 # Two compile fixes are applied on the fly (g++ 13 instead of the reference's clang++):
 #   1. queryexec_ctx.h:269-277 anonymous struct with std::vector members (clang extension):

@@ -23,7 +23,7 @@ device_encode = "--device-encode" in sys.argv
 argv = [a for a in sys.argv if a != "--device-encode"]
 ndocs = int(argv[1]) if len(argv) > 1 else 100_000_000
 out_path = argv[2] if len(argv) > 2 else None
-peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6650.0
+peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0  # H100 SXM data sheet
 NT = 4096
 want = {}
 for t in (4095, 2000, 300):

@@ -11,7 +11,7 @@ import trinity_b200 as tb
 
 ndocs = int(sys.argv[1]) if len(sys.argv) > 1 else 100_000_000
 only = sys.argv[2].lower() if len(sys.argv) > 2 else ""
-peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6650.0
+peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0  # H100 SXM data sheet
 for codec, name in ((0, "GOOGLE"), (1, "LUCENE")):
     if only and not only.startswith(name.lower()):
         continue

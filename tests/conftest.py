@@ -14,7 +14,7 @@ sys.path.insert(0, str(ROOT / "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the kernels are built for sm_90a)")
 
 
 @pytest.fixture(scope="session", autouse=True)

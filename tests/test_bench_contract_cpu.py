@@ -90,3 +90,35 @@ def test_reference_side_binding_fails_loudly_without_a_gpu(ref):
     assert "CUDA" in refg.err()
     ids, _ = r.exec("a AND b", False, 4000)  # no twin registered: the stock CPU span
     assert np.array_equal(ids, np.arange(6, 2000, 6, dtype=np.uint32))
+
+
+def test_dump_outputs_writes_what_the_caller_received(tmp_path):
+    """--dump-outputs: float arrays only, docIDs exact, the sample drawn from a fixed seed (two runs write the same files)"""
+    import numpy as np
+
+    sys.path.insert(0, str(ROOT))
+    import bench
+    import trinity_b200 as tb
+
+    counts = np.array([3, 0, 5000], np.uint64)
+    off = np.concatenate([np.zeros(1, np.int64), np.cumsum(counts).astype(np.int64)])
+    ids = np.concatenate([np.array([7, 99_999_999, 4_000_000_000], np.uint32), np.arange(1, 10_001, 2, dtype=np.uint32)])
+    res = tb.BatchResult(3, tb.MODE_DOCS_ONLY, 0, off, ids, None, counts, 0, 0, 0, 0.0)
+    for run in ("a", "b"):
+        assert bench.dump_outputs(res, tb.MODE_DOCS_ONLY, 100, 3, tmp_path / run, "and2_") <= 64 << 20
+    names = sorted(p.name for p in (tmp_path / "a").iterdir())
+    assert names == ["and2_docid_sample.npy", "and2_docid_sample_pos.npy", "and2_docid_sums_mod2p52.npy", "and2_match_counts.npy"]
+    for n in names:
+        a, b = np.load(tmp_path / "a" / n), np.load(tmp_path / "b" / n)
+        assert a.dtype in (np.float32, np.float64) and np.array_equal(a, b), n
+    sample, pos = np.load(tmp_path / "a" / "and2_docid_sample.npy"), np.load(tmp_path / "a" / "and2_docid_sample_pos.npy")
+    assert list(sample[0, :4]) == [7, 99_999_999, 4_000_000_000, -1] and (sample[1] == -1).all()
+    at = pos[2][pos[2] >= 0].astype(np.int64)
+    assert len(at) == 1024 and np.array_equal(sample[2, :1024], ids[3:][at])
+    assert list(np.load(tmp_path / "a" / "and2_docid_sums_mod2p52.npy")) == [4_100_000_006, 0, 25_000_000]
+
+    topk = tb.BatchResult(2, tb.MODE_SCORED_TOPK, 2, np.array([0, 2, 4]), np.array([5, 9, 3, 0], np.uint32),
+                          np.array([2.5, 1.0, 0.5, -1.0], np.float32), np.array([2, 1], np.uint64), 0, 0, 0, 0.0)
+    bench.dump_outputs(topk, tb.MODE_SCORED_TOPK, 2, 2, tmp_path / "t", "or10_")
+    assert np.array_equal(np.load(tmp_path / "t" / "or10_topk_docids.npy"), [[5, 9], [3, -1]])
+    assert np.array_equal(np.load(tmp_path / "t" / "or10_topk_scores.npy"), np.array([[2.5, 1.0], [0.5, -1.0]], np.float32))

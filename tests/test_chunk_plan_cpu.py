@@ -1,5 +1,5 @@
-"""How trn_exec_batch splits a batch into pipelined launches (csrc/chunkplan.h, the function the engine itself calls) on the scenarios the
-rule was tuned on (profiles/r02_y, r02_z, r02_ab, r02_ac): first batch of a shape by referenced postings; afterwards by the previous batch's
+"""How trn_exec_batch splits a batch into pipelined launches (csrc/chunkplan.h, the function the engine itself calls) on the benchmark's
+scenarios: first batch of a shape by referenced postings; afterwards by the previous batch's
 result size, c = sqrt(D / 4 tail), the last chunk tapered into 1/2, 1/4, 1/4."""
 import ctypes as C
 
@@ -39,19 +39,19 @@ def test_first_batch_of_a_shape_goes_by_referenced_postings():
 
 
 def test_result_size_rule_on_the_measured_scenarios():
-    # and2 at N = 1: 0.675 GB out -> D = 15 ms, tail 0.15 -> 5 chunks + taper (profiles/r02_ac: 45.5K q/s e2e)
+    # and2 at N = 1: 0.675 GB out -> D = 15 ms, tail 0.15 -> 5 chunks + taper
     single, s = plan(**AND2, hint_bytes=674_787_528, hint_postings=AND2["est"], same=True)
     assert not single and len(s) == 7 and s[:4] == [200] * 4 and s[4:] == [100, 50, 50]
-    # one of 8 shards: 92.6 MB -> D = 2.06 ms -> 2 chunks + taper (3.84-3.92 ms per call)
+    # one of 8 shards: 92.6 MB -> D = 2.06 ms -> 2 chunks + taper
     single, s = plan(**AND2_SHARD, hint_bytes=92_574_116, hint_postings=AND2_SHARD["est"], same=True)
     assert not single and s == [500, 250, 125, 125]
-    # tree8 at N = 1: 0.54 GB, tree tail 0.9 ms -> 2 chunks + taper (10.66K q/s e2e vs 10.0K with 8 + 2)
+    # tree8 at N = 1: 0.54 GB, tree tail 0.9 ms -> 2 chunks + taper
     single, s = plan(**TREE8, hint_bytes=540_682_420, hint_postings=TREE8["est"], same=True)
     assert not single and s == [500, 250, 125, 125]
-    # tree8 on one of 8 shards: 67 MB = 1.5 ms of copy is not worth two 0.9 ms tails -> one call (15.5 ms vs 23.3 ms in 8 chunks)
+    # tree8 on one of 8 shards: 67 MB = 1.5 ms of copy is not worth two 0.9 ms tails -> one call
     single, s = plan(**TREE8_SHARD, hint_bytes=67_373_840, hint_postings=TREE8_SHARD["est"], same=True)
     assert single and s == [1000]
-    # a lone chunk whose copy IS worth two launches is still tapered (and2 shard with the 0.3 ms tail of profiles/r02_ab)
+    # a lone chunk whose copy IS worth two launches is still tapered (and2 shard with a 0.3 ms tail)
     single, s = plan(**AND2_SHARD, hint_bytes=92_574_116, hint_postings=AND2_SHARD["est"], same=True, tail_ms=0.3)
     assert not single and s == [500, 250, 250]
 

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path (through the C ABI) vs the reference's own CPU code (oracle/_ref).
+"""GPU parity tests: the sm_90a path (through the C ABI) vs the reference's own CPU code (oracle/_ref).
 docID sets bit-exact; BM25 within 1e-5 relative (north_star)."""
 import numpy as np
 import pytest

@@ -1,8 +1,8 @@
-"""trinity_b200 — B200-native execution engine for Trinity's inverted-index hot path.
+"""trinity_b200 — GPU-native (H100, sm_90a) execution engine for Trinity's inverted-index hot path.
 
 Thin Python plumbing over the C ABI (include/trinity_b200.h).  Class and method names follow the reference's
 domain vocabulary (IndexSession/Encoder, IndexSource, exec_query, term_index_ctx, postings, docsets);
-all decode / docset / scoring work happens in the sm_100a kernels of libtrinity_b200.so — there is no CPU path.
+all decode / docset / scoring work happens in the sm_90a kernels of libtrinity_b200.so — there is no CPU path.
 """
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
-"""Builds libtrinity_b200.so (sm_100a CUDA kernels + host C++ + C ABI) in-tree with nvcc.
+"""Builds libtrinity_b200.so (sm_90a CUDA kernels + host C++ + C ABI) in-tree with nvcc.
 
-Run as `python -m trinity_b200.build` or through `__graft_entry__.build()`.  The shared object is
-git-ignored but travels with gpurun snapshots.
+Run as `python -m trinity_b200.build` or through `__graft_entry__.build()`.  The shared object and the
+object files under build/ are git-ignored.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ CU_SOURCES = ["kernels.cu", "engine.cu"]
 CXX_SOURCES = ["codecs.cpp", "host_api.cpp", "segment.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
 ]

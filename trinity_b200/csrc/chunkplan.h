@@ -31,12 +31,12 @@ inline ChunkPlan plan_chunks(const ChunkPlanIn &in) {
         uint32_t  nchunks  = std::max(1u, in.max_chunks);
         bool      taperOne = false;
         if (nchunks > 1) {
-                // a chunk must be worth its launch tails: as many chunks as the referenced postings pay for (profiles/r02_h: on one of 8 shards the
-                // whole batch is 2.75 ms of kernel time, 4.4 ms in 8 launches)
+                // a chunk must be worth its launch tails: as many chunks as the referenced postings pay for (a batch of a docID shard holds so
+                // little kernel time that eight launches cost more in tails than the overlapped copy saves)
                 nchunks = uint32_t(std::min<uint64_t>(nchunks, std::max<uint64_t>(1, in.est_postings / std::max<uint64_t>(1, in.chunk_postings))));
                 // With the result size of the previous batch of this shape known, the chunk count balances what chunking buys against what it
                 // costs: c chunks (the last one tapered) expose 1/(4c) of the result copy (D ms at ~45 GB/s) and add c + 2 launch tails — minimum
-                // at c = sqrt(D / (4 tail)).  Measured: profiles/r02_t, r02_y, r02_z, r02_ab, r02_ac (engine.cu, trn_exec_batch).
+                // at c = sqrt(D / (4 tail)) (engine.cu, trn_exec_batch).
                 if (in.rule_sqrt && in.hint_bytes && in.hint_same_shape && in.est_postings >= in.hint_postings - in.hint_postings / 4 &&
                     in.est_postings <= in.hint_postings + in.hint_postings / 4) {
                         const double D    = double(in.hint_bytes) / 45e6; // ms

@@ -136,7 +136,7 @@ namespace Codecs {
 // >= (tf_base + j) << tf_shift.  The entries cover only [first_doc, last_doc] of the term (inside THIS index source: a docID-range
 // shard indexes its own range), and tf_shift is the smallest granularity >= kDirMinShift that keeps the table at or below one entry
 // per kDirBlocksPerEntry blocks — so the whole directory is O(blocks + terms), never terms x tiles.  A lookup reads two neighbouring
-// entries and finishes with a binary search over the blk_last entries between them (dependent loads: profiles/r02_n shows them as the
+// entries and finishes with a binary search over the blk_last entries between them (dependent loads: they were the
 // top stall of the candidate probes when a frequent term had 128 blocks per 8192-document entry, hence the finer granularity: a term
 // with 64 docIDs per block gets 512-docID entries = 8 blocks = 3 steps); smaller terms (tf_shift == kDirNoTable) search all of blk_last.
 static constexpr uint32_t kDirMinShift       = 9;

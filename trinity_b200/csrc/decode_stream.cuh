@@ -2,7 +2,7 @@
 // parity probe of the decoders) == PostingsListIterator::next() over whole lists (google_codec.cpp:777-819 + unpack_block :596-639;
 // lucene_codec.cpp:568-594 + refill_documents :515-558 + FastPFor<4> __decodeArray fastpfor.h:222-270).  (Included by kernels.cu.)
 //
-// The round-1 decoders were instruction-bound at 16-24 % of the HBM roofline (profiles/r01_g, r01_j): a register-staged copy loop
+// The first decoders were instruction-bound at a fraction of the HBM roofline: a register-staged copy loop
 // (LDG -> STS: the top stall line), a byte-wise varbyte walk through generic pointers and a second pass to find the freq section.
 // Here
 //   * the bytes of a unit (32 consecutive blocks of one term: a contiguous span of the chunk, positions included) arrive by ONE 1-D bulk

@@ -87,7 +87,7 @@ struct trn_ctx {
         int          device{0};
         cudaStream_t stream{nullptr};
         std::string  err;
-        int          num_sms{148};
+        int          num_sms{132}; // set from the device in trn_create
         // index
         bool                 have_index{false};
         int                  codec{0};
@@ -96,11 +96,11 @@ struct trn_ctx {
         uint32_t             min_docid{1}; // smallest docID any term holds (a docID-range shard does not start at 1)
         uint32_t             nterms{0}, max_docid{0}, tile_shift{13}, ntiles{0}; // tile_shift: directory granularity == scored tile (8192 docs, the reference's window docset_spans.h:74)
         uint32_t             docs_shift{14}; // docID tile (log2) of the warp-per-tile DocumentsOnly kernel
-        bool                 tree_masks{false}; // TRN_TREE_MASKS=1: flat-tree queries decode their frequent leaves in a masked second pass (flat_tree_masks). Measured
-                                                // (profiles/r02_i..k): halves the DRAM bytes, but the needed blocks of a tile fill a fraction of a 32-lane group, so
-                                                // the warp-instruction count does not drop: 8.5-9.0K vs 9.2-11.1K q/s on the benchmark's trees. Off by default.
-                                                // (profiles/r02_ag: not a matter of WHICH leaves are admitted — 8.2-8.4K q/s with TRN_TREE_MASK_NEED 0.6 ... 0.05 vs
-                                                // 11.2K off: a few masked queries raise the launch-wide slot count and take resident warps from every query.)
+        bool                 tree_masks{false}; // TRN_TREE_MASKS=1: flat-tree queries decode their frequent leaves in a masked second pass (flat_tree_masks). It
+                                                // halves the DRAM bytes, but the needed blocks of a tile fill a fraction of a 32-lane group, so the warp-instruction
+                                                // count does not drop and the benchmark's trees ran slower with it. Off by default. (Not a matter of WHICH leaves
+                                                // are admitted — TRN_TREE_MASK_NEED does not recover it: a few masked queries raise the launch-wide slot count and
+                                                // take resident warps from every query.)
         uint32_t             tree_shift{13}; // TRN_TREE_SHIFT: docID tile (log2) of the flat-tree launch of k_exec_docs (0 = flat-tree path off)
         uint32_t             run_tiles{128};  // TRN_RUN_TILES: consecutive tiles per work item of the flat scored kernel (top-k state lives across a run)
         int                  flat_threads{320}; // TRN_SF_THREADS: CTA size of k_score_flat (256/320/384: two CTAs per SM; 512/640: one)
@@ -135,7 +135,7 @@ struct trn_ctx {
         uint64_t     hint_bytes{0}, hint_postings{0}; // result bytes / referenced postings of the previous host-buffer batch ...
         uint32_t     hint_nq{0};                     // ... and its shape: the next batch of the same shape sizes its chunks from them
         int          hint_mode{-1};
-        uint32_t     pipeline_chunks{8}; // TRN_PIPELINE_CHUNKS (profiles/r02_n: 4 -> 38.4K, 6 -> 40.1K, 8 -> 40.7K, 12 -> 40.1K q/s end to end on the headline batch)
+        uint32_t     pipeline_chunks{8}; // TRN_PIPELINE_CHUNKS: upper bound of the chunk plan (chunkplan.h)
         uint32_t     last_items{0}; // work items of the last exec_device_impl call (compact results: entries of item_desc)
         uint64_t     last_total_hint{0};
         // host-side breakdown of the last trn_exec_batch / trn_exec_batch_device call (trn_last_timings)
@@ -243,7 +243,7 @@ struct Compiler {
 
         // Slots: in DocumentsOnly plans a child's bitmap is dead once it has been combined into its parent, so its slot is handed out
         // again (scored plans keep every slot: the deferred scoring pass reads branch bitmaps at the end).  Fewer live slots = less
-        // shared memory per worker = more resident warps (the 8-term trees ran at 12 warps/SM with one slot per node, profiles/r01_u_*).
+        // shared memory per worker = more resident warps (with one slot per node the 8-term trees left few warps resident per SM).
         std::vector<uint32_t> free_slots;
         int alloc_slot() {
                 if (!scored && !free_slots.empty()) {
@@ -1189,7 +1189,7 @@ extern "C" int trn_query_truth_table(const trn_qnode *nodes, uint32_t nnodes, ui
 // Leaf bitmaps are numbered by descending block count: the (leaf, block) list of a tile is then ordered from the frequent terms (blocks
 // of 1-byte deltas, four codes per decoder step) to the rare ones (2-byte deltas, blocks that straddle the tile), so that the 32 lanes
 // of a group mostly walk blocks of the same kind — a rare term's lane among frequent ones kept the whole warp in the loop for its 16-31
-// slow steps (profiles/r02_g: the slow steps ran at 5.8 of 32 lanes and were as many instructions as the fast ones).
+// slow steps (those ran at a few of 32 lanes and were as many instructions as the fast ones).
 // Afterwards the copies are coalesced (flat_tree_coalesce): `SET d <- s` where s is not read again becomes a renaming of d, so a chain
 // like SET t <- leaf; AND t, leaf2; OR acc, t runs in the leaf's own bitmap: fewer operations per tile and — what matters more — fewer
 // bitmaps per warp (13 -> 8 for the 8-term trees of the benchmark), i.e. more resident warps.
@@ -1796,7 +1796,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 const uint32_t planSlots = cc.next_slot + 1; // + scratch slot (applied below, once the path of the query is known)
                 // Candidate-driven evaluation (exec_docs_cand.cuh) when some term that EVERY match must hold is sparse: cost follows that
                 // lead's postings (~cand_cost/2 warp-instructions per 32 candidates and probed term; the crossover was tuned on the and2
-                // workload: 900 beats 450 and 1500) instead of the docID space (~1500 per tile + ~27 per block in it, profiles/r01_l_*).
+                // workload: 900 beats 450 and 1500) instead of the docID space (~1500 per tile + ~27 per block in it).
                 // The boolean function of the tree over its (<= 8 distinct) terms is tabulated here; the device probes every term for
                 // each candidate and looks the membership bits up.
                 bool candidate{false};
@@ -1910,7 +1910,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 }
                 // Flat-tree path (exec_docs_flat.cuh): a DocumentsOnly tree that is neither an all-term run nor candidate-driven decodes ALL its
                 // leaves of a tile in one flat (leaf, block) pass — each leaf into a bitmap of its own — and then runs slot operations only.
-                // The per-leaf groups of the step-program path ran at 10 of 32 lanes with up to 8 live bitmaps per warp (profiles/r01_u); here
+                // The per-leaf groups of the step-program path ran at a third of the lanes with up to 8 live bitmaps per warp; here
                 // the lanes are packed across leaves, and a smaller tile pays for the extra bitmaps.
                 bool treeFlat{false};
                 if (!scored && !candidate && dq.flat == 0u && c->codec == TRN_CODEC_GOOGLE && c->tree_shift && !r.empty() && !cc.has_phrase) {
@@ -2289,9 +2289,7 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
         if (!c || !out)
                 return TRN_ERR_ARG;
         // how the batch is split into pipelined launches: chunkplan.h (a pure function of what is known here, pinned on the CPU by
-        // tests/test_chunk_plan_cpu.py).  Measured (profiles/r02_t, r02_y, r02_z, r02_ab, r02_ac): and2 at N = 1 45.3-46.3K q/s end to end with
-        // 3..6 + 2 launches vs 44.7K with 8 + 2; tree8 10.66K with 2 + 2 vs 10.0K with 8 + 2; one of 8 shards: and2 3.84 ms with 2 + 2 launches,
-        // 3.88 with 1 + 2, 4.32 with 4 + 2, 4.52 with one; the LUCENE conjunction 8.51 ms with 2 + 2 vs 8.83 with 1 + 2.
+        // tests/test_chunk_plan_cpu.py).
         ChunkPlanIn pin;
         pin.nq   = nq;
         pin.topk = mode == TRN_MODE_SCORED_TOPK;
@@ -2749,7 +2747,7 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
         if (units) {
                 const int grid = int(std::min<uint64_t>(uint64_t(c->num_sms) * 8, (units + 3) / 4));
                 // GOOGLE: the materialising variant uses the single-pass kernel with 16-byte vector stores (k_decode_google); the fused
-                // checksum-only variant is faster with the span-staged kernel (measured, profiles/r01_g_microbench_decode.txt)
+                // checksum-only variant is faster with the span-staged kernel (scripts/microbench_decode.py compares the two)
                 const bool forceNew = decodeKernel == "single-pass";
                 if (!legacyDecode)
                         CK(launch_decode_stream(dev_index(c), c->d_dec_units.as<DecUnit>(), c->d_dec_c.as<uint64_t>(), uint32_t(units),

@@ -4,8 +4,8 @@
 // exec_docs_flat.cuh) or a 32-block group of a lead term for the candidate-driven path (exec_docs_cand.cuh); the host picks the path
 // per query (engine.cu, exec_device_impl).
 //
-// Why a second kernel: the ncu capture of the CTA-per-tile kernel on the 2-term AND workload (profiles/r01_a_*) showed DRAM at 5 % of
-// peak, 37 % issue utilisation and 47 % of all stall samples on CTA barriers — 4 warps waiting for the slowest lane-serial block
+// Why a second kernel: the ncu capture of the CTA-per-tile kernel on the 2-term AND workload showed DRAM far from
+// peak, low issue utilisation and half of all stall samples on CTA barriers — 4 warps waiting for the slowest lane-serial block
 // decode at every step.  Set queries need no score tile, so the whole per-tile state (2-3 slot bitmaps + one staging area) fits a
 // warp: every warp is an independent worker that never waits for another warp (only __syncwarp), and the SM always has
 // as many runnable decode chains as it has resident warps.
@@ -19,7 +19,7 @@ static constexpr uint32_t kGatherBytes     = 80;  // bytes of a block's head eac
 static constexpr uint32_t kGatherBufBytes  = 32 * kGatherBytes;  // one group
 // per-warp staging: ONE gather buffer + a 128-word area (need-list of the block-skipping path / scratch words of the word builders / Lucene
 // exception patches).  A second, prefetching buffer was measured and dropped: it costs a quarter of the resident warps (24 instead of 32
-// per SM) and lost 49 vs 53 ms on the headline batch (profiles/r01_e, r01_l).
+// per SM) and made the headline batch slower.
 static constexpr uint32_t kDocsStageBytes1 = kGatherBufBytes + 512;
 
 // ---- lane-gather staging with cp.async (LDGSTS): no registers, no L1 allocation, completion tracked per group
@@ -97,8 +97,8 @@ __device__ __forceinline__ uint32_t lds_u8(uint32_t saddr) {
         return v;
 }
 
-// Byte-wise decoder over the lane's gather slot.  The ncu capture of the span-staged whole-list decoder (plain byte loads,
-// profiles/r01_j_*) needs 2.0 warp-instructions per posting for deltas AND freqs at 30/32 lanes, fewer than the 64-bit-window decoder
+// Byte-wise decoder over the lane's gather slot.  The span-staged whole-list decoder (plain byte loads) needs about
+// two warp-instructions per posting for deltas AND freqs with nearly all lanes active, fewer than the 64-bit-window decoder
 // spends on deltas alone: a 1-byte code costs one LDS.U8, one compare and the adds.  Codes of up to two bytes (gaps < 16384) always
 // lie inside the 80-byte slot (31 x 2 + 15 bytes of alignment slack); the first longer code switches the lane to global memory.
 template <class SINK>
@@ -144,8 +144,7 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {
 // Plain-store word builder for a bitmap that only ONE term writes (flat conjunctions keep one slot per operand).  The blocks of
 // a term partition the docID space, so every 32-doc word strictly between a block's first and last word belongs to that block's
 // lane alone: it is written with a predicated STS when the lane moves on — no atomic, and no branch (ptxas turns a predicated
-// red.shared into BSSY / BRA / ATOMS / BSYNC: three control instructions per posting and the branch-resolve stalls of
-// profiles/r01_k_*).  Only a block's LAST word can be shared, with the following block(s) of the term; the caller ORs it in
+// red.shared into BSSY / BRA / ATOMS / BSYNC: three control instructions per posting and branch-resolve stalls).  Only a block's LAST word can be shared, with the following block(s) of the term; the caller ORs it in
 // atomically AFTER those have stored (see flat_exec_google).
 struct OwnAcc {
         uint32_t bm;           // shared-state-space address of the term's bitmap
@@ -179,8 +178,8 @@ __device__ __forceinline__ void own_add_if(OwnAcc &bs, bool on, uint32_t rel) {
 }
 
 // Warp-voted decoder into an OwnAcc.  Its predecessor let every lane choose between a 4-wide body and byte-wise excursions on its
-// own; the ncu capture (profiles/r01_l_*) shows what that cost: 6 % of the 4-byte words hold a 2-byte code, but each of them sent its
-// warp through ~3 byte-wise iterations at 2 of 32 lanes — more instructions than the 4-wide body itself.  Here every iteration reads a 32-bit window at ANY byte position (two aligned shared loads + funnel shift:
+// own, which cost this: few of the 4-byte words hold a 2-byte code, but each of them sent its
+// warp through ~3 byte-wise iterations at a few of 32 lanes — more instructions than the 4-wide body itself.  Here every iteration reads a 32-bit window at ANY byte position (two aligned shared loads + funnel shift:
 // no alignment prologue, no re-alignment), and the warp votes: all lanes see four 1-byte codes => the 4-wide body; otherwise ALL
 // lanes run one predicated, branch-free step that consumes the leading 1-byte codes of the window plus the first 2-byte code
 // (1..4 postings).  The two bodies are never executed in the same iteration.
@@ -256,7 +255,7 @@ __device__ __forceinline__ void google_block_docs_vote(unsigned m, const uint8_t
 
 // Per-lane decoder into an OwnAcc — no votes: every lane walks ITS block through 32-bit windows of its gather slot, four 1-byte codes per
 // window when it can, else up to two codes of 1-2 bytes (two such codes always fit a window); a longer code sends the lane to global
-// memory for the rest of the block.  Used where the lanes of a group belong to different lists (flat-tree plans: profiles/r02_f shows the
+// memory for the rest of the block.  Used where the lanes of a group belong to different lists (flat-tree plans: there the
 // warp-voted decoder above paying its one-code-per-step path for the whole warp whenever ONE lane holds a 2-byte code): a lane in a
 // sparse list then costs the lanes in dense lists an idle step, not a slow step.
 // `past`: 2^31 - W when every docID of the source is below 2^31 (a docID relative to the tile start in [W, 2^31) then lies BEHIND the tile
@@ -380,7 +379,7 @@ __device__ void google_leaf_warp(const DevIndex &ix, const DevTerm &T, uint32_t 
         } else {
                 // Sparse destination docset (few candidates): first collect the blocks whose docID range still holds a candidate — the
                 // advance()/skiplist step of the reference (google_codec.cpp:821-934) — THEN decode them 32 at a time.  Decoding inside the
-                // scan loop ran the lane-serial block decoder with ~4 of 32 lanes active (profiles/r01_e_*), which cost as many issue slots
+                // scan loop ran the lane-serial block decoder with a few of 32 lanes active, which cost as many issue slots
                 // as all the dense tiles together.
                 uint32_t *     list = reinterpret_cast<uint32_t *>(stage + kGatherBufBytes); // behind the first gather buffer
                 const uint32_t cap  = (stageBytes - kGatherBufBytes) / 4u - 32u;

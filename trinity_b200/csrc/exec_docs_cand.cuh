@@ -4,7 +4,7 @@
 //
 // Why: the bitmap path pays ~1500 warp-instructions per (query, 16384-doc tile) before it decodes anything (slot clears, the
 // word-wise AND, count, emission), and a sparse operand contributes one or two blocks per tile, so most (query, tile) items of the
-// 2-term AND workload are nearly empty groups at a few active lanes (profiles/r01_l_*: 16.8 of 32 threads per instruction; 55 % of
+// 2-term AND workload are nearly empty groups at a few active lanes (most of
 // the work items belong to queries whose rarest term has < 4 blocks per tile).  Here a work item is one GROUP OF 32 BLOCKS OF THE
 // LEAD TERM, wherever its documents lie:
 //   1. lane = block: the 32 blocks are decoded into a candidate array in shared memory (row stride 33 words: conflict-free for
@@ -27,7 +27,7 @@ static constexpr uint32_t kCandInvalid = 0xffffffffu;
 
 // one lane decodes the doc section of ITS staged block into out[0..n).  Branch-free per code: the 32 lanes of a group hold blocks with
 // different mixes of 1-, 2- and 3-byte codes, and a loop that branches on the code length (with early exits) does not reconverge before
-// its end — profiles/r02_n: this function ran at 2.1 of 32 lanes.  Every lane runs the same 31 steps; a lane whose block ends, whose next
+// its end: such a loop ran at a few of 32 lanes.  Every lane runs the same 31 steps; a lane whose block ends, whose next
 // code may leave its 80-byte slot or is longer than 3 bytes goes idle and finishes from global memory afterwards.
 __device__ __forceinline__ void google_block_to_array(const uint8_t *__restrict__ index, uint32_t off, const uint8_t *buf, int lane, uint32_t n, uint32_t prev,
                                                       uint32_t last, uint32_t *out) {

@@ -3,14 +3,14 @@
 //
 // The per-tile blocks of ALL operand terms form one flat (term, block) list that the warp consumes 32 at a time, each lane decoding
 // its block into the bitmap of ITS term; the conjunction is one word-wise AND at the end.  Compared with running the terms one after
-// another this keeps the lanes full when a term has fewer than 32 blocks in the tile (ncu on the term-at-a-time path: 11.7 of 32
-// lanes active per instruction, profiles/r01_b_*).  When the rarest term is sparse inside the tile the caller falls back to the
+// another this keeps the lanes full when a term has fewer than 32 blocks in the tile (the term-at-a-time path kept about a third
+// of the lanes active per instruction).  When the rarest term is sparse inside the tile the caller falls back to the
 // sequential path, whose advance()-style block skipping then saves more than the lane packing gains.
 //
 // Staging: every lane copies only the head of ITS block (kGatherBytes from the 16B-aligned address below the first doc-delta byte)
 // with cp.async (LDGSTS) into its own slot — the doc-delta section of a 32-doc block is at most 31 x 2 bytes for gaps < 16384, and
 // the inline hits behind it (half of the index bytes) never enter the SM.  (The span-copy version kept 6 KB per warp for one group,
-// capped the SM at 20 resident warps and exposed every group's global-load latency: 14 % of all stall samples, profiles/r01_c_*.)
+// capped the SM at 20 resident warps and exposed every group's global-load latency.)
 #pragma once
 
 static constexpr uint32_t kFlatMaxLeaves = 16;
@@ -183,7 +183,7 @@ __device__ void google_leaf_own(const DevIndex &ix, const DevTerm &T, uint32_t b
 // Flat-tree plans (DevQuery::flat == 5): a DocumentsOnly tree that is neither an all-term run nor candidate-driven.  The host puts one
 // [OP_LEAF M_NONE dst = j] marker per leaf at the front of the program (leaf j owns bitmap slot j) and turns the rest into slot operations.
 // Per tile: ONE flat (leaf, block) pass decodes every leaf's blocks into its own bitmap with the plain-store word builder (lanes packed
-// across leaves: the per-leaf groups of the step-program path ran at 10 of 32 lanes, profiles/r01_u), then the slot operations run as
+// across leaves: the per-leaf groups of the step-program path ran at a third of the lanes), then the slot operations run as
 // 128-bit vector operations.  Everything that depends only on the query — the leaves' term records, the slot operations (packed into one
 // word each) — is loaded ONCE per query into lane registers (lane j: leaf j; lane k: operation k) and reused for all of its tiles.
 struct TreeState {

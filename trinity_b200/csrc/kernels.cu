@@ -1,4 +1,4 @@
-// sm_100a kernels of the trinity_b200 hot path.
+// sm_90a kernels of the trinity_b200 hot path.
 //
 //   k_exec_tiles   fused postings-block decode -> docset algebra -> BM25 accumulate -> emit / top-k candidates
 //                  one work item = (query, docID tile of 2^tile_shift docs); persistent CTAs pull items from a ticket.
@@ -285,7 +285,7 @@ __device__ __forceinline__ uint32_t lucene_intblock(const uint8_t *s, uint32_t o
         if (cexcept) {
                 // Exception patching (fastpfor.h:248-266): out[pos] |= exc << b.  Lane e owns exception e; the patched values travel through a
                 // warp-private scratch (the first version had EVERY lane walk ALL exceptions: ~15 instructions x cexcept per int-block,
-                // the top instruction hot spot of the OR/BM25 profile profiles/r01_f_*).
+                // the top instruction hot spot of the OR/BM25 workload).
                 const uint32_t maxbits = bytes[2];
                 const uint32_t k       = maxbits - b;
                 const uint32_t excw    = meta + 4u + ((bytesize + 3u) & ~3u) + 8u; // past bitmap word and count word

@@ -6,8 +6,8 @@
 // (lucene_codec.cpp:515-594, fastpfor.h:222-270), Scorer::score (similarity.h:228-235) and the application's top-k sink (matches.h:155-171).
 //
 // Why a second scored kernel: the general step-program kernel (k_exec_tiles) runs a disjunction term after term with a CTA barrier in
-// between — its ncu capture on this workload (profiles/r01_n) shows 8 warp-instructions per posting, 38 % issue utilisation and 2.6
-// warps stalled on barriers per issue: half of the ten terms of a query have at most one block in a tile, and three of four warps
+// between — on this workload it spends several warp-instructions per posting, with low issue utilisation and
+// warps stalled on barriers: half of the ten terms of a query have at most one block in a tile, and three of four warps
 // wait while one decodes it.  Here
 //   * a tile's blocks of ALL terms form one flat (term, block) list that the 8 warps consume round-robin, with NO barrier between terms:
 //     scores are added to the fp32 tile with shared-memory atomics (a document can be hit by two warps working on different terms);
@@ -124,8 +124,8 @@ __device__ __forceinline__ uint32_t lucene_intblock_v(const uint8_t *s, uint32_t
 // acc[rel[g]] += sc[g] for the postings selected by `on` (bit g), atomically (another warp may be adding another term's score to the
 // same document).  Shared memory has no native fp32 add: atomicAdd compiles to a load / add / compare-and-swap loop per posting, and four
 // of them in a row are four serialised ~100-cycle chains.  Here the four loads, adds and CAS attempts are issued side by side; a CAS that
-// lost a race (rare) retries on its own.  (Measured alternative, profiles/r02_t: scores as u32 fixed-point units with native ATOMS.ADD — same
-// instruction count, the uncontended CAS chains cost little, and 5 % SLOWER on the 10-term OR workload: 1867 vs 1973 q/s; not kept.)
+// lost a race (rare) retries on its own.  (Measured alternative: scores as u32 fixed-point units with native ATOMS.ADD — same instruction count, the
+// uncontended CAS chains cost little, and slower on the 10-term OR workload; not kept.)
 __device__ __forceinline__ void sf_add4(float *acc, const uint32_t rel[4], const float sc[4], uint32_t on) {
         uint32_t *a = reinterpret_cast<uint32_t *>(acc);
         uint32_t  old[4], seen[4];
