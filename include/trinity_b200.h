@@ -305,6 +305,22 @@ int trn_debug_chunk_plan(uint32_t nq, int topk, uint64_t est_postings, uint64_t 
                          double tail_ms, double tail_tree_ms, uint64_t hint_bytes, uint64_t hint_postings, int hint_same_shape, uint32_t *sizes, uint32_t cap,
                          uint32_t *n, int *single_call);
 
+/* Debug view (tests, tooling): the path the host chose for every query of the last trn_exec_batch / trn_exec_batch_device call, one
+ * TRN_ROUTE_* code per query into out[0..cap); *n = the batch's query count (TRN_ERR_CAPACITY if cap is smaller; 0 after a failed call).
+ * DocumentsOnly plans run in k_exec_docs as a step program, a flat AND / OR of terms (GOOGLE), the candidate-driven conjunction (GOOGLE)
+ * or a flat tree (GOOGLE); scored plans run in k_score_flat (LUCENE flat OR / single term) or k_exec_tiles.  A flat AND needs one docset
+ * slot per operand: it is reported as a step program when its launch has fewer slots (the effective limit is min(16, slots of the launch);
+ * conjunctions of <= 3 terms raise the slot count themselves).  The codes are plan-level: a flat AND whose rarest operand is sparse in
+ * a tile still runs that tile as a step program, and such per-tile choices are not visible here. */
+#define TRN_ROUTE_STEPS 0        /* DocumentsOnly: step program of k_exec_docs                       */
+#define TRN_ROUTE_FLAT_AND 1     /* DocumentsOnly: flat conjunction of terms (GOOGLE)                */
+#define TRN_ROUTE_FLAT_OR 2      /* DocumentsOnly: flat disjunction of terms (GOOGLE)                */
+#define TRN_ROUTE_CANDIDATE 3    /* DocumentsOnly: candidate-driven evaluation (GOOGLE)              */
+#define TRN_ROUTE_SCORE_FLAT 4   /* scored: k_score_flat (LUCENE)                                    */
+#define TRN_ROUTE_FLAT_TREE 5    /* DocumentsOnly: flat-tree form of the step program (GOOGLE)       */
+#define TRN_ROUTE_EXEC_TILES 6   /* scored: step program of k_exec_tiles                             */
+int trn_debug_last_routes(trn_ctx *, uint8_t *out, uint32_t cap, uint32_t *n);
+
 /* Split form used by bench.py / multi-GPU: run on device only, results stay in HBM ... */
 int trn_exec_batch_device(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out_counts_only);
 /* ... device pointers of the last SCORED_TOPK run: nq*k u32 docids, nq*k f32 scores (unused slots: docid 0, score -1.0; real scores are >= 0), nq u32 counts */

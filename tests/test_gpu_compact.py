@@ -1,7 +1,8 @@
 """TRN_MODE_DOCS_COMPACT on the device: the same DocumentsOnly plans, results leaving the GPU as per-tile bitmaps / 16-bit offsets /
 docIDs (whichever is smallest), replayed on the host by trn_result_decode — must equal the plain DocumentsOnly stream and the reference's
-exec_query, on every path of k_exec_docs (candidate-driven, flat AND/OR, flat-tree, step programs; both codecs), through the pipelined
-call (large batch) and the single-call form (small batch), with masked documents, and for a docID-range shard."""
+exec_query, on every path of k_exec_docs (GOOGLE: step programs, flat AND/OR and flat-tree plans in the first test, candidate-driven plans
+in the second; LUCENE: step programs — asserted through GpuIndexSource.last_routes), through the pipelined call (large batch) and the
+single-call form (small batch), with masked documents, and for a docID-range shard."""
 import numpy as np
 import pytest
 
@@ -48,7 +49,12 @@ def test_compact_equals_plain_and_reference(ref, codec):
     encodings = set()
     for batch in (plans, plans[:5]):  # pipelined call (>= 32 queries) and the single-call form
         plain = g.exec_batch(batch, tb.MODE_DOCS_ONLY)
+        routes = set(g.last_routes().tolist())
         comp = g.exec_batch(batch, tb.MODE_DOCS_COMPACT, copy=False)
+        assert set(g.last_routes().tolist()) == routes
+        if batch is plans:  # the paths this test claims to cover were taken
+            want_routes = {tb.ROUTE_STEPS, tb.ROUTE_FLAT_AND, tb.ROUTE_FLAT_OR, tb.ROUTE_FLAT_TREE} if codec == tb.CODEC_GOOGLE else {tb.ROUTE_STEPS}
+            assert routes >= want_routes if codec == tb.CODEC_GOOGLE else routes == want_routes, routes
         assert np.array_equal(comp.match_counts, plain.match_counts)
         assert comp.result_bytes() <= plain.result_bytes() + 4 * comp.nitems
         desc = np.ctypeslib.as_array(comp.raw.item_desc, shape=(max(comp.nitems, 1),))[: comp.nitems]
@@ -97,6 +103,7 @@ def test_compact_sparse_results_and_a_shard(ref):
     qs = ["t1 AND t2", "t1 AND t5", "t4 AND t6", "t1 OR t2", "t3 AND (t1 OR t2)", "(t1 AND t2) OR (t3 AND t7)", "t1 AND t2 AND t7", "t1 NOT t2", "t6", "t1"] * 4
     plans = [tb.parse_query(q, tdict) for q in qs]
     comp = g.exec_batch(plans, tb.MODE_DOCS_COMPACT, copy=False)
+    assert tb.ROUTE_CANDIDATE in g.last_routes().tolist()
     for i, q in enumerate(qs[:10]):
         assert_same_docs(comp.decode_query(i), r.exec(q, False, ndocs + 1)[0], f"[{q}] shard")
     g.close()

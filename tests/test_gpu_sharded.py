@@ -3,7 +3,10 @@ uploaded into S separate device-resident IndexSources (what S ranks would hold),
 concatenate in shard order, top-k lists go through the exchange step's own merge kernel (`trn_merge_topk` == k_topk_merge on the
 all-gathered [shard][nq][k] layout).  Reference: exec_query over the whole index (exec.h:56-61,84-177; BM25 over collection statistics,
 similarity.h:209-217).  Covers shards whose first docID is not 1, shards where a term is empty, k that no shard can fill, ties across
-shards."""
+shards.  The closed-form freq pattern gives exact ties wherever a document's score has at most two contributions (a + b is the same float
+in either order): those top-k plans are checked strictly, docID order at every rank included (assert_topk_exact).  The 10-term OR and the
+two-conjunction OR sum more contributions, in an order that differs between the kernels and the reference, so their tie classes need not
+be bit-identical: they are checked modulo near-ties (assert_topk_equal)."""
 import numpy as np
 import pytest
 import torch
@@ -11,7 +14,7 @@ import torch
 import trinity_b200 as tb
 from refharness import RefIndex
 from trinity_b200.sharded import device_view, shard_range
-from util import Pair, assert_same_docs, assert_topk_equal, closed_form_lists
+from util import Pair, assert_same_docs, assert_topk_equal, assert_topk_exact, closed_form_lists
 
 pytestmark = pytest.mark.gpu
 CODECS = [tb.CODEC_GOOGLE, tb.CODEC_LUCENE]
@@ -21,6 +24,7 @@ DOCS_QUERIES = [
     "t10", "t9 AND t10", "rare AND t1", "rare OR t10", "t2 AND t3 AND t5 NOT rare", "[t1, t2, t3, t4]",
 ]
 TOPK_QUERIES = [" OR ".join(f"t{i}" for i in range(1, 11)), "t1 AND t2", "t3 OR t7", "rare OR t10", "t10", "rare", "(t1 AND t2) OR (t3 AND t4)"]
+EXACT_TIES = {"t1 AND t2", "t3 OR t7", "rare OR t10", "t10", "rare"}  # at most two contributions per document
 
 
 def _lists(ndocs):
@@ -94,7 +98,8 @@ def test_sharded_results_equal_unsharded_reference(ref, codec, nshards):
             wd, ws = whole.ref.exec(q, True, ndocs + 1)
             assert counts[i] == len(wd), f"{nshards} shards [{q}]: summed match counts"
             keep = ms[i] >= 0
-            assert_topk_equal(md[i][keep], ms[i][keep], wd, ws, k, f"{nshards} shards [{q}] k={k}")
+            check = assert_topk_exact if q in EXACT_TIES else assert_topk_equal
+            check(md[i][keep], ms[i][keep], wd, ws, k, f"{nshards} shards [{q}] k={k}")
     for s in shards:
         s.gpu.close()
 

@@ -101,6 +101,24 @@ def test_compact_segments_replay_in_every_encoding():
     assert lib().trn_result_for_each(C.byref(r), 0, fn, None) == 0 and len(seen) == 10
 
 
+@pytest.mark.parametrize("shift", [13, 14])
+def test_compact_segments_of_the_last_tile_below_2_32(shift):
+    """the tile base of the last tile of the docID space: (tile_lo << tile_shift) + offset must reach 2^32 - 2 without wrapping"""
+    top = 2**32 - 2  # largest valid docID (DocIDsEND = 2^32 - 1)
+    tile_lo = (2**32 >> shift) - 1
+    first = tile_lo << shift
+    ids = np.array([first, first + 1, first + 255, first + 256, first + (1 << shift) // 2, top - 1, top], np.uint32)
+    qs = [(tile_lo, [ids], [enc]) for enc in (ENC_U16, ENC_U8B, ENC_BITMAP)]
+    # and one query whose last item is the top tile, behind the tile below it
+    below = ids - np.uint32(1 << shift)
+    qs.append((tile_lo - 1, [below, ids], [ENC_U8B, ENC_U16]))
+    r, keep = _compact(qs, shift)
+    for q, (_, items, _) in enumerate(qs):
+        want = np.concatenate(items)
+        rc, n, got = _decode(r, q, len(want))
+        assert rc == 0 and n == len(want) and np.array_equal(got, want), (shift, q, got)
+
+
 def test_plain_results_replay_too():
     ids = np.array([2, 5, 9, 11, 400], np.uint32)
     off = np.array([0, 2, 2, 5], np.uint64)

@@ -7,12 +7,13 @@ import trinity_b200 as tb
 from refharness import RefIndex
 
 PRIMES = [2, 3, 5, 7, 11, 13, 17, 19, 23, 29]
+PRIMES18 = PRIMES + [31, 37, 41, 43, 47, 53, 59, 61]  # t11 .. t18: plans wider than the kernels' leaf limits
 
 
-def closed_form_lists(ndocs: int):
-    """term t_i = multiples of PRIMES[i] (SURVEY.md Appendix C); freq pattern gives BM25 something to chew on"""
+def closed_form_lists(ndocs: int, primes=PRIMES):
+    """term t_i = multiples of primes[i] (SURVEY.md Appendix C); freq pattern gives BM25 something to chew on"""
     out = []
-    for p in PRIMES:
+    for p in primes:
         d = np.arange(p, ndocs + 1, p, dtype=np.uint32)
         f = (1 + (d // p) % 5).astype(np.uint32)
         out.append((d, f))
@@ -47,6 +48,29 @@ class Pair:
         return nodes
 
 
+def merged_topk(gpus, plans, k):
+    """SCORED_TOPK on every shard, the per-shard lists gathered as [shard][nq][k] on the device and merged by trn_merge_topk
+    (the exchange step of the multi-GPU path) -> per query (docIDs, scores), padding dropped"""
+    import torch
+    from trinity_b200.sharded import device_view
+    ns, nq = len(gpus), len(plans)
+    gd = torch.zeros((ns, nq, k), dtype=torch.int32, device="cuda")
+    gs = torch.zeros((ns, nq, k), dtype=torch.float32, device="cuda")
+    for si, g in enumerate(gpus):
+        g.exec_batch_device(plans, tb.MODE_SCORED_TOPK, k)
+        dptr, sptr, _ = g.last_topk_device()
+        torch.cuda.synchronize()
+        gd[si].view(-1).copy_(device_view(dptr, nq * k, torch.int32))
+        gs[si].view(-1).copy_(device_view(sptr, nq * k, torch.float32))
+    md = torch.zeros((nq, k), dtype=torch.int32, device="cuda")
+    ms = torch.zeros((nq, k), dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    gpus[0].merge_topk(gd.data_ptr(), gs.data_ptr(), ns, nq, k, md.data_ptr(), ms.data_ptr())
+    torch.cuda.synchronize()
+    md, ms = md.cpu().numpy().view(np.uint32), ms.cpu().numpy()
+    return [(md[i][ms[i] >= 0], ms[i][ms[i] >= 0]) for i in range(nq)]
+
+
 def assert_same_docs(got: np.ndarray, want: np.ndarray, what: str):
     if len(got) != len(want) or not np.array_equal(got, want):
         n = min(len(got), len(want))
@@ -72,6 +96,24 @@ def ref_topk(ids: np.ndarray, scores: np.ndarray, k: int):
     """(score desc, docID asc) top-k of the reference's full (id, score) stream"""
     order = np.lexsort((ids, -scores))[:k]
     return ids[order], scores[order]
+
+
+def assert_topk_exact(gd, gs, rd, rs_all, k, what, rtol=1e-5):
+    """strict top-k parity for corpora whose tie classes come out bit-identical on both sides: the docIDs equal the reference's
+    (score desc, docID asc) top-k at EVERY rank, ties included, and the scores agree within rtol.  The reference's scores are ranked as
+    float32, the type the top-k sink keeps (a tie class the GPU sees as one float is one class here too)."""
+    rd = np.asarray(rd, np.uint32)
+    rs32 = np.asarray(rs_all, np.float32)
+    order = np.lexsort((rd, -rs32))[:k]
+    td, ts = rd[order], np.asarray(rs_all, np.float64)[order]
+    gd = np.asarray(gd, np.uint32)
+    assert len(gd) == len(td), f"{what}: top-k length {len(gd)} != {len(td)}"
+    if not np.array_equal(gd, td):
+        i = int(np.flatnonzero(gd != td)[0])
+        lo = max(0, i - 2)
+        raise AssertionError(f"{what}: top-k docID at rank {i}: got {gd[lo:i + 3]} (scores {np.asarray(gs)[lo:i + 3]}) "
+                             f"want {td[lo:i + 3]} (scores {ts[lo:i + 3]})")
+    assert_close_scores(gs, ts, what + " (top-k scores)", rtol)
 
 
 def assert_topk_equal(gd, gs, rd, rs_all, k, what, rtol=1e-5):

@@ -18,6 +18,8 @@ CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
 MODE_DOCS_COMPACT = 3  # DocumentsOnly, compact result segments (bitmap / bucketed 8-bit offsets / 16-bit offsets / docIDs per tile): trn_result_decode replays them
 NODE_TERM, NODE_AND, NODE_OR, NODE_NOT, NODE_OPTIONAL, NODE_SOME, NODE_PHRASE = 0, 1, 2, 3, 4, 5, 6
+# the path a query ran (GpuIndexSource.last_routes, == TRN_ROUTE_* of include/trinity_b200.h)
+ROUTE_STEPS, ROUTE_FLAT_AND, ROUTE_FLAT_OR, ROUTE_CANDIDATE, ROUTE_SCORE_FLAT, ROUTE_FLAT_TREE, ROUTE_EXEC_TILES = 0, 1, 2, 3, 4, 5, 6
 EMPTY_TERM = 0xFFFFFFFF
 DOC_IDS_END = 0xFFFFFFFF  # DocIDsEND, common.h:43
 
@@ -451,6 +453,13 @@ class GpuIndexSource:
         t = TrnTimings()
         self._ck(self._L.trn_last_timings(self._h, C.byref(t)))
         return {n: float(getattr(t, n)) for n, _ in TrnTimings._fields_}
+
+    def last_routes(self) -> np.ndarray:
+        """debug: the path (ROUTE_*) every query of the last exec_batch / exec_batch_device call ran"""
+        n = C.c_uint32()
+        out = np.zeros(max(getattr(self, "_last", (0, 0, 0))[2], 1), np.uint8)
+        self._ck(self._L.trn_debug_last_routes(self._h, _ptr(out), len(out), C.byref(n)))
+        return out[: n.value].copy()
 
     def last_topk_device(self):
         d, s, c = C.c_void_p(), C.c_void_p(), C.c_void_p()

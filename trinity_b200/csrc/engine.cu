@@ -145,6 +145,8 @@ struct trn_ctx {
         uint32_t last_nq{0}, last_k{0}, last_launches{0};
         uint64_t last_postings{0}, last_bytes{0};
         float    last_ms{0};
+        // path (TRN_ROUTE_*) of every query of the last exec_device_impl call / of the last whole batch (trn_debug_last_routes)
+        std::vector<uint8_t> call_routes, last_routes;
 };
 
 #define CK(call)                                                                                                                                               \
@@ -1723,6 +1725,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         uint32_t              maxSlots{1};
         bool                  anyCandidate{false}, anyMembership{false}, anyPhrase{false};
         uint64_t              items{0}, segCap{0}, candTotal{0}, postings{0}, bytes{0};
+        c->call_routes.assign(nq, 0);
         for (uint32_t q = 0; q < nq; ++q) {
                 const auto &Q = queries[q];
                 if (!Q.nodes || !Q.nnodes)
@@ -1931,6 +1934,14 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 }
                 if (!flatScored && !treeFlat)
                         maxSlots = std::max(maxSlots, planSlots);
+                // the path this query takes (trn_debug_last_routes): scored plans run k_score_flat or k_exec_tiles; the LUCENE
+                // instantiation of k_exec_docs has no flat AND / OR form and runs those plans as step programs
+                if (scored)
+                        c->call_routes[q] = flatScored ? TRN_ROUTE_SCORE_FLAT : TRN_ROUTE_EXEC_TILES;
+                else if (c->codec == TRN_CODEC_LUCENE && (dq.flat == 1u || dq.flat == 2u))
+                        c->call_routes[q] = TRN_ROUTE_STEPS;
+                else
+                        c->call_routes[q] = uint8_t(dq.flat); // 0 steps, 1 flat AND, 2 flat OR, 3 candidate-driven, 5 flat-tree (== TRN_ROUTE_*)
                 if (candidate) {
                 } else if (r.empty()) {
                         dq.tile_lo = 0;
@@ -1981,6 +1992,16 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 if (need > stageB)
                         maxSlots = std::max(maxSlots, (need - stageB + slotBytes - 1u) / slotBytes);
         }
+        // a flat conjunction keeps one bitmap per operand: with more operands than the launch has slots, flat_exec_google hands every
+        // tile to the step program (the launch's slot count is final only here)
+        for (uint32_t q = 0; q < nq; ++q)
+                if (c->call_routes[q] == TRN_ROUTE_FLAT_AND) {
+                        uint32_t nleaf{0};
+                        for (uint32_t si = 0; si < hq[q].nsteps; ++si)
+                                nleaf += steps[hq[q].step_begin + si].op == OP_LEAF;
+                        if (nleaf > maxSlots)
+                                c->call_routes[q] = TRN_ROUTE_STEPS;
+                }
 
         // ---- result staging must fit the device: a caller (trn_exec_batch) reacts to TRN_ERR_CAPACITY by splitting the batch
         if (mode != TRN_MODE_SCORED_TOPK) {
@@ -2186,12 +2207,14 @@ extern "C" int trn_exec_batch_device(trn_ctx *c, const trn_query *queries, uint3
         CK(cudaSetDevice(c->device));
         c->have_kernel_events = false;
         c->tm                 = trn_timings{};
+        c->last_routes.clear();
         const double t0       = now_ms();
         CK(cudaEventRecord(c->ev0, c->stream));
         const int r = exec_device_impl(c, queries, nq, mode, k, out, 0, c->evk0, c->evk1);
         c->tm.total_ms = float(now_ms() - t0);
         if (r != TRN_OK)
                 return r;
+        c->last_routes = c->call_routes;
         CK(cudaEventRecord(c->ev1, c->stream));
         return TRN_OK;
 }
@@ -2334,6 +2357,8 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
         }
         CK(cudaSetDevice(c->device));
         c->tm            = trn_timings{};
+        c->last_routes.clear();
+        std::vector<uint8_t> routes(nq, 0);
         const double tB0 = now_ms();
         const bool scored = mode == TRN_MODE_SCORED_ALL;
         CK(c->h_offsets.ensure((size_t(nq) + 1) * 8));
@@ -2449,6 +2474,7 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
                 }
                 if (r != TRN_OK)
                         return r;
+                std::copy(c->call_routes.begin(), c->call_routes.end(), routes.begin() + ch[i].q0);
                 CK(cudaEventRecord(c->ev_done[set], c->stream));
                 if (compact) {
                         if (chunkItems.size() <= i) {
@@ -2510,7 +2536,19 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
                 out->device_ms = ms;
         out->exec_kernel_ms = ksum;
         // the split-form API (trn_fetch_results / trn_last_topk_device) refers to a whole batch; a pipelined call leaves none behind
-        c->last_mode = -1;
+        c->last_mode   = -1;
+        c->last_routes = std::move(routes);
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_last_routes(trn_ctx *c, uint8_t *out, uint32_t cap, uint32_t *n) {
+        if (!c || !n)
+                return TRN_ERR_ARG;
+        *n = uint32_t(c->last_routes.size());
+        if (cap < *n)
+                return fail(c, TRN_ERR_CAPACITY, "trn_debug_last_routes: buffer too small");
+        if (*n)
+                std::memcpy(out, c->last_routes.data(), *n);
         return TRN_OK;
 }
 

@@ -328,25 +328,6 @@ __device__ __forceinline__ void google_block_docs_gather(unsigned, const uint8_t
         google_block_docs_bytes(index, off, buf, lane, n, prev, last, lo, W, bs);
 }
 
-// generic-pointer fallback (blocks that do not fit the staging area are read straight from global memory)
-template <bool INTERIOR>
-__device__ __forceinline__ void google_block_docs(const uint8_t *p, uint32_t n, uint32_t prev, uint32_t last, uint32_t lo, uint32_t hi, BitSink &bs) {
-        uint32_t doc = prev;
-        for (uint32_t i = 0; i + 1u < n; ++i) {
-                doc += varbyte_get(p);
-                if (INTERIOR)
-                        bs.add(doc - lo);
-                else {
-                        if (doc >= hi)
-                                return;
-                        if (doc >= lo)
-                                bs.add(doc - lo);
-                }
-        }
-        if (INTERIOR || (last >= lo && last < hi))
-                bs.add(last - lo);
-}
-
 // Decode blocks [bA, bB] of a Google term into the warp's bitmap.  `sparse`: the destination docset holds few candidates — check each
 // block's docID range against it first and skip blocks (and whole groups) without candidates.
 __device__ void google_leaf_warp(const DevIndex &ix, const DevTerm &T, uint32_t bA, uint32_t bB, uint32_t lo, uint32_t hi, BitSink &bs, const uint32_t *skipfilt,

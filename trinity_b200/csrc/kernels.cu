@@ -165,18 +165,20 @@ __device__ __forceinline__ void google_block(const uint8_t *p, uint32_t n, uint3
                 for (uint32_t i = 0; i + 1 < n; ++i)
                         pf += varbyte_len(*pf);
         }
-        uint32_t doc = prev;
+        const uint32_t W = hi - lo; // tile membership is doc - lo < W: hi wraps to 0 for the last tile of a 2^32 docID space
+        uint32_t       doc = prev;
         for (uint32_t i = 0; i + 1 < n; ++i) {
                 doc += varbyte_get(p);
                 uint32_t fr = 0;
                 if (NEED_FREQ)
                         fr = varbyte_get(pf);
-                if (doc >= hi)
-                        return;
-                if (doc >= lo)
+                if (doc >= lo) {
+                        if (doc - lo >= W)
+                                return;
                         v.visit(doc, fr);
+                }
         }
-        if (last >= lo && last < hi) {
+        if (last - lo < W) {
                 uint32_t fr = 0;
                 if (NEED_FREQ)
                         fr = varbyte_get(pf);
@@ -365,7 +367,7 @@ __device__ void lucene_leaf(const DevIndex &ix, const DevTerm &T, uint32_t bA, u
 #pragma unroll
                         for (int t = 0; t < 4; ++t) {
                                 const uint32_t doc = base + d[t];
-                                if (doc >= lc.lo && doc < lc.hi)
+                                if (doc - lc.lo < lc.hi - lc.lo) // (not doc < hi: hi wraps to 0 for the last tile of a 2^32 docID space)
                                         lc.visit(doc, f[t]);
                         }
                 } else {
@@ -383,10 +385,11 @@ __device__ void lucene_leaf(const DevIndex &ix, const DevTerm &T, uint32_t bA, u
                                 for (uint32_t i = 0; i < tail; ++i) {
                                         doc += varbyte_get(p);
                                         const uint32_t fr = varbyte_get(p);
-                                        if (doc >= lc.hi)
-                                                break;
-                                        if (doc >= lc.lo)
+                                        if (doc >= lc.lo) {
+                                                if (doc - lc.lo >= lc.hi - lc.lo)
+                                                        break;
                                                 lc.visit(doc, fr);
+                                        }
                                 }
                         }
                 }
