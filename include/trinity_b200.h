@@ -320,6 +320,12 @@ int trn_debug_chunk_plan(uint32_t nq, int topk, uint64_t est_postings, uint64_t 
 #define TRN_ROUTE_FLAT_TREE 5    /* DocumentsOnly: flat-tree form of the step program (GOOGLE)       */
 #define TRN_ROUTE_EXEC_TILES 6   /* scored: step program of k_exec_tiles                             */
 int trn_debug_last_routes(trn_ctx *, uint8_t *out, uint32_t cap, uint32_t *n);
+/* Host-only view of the same decision (tests, tooling; no GPU needed): plans a batch as trn_exec_batch would on a context that trn_create
+ * made with this environment and that holds this index (trn_upload_index's arguments), without executing it.  routes[0..nq) receives the
+ * TRN_ROUTE_* of every query, nslots[0] the docset slots of the step-program launch (k_exec_docs / k_exec_tiles), nslots[1] those of the
+ * flat-tree launch of k_exec_docs.  LUCENE phrase plans are refused as on a context without trn_upload_hits. */
+int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
+                   uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap);
 
 /* Split form used by bench.py / multi-GPU: run on device only, results stay in HBM ... */
 int trn_exec_batch_device(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out_counts_only);

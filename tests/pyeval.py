@@ -77,7 +77,7 @@ def evaluate(nodes, lists, ndocs, weights=None, quirk=True, positions=None):
             return sum(sorted(kids)[:max(0, len(kids) - int(n["term"]) + 1)])
         return min(kids) if kind == tb.NODE_AND else sum(kids)
 
-    # the reference's root-Filter-over-disjunction quirk (exec.cpp:488-501 + docset_spans.cpp:98-111), see engine.cu
+    # the reference's root-Filter-over-disjunction quirk (exec.cpp:488-501 + docset_spans.cpp:98-111), see planner.cpp
     root, traversed = 0, False
     while int(nodes[root]["kind"]) == tb.NODE_NOT and cost(int(nodes[root]["first_child"]) + 1) <= cost(int(nodes[root]["first_child"])):
         root, traversed = int(nodes[root]["first_child"]), True

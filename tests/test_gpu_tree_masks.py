@@ -1,4 +1,4 @@
-"""Flat-tree plans with the masked second decode pass (engine.cu flat_tree_masks, exec_docs_flat.cuh tree_exec_google) on the device vs the
+"""Flat-tree plans with the masked second decode pass (planner.cpp flat_tree_masks, exec_docs_flat.cuh tree_exec_google) on the device vs the
 reference's exec_query: a skewed vocabulary (df from 10 to half of the documents) so that frequent leaves are decoded block-selectively
 under masks built from the rare ones; every tree shape of the benchmark plus nested ones, random term choices; documents bit-exact.
 Also with TRN_TREE_MASKS=0 (one pass) and for a source that does not start at docID 1 (a shard)."""

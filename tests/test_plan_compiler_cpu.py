@@ -1,4 +1,4 @@
-"""The plan compiler (engine.cu Compiler == build_iterator + build_span flattened into slot operations) checked WITHOUT a GPU: its step
+"""The plan compiler (planner.cpp Compiler == build_iterator + build_span flattened into slot operations) checked WITHOUT a GPU: its step
 programs, interpreted on the CPU (tests/stepsim.py), must give the documents and scores of the structural evaluator — which is itself
 pinned against the reference's exec_query (test_frontend_cpu).  Covers slot reuse (DocumentsOnly), the deferred scoring passes,
 MatchSome counters and the reference's root-filter quirk."""
@@ -84,7 +84,7 @@ TREE8 = ["({0} OR {1}) AND ({2} OR {3}) AND {4} NOT ({5} OR {6} OR {7})", "{0} A
 
 
 def test_flat_tree_masked_second_pass_matches_the_structural_evaluator():
-    """flat-tree programs with the masked second decode pass (engine.cu flat_tree_masks): frequent leaves keep only the postings inside
+    """flat-tree programs with the masked second decode pass (planner.cpp flat_tree_masks): frequent leaves keep only the postings inside
     a mask computed from the other leaves — whatever subset of the postings outside the mask survives, the documents must not change"""
     ndocs = 300_000
     rng = np.random.default_rng(77)

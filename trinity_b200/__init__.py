@@ -263,6 +263,34 @@ def query_truth_table(nodes: np.ndarray):
     return [int(terms[j]) for j in range(n.value)], tb_, int(nec.value)
 
 
+def _pack_queries(queries: Sequence[np.ndarray]):
+    arr = (TrnQuery * len(queries))()
+    keep = []
+    for i, q in enumerate(queries):
+        q = np.ascontiguousarray(q, dtype=QNODE_DTYPE)
+        keep.append(q)
+        arr[i].nodes = q.ctypes.data
+        arr[i].nnodes = len(q)
+        arr[i].root = 0
+    return arr, keep
+
+
+def debug_plan(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequence[np.ndarray], mode: int, k: int = 100, max_docid: int = 0):
+    """(routes, (nslots, tree_slots)): the path (ROUTE_*) every query of the batch would run and the docset slots of the step-program and
+    flat-tree launches, planned on the host as a GpuIndexSource created with this environment would (no GPU needed)"""
+    index = np.ascontiguousarray(index, dtype=np.uint8)
+    terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)
+    arr, keep = _pack_queries(queries)
+    routes = np.zeros(max(len(queries), 1), np.uint8)
+    slots = (C.c_uint32 * 2)()
+    err = C.create_string_buffer(256)
+    rc = lib().trn_debug_plan(codec, _ptr(index), index.size, _ptr(terms), len(terms), max_docid, C.cast(arr, C.c_void_p), len(queries), mode, k,
+                              _ptr(routes), slots, err, 256)
+    if rc != 0:
+        raise TrinityError(err.value.decode("utf-8", "replace") or f"rc={rc}")
+    return routes[: len(queries)].copy(), (int(slots[0]), int(slots[1]))
+
+
 def bm25_idf(doc_freq: int, docs_cnt: int) -> float:
     return float(lib().trn_bm25_idf(doc_freq, docs_cnt))
 
@@ -384,15 +412,7 @@ class GpuIndexSource:
         return nodes
 
     def _pack(self, queries: Sequence[np.ndarray]):
-        arr = (TrnQuery * len(queries))()
-        keep = []
-        for i, q in enumerate(queries):
-            q = np.ascontiguousarray(q, dtype=QNODE_DTYPE)
-            keep.append(q)
-            arr[i].nodes = q.ctypes.data
-            arr[i].nnodes = len(q)
-            arr[i].root = 0
-        return arr, keep
+        return _pack_queries(queries)
 
     def exec_batch_device(self, queries: Sequence[np.ndarray], mode: int, k: int = 100, packed=None):
         arr, keep = packed if packed is not None else self._pack(queries)

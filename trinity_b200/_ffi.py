@@ -21,7 +21,7 @@ EXPORTS = [
     "trn_create", "trn_destroy", "trn_last_error", "trn_set_stream", "trn_upload_index", "trn_set_masked_documents", "trn_index_info_get",
     "trn_exec_batch", "trn_exec_batch_device", "trn_last_topk_device", "trn_merge_topk", "trn_fetch_results", "trn_last_timings",
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_debug_chunk_plan",
-    "trn_debug_last_routes",
+    "trn_debug_last_routes", "trn_debug_plan",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -141,5 +141,6 @@ def lib() -> C.CDLL:
         P(u32), P(i32))
     sig("trn_encode_google", i32, vp, vp, u32, vp, vp, vp, u32, u32, P(u32), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_debug_last_routes", i32, vp, vp, u32, P(u32))
+    sig("trn_debug_plan", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, P(u32), C.c_char_p, C.c_size_t)
     _lib = L
     return L

@@ -17,7 +17,7 @@ LIB = ROOT / "libtrinity_b200.so"
 OBJ = ROOT / "build"
 
 CU_SOURCES = ["kernels.cu", "engine.cu"]
-CXX_SOURCES = ["codecs.cpp", "host_api.cpp", "segment.cpp"]
+CXX_SOURCES = ["codecs.cpp", "host_api.cpp", "planner.cpp", "segment.cpp"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -1,6 +1,8 @@
-// Device-side data layout shared by engine.cu (host) and kernels.cu (device).
+// Device-side data layout shared by the host (planner.cpp, engine.cu) and kernels.cu (device).
 #pragma once
+#include "../../include/trinity_b200.h"
 #include <cstdint>
+#include <vector_types.h>
 
 namespace trn {
 
@@ -86,13 +88,9 @@ struct DevQuery {
         uint32_t cand_cap;
         uint32_t gen_base;  // the query's first ticket in the step-program launch (k_exec_tiles / k_exec_docs); queries other kernels / launches run own none
         uint32_t gen_base2; // k_exec_docs, second launch (flat-tree plans on a smaller tile): the query's first ticket there
-        uint32_t flat; // 0 = general step program; 1 = conjunction of terms only; 2 = disjunction of terms only (see exec_docs_flat.cuh);
-                       // 3 = candidate-driven (exec_docs_cand.cuh): items are 32-block groups of a lead term every match must hold; the
-                       //     step program is replaced by [OP_LEAF lead, OP_LEAF other terms..., OP_TABLE...]: root_slot = number of NECESSARY
-                       //     terms (they come first), the truth table decides over the membership bits of the others
-                       // 4 = scored flat disjunction run by k_score_flat; 5 = flat-tree (exec_docs_flat.cuh): the program starts with one
-                       //     [OP_LEAF M_NONE dst = leaf slot] per leaf — all leaves of the tile are decoded in ONE flat (leaf, block) pass into
-                       //     bitmaps of their own — followed by slot operations only
+        uint32_t route;     // the path the query runs: TRN_ROUTE_* (include/trinity_b200.h), decided by plan_batch (planner.h).  A candidate-driven
+                            // query's items are 32-block groups of its lead term and root_slot is the number of its necessary terms (plan_batch);
+                            // a flat-tree program has the layout of flat_tree_transform
 };
 
 // ---- flat scored disjunctions (k_score_flat, score_flat.cuh)

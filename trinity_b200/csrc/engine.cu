@@ -1,9 +1,7 @@
 // trn_ctx: the device-resident index source + batch executor behind the C ABI (include/trinity_b200.h).
 // Host responsibilities mirror the host side of the reference's exec path:
 //   * upload == AccessProxy construction + Decoder::init for every term (google_codec.cpp:936-983, lucene_codec.cpp:877-932)
-//   * plan compile == queryexec_ctx::build_iterator + build_span (exec.cpp:253-505): operator tree -> per-tile step program,
-//     including the IteratorScorer combination rules of docset_iterators_scorers.cpp:8-242 (which leaves contribute to a
-//     document's score is structural; see compile_node()).
+//   * plan compile == queryexec_ctx::build_iterator + build_span (exec.cpp:253-505): planner.h (plan_batch), called per batch here
 // There is NO CPU execution fallback: every docset/score operation runs in kernels.cu.
 #include "../../include/trinity_b200.h"
 #include "codecs.h"
@@ -11,6 +9,7 @@
 #include "hitcursor.h"
 #include "chunkplan.h"
 #include "kernels.h"
+#include "planner.h"
 #include <algorithm>
 #include <array>
 #include <chrono>
@@ -90,22 +89,10 @@ struct trn_ctx {
         int          num_sms{132}; // set from the device in trn_create
         // index
         bool                 have_index{false};
-        int                  codec{0};
-        int                  cand_cost{900}; // TRN_CAND_COST: modelled warp-instructions per 32 candidates of the candidate-driven conjunction (0 = never use it)
+        PlanConfig           pc; // the planner's view of the index, its knobs and the kernels' limits (trn_create, trn_upload_index)
         uint32_t             block_docs{32}; // documents per full block of the uploaded index (GOOGLE 32 unless built for the decode sweep; LUCENE 128)
-        uint32_t             min_docid{1}; // smallest docID any term holds (a docID-range shard does not start at 1)
-        uint32_t             nterms{0}, max_docid{0}, tile_shift{13}, ntiles{0}; // tile_shift: directory granularity == scored tile (8192 docs, the reference's window docset_spans.h:74)
-        uint32_t             docs_shift{14}; // docID tile (log2) of the warp-per-tile DocumentsOnly kernel
-        bool                 tree_masks{false}; // TRN_TREE_MASKS=1: flat-tree queries decode their frequent leaves in a masked second pass (flat_tree_masks). It
-                                                // halves the DRAM bytes, but the needed blocks of a tile fill a fraction of a 32-lane group, so the warp-instruction
-                                                // count does not drop and the benchmark's trees ran slower with it. Off by default. (Not a matter of WHICH leaves
-                                                // are admitted — TRN_TREE_MASK_NEED does not recover it: a few masked queries raise the launch-wide slot count and
-                                                // take resident warps from every query.)
-        uint32_t             tree_shift{13}; // TRN_TREE_SHIFT: docID tile (log2) of the flat-tree launch of k_exec_docs (0 = flat-tree path off)
-        uint32_t             run_tiles{128};  // TRN_RUN_TILES: consecutive tiles per work item of the flat scored kernel (top-k state lives across a run)
+        uint32_t             nterms{0}, ntiles{0}; // ntiles: of pc.tile_shift
         int                  flat_threads{320}; // TRN_SF_THREADS: CTA size of k_score_flat (256/320/384: two CTAs per SM; 512/640: one)
-        uint32_t             scored_shift{13};  // TRN_SCORED_SHIFT: log2 of k_score_flat's tile (13 = the reference's window, 14)
-        int                  flat_scored{1}; // TRN_FLAT_SCORED=0: every scored query through the general step-program kernel (A/B switch)
         uint64_t             index_bytes{0}, dir_bytes{0}, total_blocks{0}, total_postings{0};
         DevBuf               d_index, d_blk_last, d_blk_off, d_terms, d_tile_first, d_masked;
         bool                 have_masked{false};
@@ -145,8 +132,7 @@ struct trn_ctx {
         uint32_t last_nq{0}, last_k{0}, last_launches{0};
         uint64_t last_postings{0}, last_bytes{0};
         float    last_ms{0};
-        // path (TRN_ROUTE_*) of every query of the last exec_device_impl call / of the last whole batch (trn_debug_last_routes)
-        std::vector<uint8_t> call_routes, last_routes;
+        std::vector<uint8_t> last_routes; // TRN_ROUTE_* of every query of the last batch (trn_debug_last_routes)
 };
 
 #define CK(call)                                                                                                                                               \
@@ -162,596 +148,20 @@ static inline double now_ms() {
         return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-// flat_tree_masks: a leaf is decoded in the masked pass when at most this share of its blocks is expected to survive its mask (TRN_TREE_MASK_NEED)
-static double g_tree_mask_need = 0.6;
-
 static int fail(trn_ctx *c, int code, const std::string &m) {
         c->err = m;
         return code;
 }
 
-// =================================================================================================== plan compiler
-namespace {
-struct Range {
-        uint32_t lo{1}, hi{0}; // inclusive docIDs; empty when lo > hi
-        bool     empty() const {
-                return lo > hi;
-        }
-};
-
-// every node has at most one parent: a plan is a TREE (a node shared by several parents would make the recursive passes — cost, range,
-// bound, truth tables — revisit it once per path, exponentially often in a hostile plan)
-static bool plan_is_tree(const trn_qnode *n, uint32_t nn, uint32_t root) {
-        std::vector<uint8_t> seen(nn, 0);
-        if (root < nn)
-                seen[root] = 1;
-        for (uint32_t i = 0; i < nn; ++i) {
-                if (n[i].kind == TRN_NODE_TERM)
-                        continue;
-                for (uint32_t k = 0; k < n[i].nchildren; ++k) {
-                        const uint32_t c = uint32_t(n[i].first_child) + k;
-                        if (c >= nn || seen[c])
-                                return false;
-                        seen[c] = 1;
-                }
-        }
-        return true;
+// the planner's configuration as a new context starts with it: the knobs from the environment, the limits of this build's kernels
+static PlanConfig initial_plan_config() {
+        PlanConfig pc            = plan_config_from_env();
+        pc.score_flat_max_leaves = score_flat_max_leaves();
+        pc.docs_stage_bytes      = exec_docs_stage_bytes();
+        pc.cand_smem_bytes[0]    = exec_docs_cand_smem_bytes(false);
+        pc.cand_smem_bytes[1]    = exec_docs_cand_smem_bytes(true);
+        return pc;
 }
-
-// children follow their parents in the node array (checked by validate()), so one forward pass yields every node's depth; the
-// compiler and the truth-table builder recurse once per level
-static bool plan_depth_ok(const trn_qnode *n, uint32_t nn) {
-        std::vector<uint8_t> depth(nn, 0);
-        for (uint32_t i = 0; i < nn; ++i) {
-                if (n[i].kind == TRN_NODE_TERM)
-                        continue;
-                if (depth[i] >= 64)
-                        return false;
-                for (uint32_t k = 0; k < n[i].nchildren; ++k) {
-                        const uint32_t c = uint32_t(n[i].first_child) + k;
-                        if (c > i && c < nn)
-                                depth[c] = uint8_t(std::max<int>(depth[c], depth[i] + 1));
-                }
-        }
-        return true;
-}
-
-struct Compiler {
-        const trn_qnode *           n;
-        uint32_t                    nn;
-        const std::vector<DevTerm> &terms;
-        bool                        scored;
-        uint32_t                    root;
-        std::vector<DevStep> &      steps;
-        uint32_t                    next_slot{0};
-        uint64_t                    postings{0}, bytes{0};
-        struct Deferred {
-                uint32_t              term;
-                double                idf;
-                std::vector<uint8_t> cond;
-                int                   phrase{-1}; // >= 0: node index of a phrase (its position check is repeated under the condition's mask)
-        };
-        std::vector<Deferred> deferred;
-        std::string           err;
-        bool                  reference_quirks{true};
-        bool                  unsupported{false};
-        bool                  allow_phrase{false}; // the caller's kernels execute OP_PHRASE (GOOGLE codec: inline hits)
-        bool                  has_phrase{false};
-        std::vector<uint32_t> leaf_nodes;          // node index of every OP_LEAF step, in program order (flat_tree_masks)
-
-        Compiler(const trn_qnode *nodes, uint32_t cnt, const std::vector<DevTerm> &t, bool sc, uint32_t r, std::vector<DevStep> &s)
-            : n{nodes}, nn{cnt}, terms{t}, scored{sc}, root{r}, steps{s} {
-        }
-
-        // Slots: in DocumentsOnly plans a child's bitmap is dead once it has been combined into its parent, so its slot is handed out
-        // again (scored plans keep every slot: the deferred scoring pass reads branch bitmaps at the end).  Fewer live slots = less
-        // shared memory per worker = more resident warps (with one slot per node the 8-term trees left few warps resident per SM).
-        std::vector<uint32_t> free_slots;
-        int alloc_slot() {
-                if (!scored && !free_slots.empty()) {
-                        const auto it = std::min_element(free_slots.begin(), free_slots.end());
-                        const int  v  = int(*it);
-                        free_slots.erase(it);
-                        return v;
-                }
-                if (next_slot >= 14) {
-                        err = "query needs more than 14 docset slots";
-                        return -1;
-                }
-                return int(next_slot++);
-        }
-        void release_slot(uint32_t s) {
-                if (!scored)
-                        free_slots.push_back(s);
-        }
-
-        bool is_leaf(uint32_t i) const {
-                return n[i].kind == TRN_NODE_TERM;
-        }
-        bool is_phrase(uint32_t i) const {
-                return n[i].kind == TRN_NODE_PHRASE;
-        }
-        // the conjunction of a phrase's distinct terms into slot `tmp` (rarest first), then the position check in place (phrase.cuh)
-        void phrase_steps(uint32_t i, uint32_t tmp, bool score) {
-                const auto &          X = n[i];
-                std::vector<uint32_t> t(X.nchildren);
-                double                idfsum{0};
-                bool                  anyEmpty{false};
-                for (uint32_t j = 0; j < X.nchildren; ++j) {
-                        t[j] = n[X.first_child + j].term;
-                        idfsum += n[X.first_child + j].weight;
-                        anyEmpty |= t[j] == kEmptyTerm || terms[t[j]].documents == 0;
-                }
-                if (anyEmpty) { // a phrase with an unknown term matches nothing
-                        push(OP_CLEAR, 0, tmp, 0, 0, 0, 0);
-                        return;
-                }
-                std::vector<uint32_t> distinct(t);
-                std::sort(distinct.begin(), distinct.end());
-                distinct.erase(std::unique(distinct.begin(), distinct.end()), distinct.end());
-                std::stable_sort(distinct.begin(), distinct.end(), [&](uint32_t a, uint32_t b) { return terms[a].documents < terms[b].documents; });
-                bool first{true};
-                for (auto term : distinct) {
-                        postings += terms[term].documents;
-                        bytes += terms[term].chunk_len;
-                        push(OP_LEAF, first ? M_SET : M_AND, tmp, 0, 0, term, 0);
-                        first = false;
-                }
-                push(OP_PHRASE, uint8_t(X.nchildren), tmp, 0, score ? F_SCORE : 0, 0, idfsum);
-                for (uint32_t j = 0; j < X.nchildren; j += 4) { // four term ids per operand step, in phrase order
-                        DevStep a;
-                        std::memset(&a, 0, sizeof(a));
-                        a.op   = OP_ARG;
-                        a.term = t[j];
-                        a.pad2 = j + 1 < X.nchildren ? t[j + 1] : 0u;
-                        const uint64_t hi = uint64_t(j + 2 < X.nchildren ? t[j + 2] : 0u) | (uint64_t(j + 3 < X.nchildren ? t[j + 3] : 0u) << 32);
-                        std::memcpy(&a.idf, &hi, 8);
-                        steps.push_back(a);
-                }
-        }
-        // a phrase operand combined into dst with `mode` (== leaf() for a term); scores score(matchCnt, sum idf) where it holds
-        bool phrase_leaf(uint32_t i, uint8_t mode, uint32_t dst, bool scoring, const std::vector<uint8_t> &cond, uint8_t extraFlags) {
-                const bool wantScore = scored && scoring;
-                if (mode == M_NONE && !wantScore)
-                        return true; // nothing to do in this pass
-                const bool immediate = wantScore && cond.empty();
-                if (wantScore && !immediate)
-                        deferred.push_back({0, 0.0, cond, int(i)});
-                if (mode == M_NONE && !immediate)
-                        return true; // the deferred pass does it all
-                const int tmp = alloc_slot();
-                if (tmp < 0)
-                        return false;
-                phrase_steps(i, uint32_t(tmp), immediate);
-                if (mode != M_NONE)
-                        push(OP_SLOT, mode, dst, uint32_t(tmp), extraFlags, 0, 0);
-                release_slot(uint32_t(tmp));
-                return true;
-        }
-        uint32_t df(uint32_t i) const {
-                const auto t = n[i].term;
-                return t == kEmptyTerm ? 0u : terms[t].documents;
-        }
-        void push(uint8_t op, uint8_t mode, uint32_t dst, uint32_t src, uint8_t flags, uint32_t term, double idf) {
-                DevStep s;
-                std::memset(&s, 0, sizeof(s));
-                s.op    = op;
-                s.mode  = mode;
-                s.dst   = uint8_t(dst);
-                s.src   = uint8_t(src);
-                s.flags = flags;
-                s.term  = term;
-                s.idf   = idf;
-                steps.push_back(s);
-        }
-        void account(uint32_t i) {
-                const auto t = n[i].term;
-                if (t != kEmptyTerm) {
-                        postings += terms[t].documents;
-                        bytes += terms[t].chunk_len;
-                }
-        }
-        // leaf combined into dst with `mode`; scoring per the structural rules
-        void leaf(uint32_t i, uint8_t mode, uint32_t dst, bool scoring, const std::vector<uint8_t> &cond, uint8_t extraFlags) {
-                account(i);
-                uint8_t flags = extraFlags;
-                if (scored && scoring) {
-                        if (cond.empty())
-                                flags |= F_SCORE;
-                        else
-                                deferred.push_back({n[i].term, n[i].weight, cond});
-                }
-                if (mode == M_NONE && !(flags & F_SCORE))
-                        return; // nothing to do in this pass
-                leaf_nodes.push_back(i);
-                push(OP_LEAF, mode, dst, 0, flags, n[i].term, n[i].weight);
-        }
-
-        // compiles internal node i into its own slot; returns the slot
-        int node(uint32_t i, bool scoring, const std::vector<uint8_t> &cond) {
-                const int sAlloc = alloc_slot();
-                if (sAlloc < 0)
-                        return -1;
-                const uint32_t s    = uint32_t(sAlloc);
-                const auto &   X    = n[i];
-                const bool     isRoot = i == root;
-                if (X.nchildren == 0 || uint32_t(X.first_child) + X.nchildren > nn) {
-                        err = "operator node without (valid) children";
-                        return -1;
-                }
-                std::vector<uint32_t> kids(X.nchildren);
-                for (uint32_t c = 0; c < X.nchildren; ++c)
-                        kids[c] = X.first_child + c;
-                auto child_cond = [&](uint32_t slotOfChild) {
-                        auto v = cond;
-                        v.push_back(uint8_t(slotOfChild));
-                        return v;
-                };
-                switch (X.kind) {
-                        case TRN_NODE_AND: {
-                                // leaves first, rarest first (== prepare_tree's df sort exec.cpp:154-170 and reorder_execnodes :216)
-                                std::stable_sort(kids.begin(), kids.end(), [&](uint32_t a, uint32_t b) {
-                                        const bool la = is_leaf(a), lb = is_leaf(b);
-                                        if (la != lb)
-                                                return la;
-                                        if (la)
-                                                return df(a) < df(b);
-                                        return false;
-                                });
-                                bool first{true};
-                                for (auto c : kids) {
-                                        const uint8_t fl = isRoot ? F_BREAK_IF_EMPTY : 0;
-                                        if (is_leaf(c))
-                                                leaf(c, first ? M_SET : M_AND, s, scoring, cond, fl);
-                                        else if (is_phrase(c)) {
-                                                if (!phrase_leaf(c, first ? M_SET : M_AND, s, scoring, cond, fl))
-                                                        return -1;
-                                        } else {
-                                                const int cs = node(c, scoring, cond);
-                                                if (cs < 0)
-                                                        return -1;
-                                                push(OP_SLOT, first ? M_SET : M_AND, s, uint32_t(cs), fl, 0, 0);
-                                                release_slot(uint32_t(cs));
-                                        }
-                                        first = false;
-                                }
-                        } break;
-                        case TRN_NODE_OR: {
-                                push(OP_CLEAR, 0, s, 0, 0, 0, 0);
-                                for (auto c : kids) {
-                                        if (is_leaf(c))
-                                                leaf(c, M_OR, s, scoring, cond, 0);
-                                        else if (is_phrase(c)) {
-                                                if (!phrase_leaf(c, M_OR, s, scoring, cond, 0))
-                                                        return -1;
-                                        } else {
-                                                // a non-leaf child of a disjunction contributes its score only for documents it matches itself
-                                                // (Disjunction scorer sums children positioned on the doc, docset_iterators_scorers.cpp)
-                                                const uint32_t willBe = next_slot;
-                                                const int      cs     = node(c, scoring, child_cond(willBe));
-                                                if (cs < 0)
-                                                        return -1;
-                                                push(OP_SLOT, M_OR, s, uint32_t(cs), 0, 0, 0);
-                                                release_slot(uint32_t(cs));
-                                        }
-                                }
-                        } break;
-                        case TRN_NODE_NOT:
-                        case TRN_NODE_OPTIONAL: {
-                                if (X.nchildren != 2) {
-                                        err = "NOT / OPTIONAL need exactly two children";
-                                        return -1;
-                                }
-                                const uint8_t fl = isRoot ? F_BREAK_IF_EMPTY : 0;
-                                if (is_leaf(kids[0]))
-                                        leaf(kids[0], M_SET, s, scoring, cond, fl);
-                                else if (is_phrase(kids[0])) {
-                                        if (!phrase_leaf(kids[0], M_SET, s, scoring, cond, fl))
-                                                return -1;
-                                } else {
-                                        const int cs = node(kids[0], scoring, cond);
-                                        if (cs < 0)
-                                                return -1;
-                                        push(OP_SLOT, M_SET, s, uint32_t(cs), fl, 0, 0);
-                                        release_slot(uint32_t(cs));
-                                }
-                                if (X.kind == TRN_NODE_NOT) {
-                                        // Filter: excluded side never scores (docset_iterators_scorers.cpp Filter -> req only)
-                                        if (is_leaf(kids[1]))
-                                                leaf(kids[1], M_ANDNOT, s, false, cond, 0);
-                                        else if (is_phrase(kids[1])) {
-                                                if (!phrase_leaf(kids[1], M_ANDNOT, s, false, cond, 0))
-                                                        return -1;
-                                        } else {
-                                                const int cs = node(kids[1], false, cond);
-                                                if (cs < 0)
-                                                        return -1;
-                                                push(OP_SLOT, M_ANDNOT, s, uint32_t(cs), 0, 0, 0);
-                                                release_slot(uint32_t(cs));
-                                        }
-                                } else if (scored && scoring) {
-                                        // Optional: main drives; opt only adds its score when it is on the document
-                                        if (is_leaf(kids[1]))
-                                                leaf(kids[1], M_NONE, s, true, cond, 0);
-                                        else if (is_phrase(kids[1])) {
-                                                if (!phrase_leaf(kids[1], M_NONE, s, true, cond, 0))
-                                                        return -1;
-                                        } else {
-                                                const uint32_t willBe = next_slot;
-                                                if (node(kids[1], true, child_cond(willBe)) < 0)
-                                                        return -1;
-                                        }
-                                } else {
-                                        // docs-only: the optional side cannot change the match set, but it is still "touched" by the reference
-                                        // (Optional::next advances opt lazily); we do not read it at all.
-                                }
-                        } break;
-                        case TRN_NODE_SOME: {
-                                // DisjunctionSome (docset_iterators.cpp:679-811): every child is evaluated into a bitmap of its own and added to a
-                                // bit-sliced saturating counter (one bitmap per counter bit); the node matches where the counter reaches `min`.
-                                // A child scores only where it matches AND the node matches (Wrapper::iterator_score sums the lead list).
-                                const uint32_t m = X.term;
-                                if (m == 0 || m > 15) {
-                                        err = "SOME: min-should-match must be in 1..15";
-                                        return -1;
-                                }
-                                uint32_t k = 1;
-                                while (((1u << k) - 1u) < m)
-                                        ++k;
-                                if (next_slot + k + 1 > 14) {
-                                        err = "query needs more than 14 docset slots";
-                                        return -1;
-                                }
-                                const uint32_t p0 = next_slot;
-                                next_slot += k;
-                                const uint32_t t = next_slot++; // shared by the leaf children
-                                for (uint32_t j = 0; j < k; ++j)
-                                        push(OP_CLEAR, 0, p0 + j, 0, 0, 0, 0);
-                                for (auto c : kids) {
-                                        uint32_t src;
-                                        if (is_leaf(c)) {
-                                                leaf(c, M_SET, t, scoring, child_cond(s), 0);
-                                                src = t;
-                                        } else if (is_phrase(c)) {
-                                                if (!phrase_leaf(c, M_SET, t, scoring, child_cond(s), 0))
-                                                        return -1;
-                                                src = t;
-                                        } else {
-                                                auto cc = child_cond(s);
-                                                cc.push_back(uint8_t(next_slot)); // the child's own slot
-                                                const int cs = node(c, scoring, cc);
-                                                if (cs < 0)
-                                                        return -1;
-                                                src = uint32_t(cs);
-                                        }
-                                        push(OP_COUNT_ADD, uint8_t(k), p0, src, 0, 0, 0);
-                                        if (src != t)
-                                                release_slot(src);
-                                }
-                                push(OP_COUNT_GE, uint8_t(k), s, p0, 0, m, 0);
-                                for (uint32_t j = 0; j < k; ++j)
-                                        release_slot(p0 + j);
-                                release_slot(t);
-                        } break;
-                        default:
-                                err = "unknown node kind";
-                                return -1;
-                }
-                return int(s);
-        }
-
-        Range range(uint32_t i) const {
-                const auto &X = n[i];
-                Range       r;
-                if (X.kind == TRN_NODE_TERM) {
-                        if (X.term != kEmptyTerm && terms[X.term].documents) {
-                                r.lo = terms[X.term].first_doc;
-                                r.hi = terms[X.term].last_doc;
-                        }
-                        return r;
-                }
-                if (X.kind == TRN_NODE_NOT || X.kind == TRN_NODE_OPTIONAL)
-                        return range(X.first_child);
-                const bool conj = X.kind == TRN_NODE_AND || X.kind == TRN_NODE_PHRASE; // a phrase needs all of its terms
-                bool       first{true};
-                for (uint32_t c = 0; c < X.nchildren; ++c) {
-                        const Range cr = range(X.first_child + c);
-                        if (conj) {
-                                if (cr.empty())
-                                        return Range{};
-                                if (first)
-                                        r = cr;
-                                else {
-                                        r.lo = std::max(r.lo, cr.lo);
-                                        r.hi = std::min(r.hi, cr.hi);
-                                        if (r.empty())
-                                                return Range{};
-                                }
-                                first = false;
-                        } else {
-                                if (cr.empty())
-                                        continue;
-                                if (first)
-                                        r = cr;
-                                else {
-                                        r.lo = std::min(r.lo, cr.lo);
-                                        r.hi = std::max(r.hi, cr.hi);
-                                }
-                                first = false;
-                        }
-                }
-                return r;
-        }
-
-        uint64_t bound(uint32_t i) const {
-                const auto &X = n[i];
-                if (X.kind == TRN_NODE_TERM)
-                        return df(i);
-                if (X.kind == TRN_NODE_NOT || X.kind == TRN_NODE_OPTIONAL)
-                        return bound(X.first_child);
-                const bool conj = X.kind == TRN_NODE_AND || X.kind == TRN_NODE_PHRASE;
-                uint64_t   b    = conj ? ~0ull : 0ull;
-                for (uint32_t c = 0; c < X.nchildren; ++c) {
-                        const uint64_t cb = bound(X.first_child + c);
-                        b                 = conj ? std::min(b, cb) : b + cb;
-                }
-                return b;
-        }
-
-        bool validate() {
-                if (root >= nn) {
-                        err = "root out of range";
-                        return false;
-                }
-                if (!plan_depth_ok(n, nn)) {
-                        err = "query tree deeper than 64 levels";
-                        return false;
-                }
-                for (uint32_t i = 0; i < nn; ++i) {
-                        if (n[i].kind == TRN_NODE_TERM) {
-                                if (n[i].term != kEmptyTerm && n[i].term >= terms.size()) {
-                                        err = "term id out of range";
-                                        return false;
-                                }
-                        } else if (n[i].kind == TRN_NODE_PHRASE) {
-                                if (!allow_phrase) {
-                                        err         = "phrase nodes need the positions (materialize_hits): a LUCENE source executes them once its hits.data has been uploaded (trn_upload_hits)";
-                                        unsupported = true;
-                                        return false;
-                                }
-                                if (n[i].nchildren < 2 || n[i].nchildren > 16 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
-                                        err = "a phrase holds 2..16 terms behind it in the node array";
-                                        return false;
-                                }
-                                for (uint32_t k = 0; k < n[i].nchildren; ++k)
-                                        if (n[n[i].first_child + k].kind != TRN_NODE_TERM) {
-                                                err = "the children of a phrase are terms";
-                                                return false;
-                                        }
-                                has_phrase = true;
-                        } else if (n[i].kind > TRN_NODE_PHRASE) {
-                                err = "unknown node kind";
-                                return false;
-                        } else {
-                                // children must come after their parent (guarantees an acyclic tree)
-                                if (n[i].nchildren == 0 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
-                                        err = "children must follow their parent in the node array";
-                                        return false;
-                                }
-                        }
-                }
-                if (!plan_is_tree(n, nn, root)) {
-                        err = "a node is referenced by more than one parent (a plan is a tree)";
-                        return false;
-                }
-                return true;
-        }
-
-        // == DocsSetIterators::cost() (docset_iterators.cpp:10-64); a conjunction's cost is its lead's, which the reference's
-        // reordering passes make the cheapest operand
-        uint64_t cost(uint32_t i) const {
-                const auto &X = n[i];
-                if (X.kind == TRN_NODE_TERM)
-                        return df(i);
-                if (X.kind == TRN_NODE_NOT || X.kind == TRN_NODE_OPTIONAL)
-                        return cost(X.first_child);
-                if (X.kind == TRN_NODE_PHRASE) // docset_iterators.cpp:50-55: cost(its[0]) + UINT32_MAX + UINT16_MAX * size
-                        return cost(X.first_child) + 0xffffffffull + 0xffffull * X.nchildren;
-                if (X.kind == TRN_NODE_SOME) { // DisjunctionSome::cost_: the (size - min + 1) cheapest children (docset_iterators.cpp:733-742)
-                        std::vector<uint64_t> cs;
-                        for (uint32_t k = 0; k < X.nchildren; ++k)
-                                cs.push_back(cost(X.first_child + k));
-                        std::sort(cs.begin(), cs.end());
-                        const uint32_t keep = X.nchildren >= X.term ? X.nchildren - X.term + 1u : 0u;
-                        uint64_t       c{0};
-                        for (uint32_t k = 0; k < keep && k < cs.size(); ++k)
-                                c += cs[k];
-                        return c;
-                }
-                uint64_t c = X.kind == TRN_NODE_AND ? ~0ull : 0ull;
-                for (uint32_t k = 0; k < X.nchildren; ++k) {
-                        const uint64_t cc = cost(X.first_child + k);
-                        c                 = X.kind == TRN_NODE_AND ? std::min(c, cc) : c + cc;
-                }
-                return c;
-        }
-
-        // REFERENCE QUIRK, mirrored for drop-in parity: build_span() (exec.cpp:488-501) turns a root Filter whose excluded side is not
-        // costlier than its required side into FilteredDocsSetSpan(build_span(req), excl).  When req is a disjunction the inner span is
-        // DocsSetSpanForDisjunctions[WithThreshold], whose process() ignores its `min` argument (docset_spans.cpp:98-111,681-694): the
-        // excluded documents the outer span stepped over are emitted by the next call anyway, so the exclusion has no effect and the
-        // reference returns the plain disjunction.  The same holds through a chain of such root filters.
-        void apply_reference_root_filter_quirk() {
-                uint32_t cur = root;
-                bool     traversed{false};
-                while (n[cur].kind == TRN_NODE_NOT && n[cur].nchildren == 2 && cost(n[cur].first_child + 1u) <= cost(n[cur].first_child)) {
-                        cur       = n[cur].first_child;
-                        traversed = true;
-                }
-                if (traversed && n[cur].kind == TRN_NODE_OR)
-                        root = cur;
-        }
-
-        // returns root slot or -1
-        int run() {
-                if (!validate())
-                        return -1;
-                if (reference_quirks)
-                        apply_reference_root_filter_quirk();
-                int rs;
-                if (is_leaf(root)) {
-                        rs = int(next_slot++);
-                        leaf(root, M_SET, uint32_t(rs), true, {}, 0);
-                } else if (is_phrase(root)) {
-                        rs = int(next_slot++);
-                        if (!phrase_leaf(root, M_SET, uint32_t(rs), true, {}, 0))
-                                return -1;
-                } else
-                        rs = node(root, true, {});
-                if (rs < 0)
-                        return -1;
-                // second pass for leaves whose contribution is conditional on a disjunction branch matching
-                for (auto &d : deferred) {
-                        uint32_t mask = d.cond[0];
-                        if (d.cond.size() > 1) {
-                                if (next_slot >= 14) {
-                                        err = "query needs more than 14 docset slots";
-                                        return -1;
-                                }
-                                mask = next_slot++;
-                                push(OP_SLOT, M_SET, mask, d.cond[0], 0, 0, 0);
-                                for (size_t j = 1; j < d.cond.size(); ++j)
-                                        push(OP_SLOT, M_AND, mask, d.cond[j], 0, 0, 0);
-                        }
-                        if (d.phrase >= 0) { // the phrase again, restricted to the condition's documents, scoring this time
-                                if (next_slot >= 14) {
-                                        err = "query needs more than 14 docset slots";
-                                        return -1;
-                                }
-                                const uint32_t tmp = next_slot++;
-                                // (phrase_steps starts with SET/CLEAR into tmp; the mask narrows the candidates before the position check)
-                                const size_t at = steps.size();
-                                phrase_steps(uint32_t(d.phrase), tmp, true);
-                                // insert [SLOT AND tmp, mask] in front of the OP_PHRASE step
-                                for (size_t z = at; z < steps.size(); ++z)
-                                        if (steps[z].op == OP_PHRASE) {
-                                                DevStep a;
-                                                std::memset(&a, 0, sizeof(a));
-                                                a.op   = OP_SLOT;
-                                                a.mode = M_AND;
-                                                a.dst  = uint8_t(tmp);
-                                                a.src  = uint8_t(mask);
-                                                steps.insert(steps.begin() + z, a);
-                                                break;
-                                        }
-                                continue;
-                        }
-                        push(OP_LEAFSCORE, M_NONE, 0, mask, 0, d.term, d.idf);
-                }
-                return rs;
-        }
-};
-} // namespace
 
 // =================================================================================================== C ABI: lifecycle
 extern "C" int trn_create(int device, trn_ctx **out) {
@@ -771,44 +181,9 @@ extern "C" int trn_create(int device, trn_ctx **out) {
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, device));
         c->num_sms = prop.multiProcessorCount;
-        if (const char *e = getenv("TRN_TILE_SHIFT")) { // directory granularity == tile of the scored kernel (experiments)
-                const int v = atoi(e);
-                if (v >= 12 && v <= 14)
-                        c->tile_shift = uint32_t(v);
-        }
-        if (const char *e = getenv("TRN_CAND_COST"))
-                c->cand_cost = std::max(0, atoi(e));
-        if (const char *e = getenv("TRN_DOCS_SHIFT")) {
-                const int v = atoi(e);
-                if (v >= 13 && v <= 17)
-                        c->docs_shift = uint32_t(v);
-        }
-        if (const char *e = getenv("TRN_TREE_SHIFT")) {
-                const int v = atoi(e);
-                if (v == 0 || (v >= 10 && v <= 14))
-                        c->tree_shift = uint32_t(v);
-        }
-        if (const char *e = getenv("TRN_TREE_MASKS"))
-                c->tree_masks = atoi(e) != 0;
-        if (const char *e = getenv("TRN_TREE_MASK_NEED")) {
-                const double v = atof(e);
-                if (v > 0.0 && v <= 1.0)
-                        g_tree_mask_need = v;
-        }
-        if (const char *e = getenv("TRN_RUN_TILES")) {
-                const int v = atoi(e);
-                if (v >= 1 && v <= 4096)
-                        c->run_tiles = uint32_t(v);
-        }
-        if (const char *e = getenv("TRN_FLAT_SCORED"))
-                c->flat_scored = atoi(e) != 0;
+        c->pc      = initial_plan_config();
         if (const char *e = getenv("TRN_SF_THREADS"))
                 c->flat_threads = atoi(e);
-        if (const char *e = getenv("TRN_SCORED_SHIFT")) {
-                const int v = atoi(e);
-                if (v == 13 || v == 14)
-                        c->scored_shift = uint32_t(v);
-        }
         if (const char *e = getenv("TRN_PIPELINE_CHUNKS")) {
                 const int v = atoi(e);
                 if (v >= 1 && v <= 16)
@@ -886,55 +261,37 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         if (nbytes >= (1ull << 32))
                 return fail(c, TRN_ERR_ARG, "index larger than 4 GiB: one IndexSource is limited to range32_t offsets (codecs.h:17-55); shard it");
         CK(cudaSetDevice(c->device));
-        BlockDirectory dir;
+        BlockDirectory       dir;
+        std::vector<DevTerm> ht;
         try {
-                std::vector<term_index_ctx> t(nterms);
-                for (uint32_t i = 0; i < nterms; ++i) {
-                        t[i].documents = terms[i].documents;
-                        t[i].offset    = terms[i].chunk_off;
-                        t[i].size      = terms[i].chunk_len;
-                }
                 const int threads = int(std::max(1u, std::min(64u, std::thread::hardware_concurrency())));
-                build_block_directory(codec == TRN_CODEC_GOOGLE ? Codec::Google : Codec::Lucene, index, nbytes, t.data(), nterms, threads, dir);
+                build_directory(codec, index, nbytes, terms, nterms, threads, dir);
         } catch (const std::bad_alloc &) {
                 return fail(c, TRN_ERR_CAPACITY, "trn_upload_index: out of host memory while building the block directory");
         } catch (const std::exception &e) {
                 return fail(c, TRN_ERR_FORMAT, e.what());
         }
-        if (max_docid == 0) // not recorded (e.g. a segment directory): the largest docID any postings list holds
-                for (uint32_t i = 0; i < nterms; ++i)
-                        if (dir.terms[i].nblocks)
-                                max_docid = std::max(max_docid, dir.terms[i].last_doc);
-        c->codec      = codec;
-        c->block_docs = dir.block_docs;
-        c->nterms     = nterms;
-        c->max_docid  = max_docid;
-        const uint32_t W = 1u << c->tile_shift;
-        c->ntiles     = uint32_t((uint64_t(max_docid) + 1 + W - 1) >> c->tile_shift);
         try {
-                c->h_terms.resize(nterms);
+                ht = dev_terms(dir, terms, nterms);
         } catch (const std::bad_alloc &) {
                 return fail(c, TRN_ERR_CAPACITY, "trn_upload_index: out of host memory");
         }
-        c->have_index     = false; // until the new index is completely in place
-        c->min_docid      = 0xffffffffu;
+        uint32_t min_docid;
+        docid_span(ht, min_docid, max_docid);
+        c->have_index   = false; // until the new index is completely in place
+        c->pc.codec     = codec;
+        c->pc.min_docid = min_docid;
+        c->pc.max_docid = max_docid;
+        c->block_docs   = dir.block_docs;
+        c->nterms       = nterms;
+        const uint32_t W = 1u << c->pc.tile_shift;
+        c->ntiles       = uint32_t((uint64_t(max_docid) + 1 + W - 1) >> c->pc.tile_shift);
+        c->h_terms      = std::move(ht);
         c->total_blocks   = 0;
         c->total_postings = 0;
-        for (uint32_t i = 0; i < nterms; ++i) {
-                auto &d     = c->h_terms[i];
-                d.documents = dir.terms[i].documents;
-                d.dir_begin = dir.terms[i].dir_begin;
-                d.nblocks   = dir.terms[i].nblocks;
-                d.first_doc = dir.terms[i].first_doc;
-                d.last_doc  = dir.terms[i].last_doc;
-                d.chunk_len = terms[i].chunk_len;
-                d.tf_begin  = dir.terms[i].tf_begin;
-                d.tf_base   = dir.terms[i].tf_base;
-                d.tf_shift  = dir.terms[i].tf_shift;
+        for (const auto &d : c->h_terms) {
                 c->total_blocks += d.nblocks;
                 c->total_postings += d.documents;
-                if (d.nblocks)
-                        c->min_docid = std::min(c->min_docid, d.first_doc);
                 if (d.nblocks && d.last_doc > max_docid)
                         return fail(c, TRN_ERR_ARG, "a term holds a docID above max_docid");
         }
@@ -986,7 +343,7 @@ extern "C" int trn_upload_hits(trn_ctx *c, const uint8_t *index, uint64_t nbytes
                 return c ? fail(c, TRN_ERR_ARG, "trn_upload_hits: bad arguments") : TRN_ERR_ARG;
         if (!c->have_index)
                 return fail(c, TRN_ERR_STATE, "no index uploaded");
-        if (c->codec != TRN_CODEC_LUCENE)
+        if (c->pc.codec != TRN_CODEC_LUCENE)
                 return fail(c, TRN_ERR_ARG, "trn_upload_hits: the GOOGLE codec keeps its hits inline (nothing to upload)");
         if (nbytes != c->index_bytes || c->h_termctx.size() != c->nterms)
                 return fail(c, TRN_ERR_ARG, "trn_upload_hits: not the index this context holds");
@@ -1037,12 +394,12 @@ extern "C" int trn_set_masked_documents(trn_ctx *c, const uint32_t *docids, uint
                 return TRN_OK;
         }
         // one bit per docID, padded so that every (largest) tile can read its whole word range
-        const uint64_t        span  = ((uint64_t(c->max_docid) >> 17) + 2) << 17;
+        const uint64_t        span  = ((uint64_t(c->pc.max_docid) >> 17) + 2) << 17;
         std::vector<uint32_t> words(span / 32, 0u);
         for (uint64_t i = 0; i < n; ++i) {
                 if (docids[i] == 0)
                         return fail(c, TRN_ERR_ARG, "masked docID 0 is not a document");
-                if (docids[i] > c->max_docid)
+                if (docids[i] > c->pc.max_docid)
                         continue; // a newer source may mask documents this source never held
                 words[docids[i] >> 5] |= 1u << (docids[i] & 31u);
         }
@@ -1058,10 +415,10 @@ extern "C" int trn_index_info_get(trn_ctx *c, trn_index_info *o) {
                 return TRN_ERR_ARG;
         if (!c->have_index)
                 return fail(c, TRN_ERR_STATE, "no index uploaded");
-        o->codec           = c->codec;
+        o->codec           = c->pc.codec;
         o->nterms          = c->nterms;
-        o->max_docid       = c->max_docid;
-        o->tile_docs       = 1u << c->tile_shift;
+        o->max_docid       = c->pc.max_docid;
+        o->tile_docs       = 1u << c->pc.tile_shift;
         o->ntiles          = c->ntiles;
         o->block_docs      = c->block_docs;
         o->index_bytes     = c->index_bytes;
@@ -1081,10 +438,10 @@ static DevIndex dev_index(trn_ctx *c) {
         ix.masked     = c->have_masked ? c->d_masked.as<uint32_t>() : nullptr;
         ix.nterms     = c->nterms;
         ix.ntiles     = c->ntiles;
-        ix.tile_shift = c->tile_shift;
-        ix.max_docid  = c->max_docid;
+        ix.tile_shift = c->pc.tile_shift;
+        ix.max_docid  = c->pc.max_docid;
         ix.block_docs = c->block_docs;
-        ix.codec      = c->codec;
+        ix.codec      = c->pc.codec;
         ix.hits       = c->have_hits ? c->d_hits.as<uint8_t>() : nullptr;
         ix.hit_base   = c->have_hits ? c->d_hit_base.as<uint32_t>() : nullptr;
         ix.hblk_off   = c->have_hits ? c->d_hblk_off.as<uint32_t>() : nullptr;
@@ -1092,608 +449,11 @@ static DevIndex dev_index(trn_ctx *c) {
         return ix;
 }
 
-// Truth vector of a query subtree over its (<= 8) distinct terms: bit `a` (0..255) = value of the node when exactly the terms whose
-// bit is set in `a` are present (bit j of `a` = term tv[j]).  Bitwise evaluation: one 256-bit operation per node.
-struct TruthVec {
-        uint64_t w[4];
-};
-static TruthVec truth_vector(const trn_qnode *nodes, uint32_t i, const uint32_t *tv, uint32_t n) {
-        static const uint64_t kPat[6] = {0xaaaaaaaaaaaaaaaaull, 0xccccccccccccccccull, 0xf0f0f0f0f0f0f0f0ull, 0xff00ff00ff00ff00ull, 0xffff0000ffff0000ull, 0xffffffff00000000ull};
-        const auto &X = nodes[i];
-        TruthVec    v{{0, 0, 0, 0}};
-        if (X.kind == TRN_NODE_TERM) {
-                for (uint32_t j = 0; j < n; ++j)
-                        if (tv[j] == X.term) {
-                                for (int q = 0; q < 4; ++q)
-                                        v.w[q] = j < 6 ? kPat[j] : (j == 6 ? ((q & 1) ? ~0ull : 0ull) : ((q & 2) ? ~0ull : 0ull));
-                                break;
-                        }
-                return v;
-        }
-        const uint32_t f = X.first_child;
-        if (X.kind == TRN_NODE_SOME) {
-                const uint32_t        nk = X.nchildren; // all of them (<= 255)
-                std::vector<TruthVec> kids(nk);
-                for (uint32_t k = 0; k < nk; ++k)
-                        kids[k] = truth_vector(nodes, f + k, tv, n);
-                for (uint32_t a = 0; a < 256; ++a) {
-                        uint32_t cnt{0};
-                        for (uint32_t k = 0; k < nk; ++k)
-                                cnt += uint32_t((kids[k].w[a >> 6] >> (a & 63u)) & 1ull);
-                        if (cnt >= X.term)
-                                v.w[a >> 6] |= 1ull << (a & 63u);
-                }
-                return v;
-        }
-        v = truth_vector(nodes, f, tv, n);
-        for (uint32_t k = 1; k < X.nchildren; ++k) {
-                const TruthVec w = truth_vector(nodes, f + k, tv, n);
-                for (int q = 0; q < 4; ++q) {
-                        if (X.kind == TRN_NODE_AND) v.w[q] &= w.w[q];
-                        else if (X.kind == TRN_NODE_OR) v.w[q] |= w.w[q];
-                        else if (X.kind == TRN_NODE_NOT) v.w[q] &= ~w.w[q];
-                        // OPTIONAL: the optional side never changes the match set
-                }
-        }
-        return v;
-}
-
-extern "C" int trn_query_truth_table(const trn_qnode *nodes, uint32_t nnodes, uint32_t root, uint32_t *terms, uint32_t *nterms, uint32_t *table, uint32_t *necessary) {
-        if (!nodes || !nnodes || root >= nnodes || !terms || !nterms || !table || !necessary)
-                return TRN_ERR_ARG;
-        for (uint32_t i = 0; i < nnodes; ++i) // same structural rules as the plan compiler: children behind their parent, bounded depth
-                if (nodes[i].kind != TRN_NODE_TERM && (nodes[i].nchildren == 0 || nodes[i].first_child <= i || uint32_t(nodes[i].first_child) + nodes[i].nchildren > nnodes))
-                        return TRN_ERR_ARG;
-        if (!plan_depth_ok(nodes, nnodes) || !plan_is_tree(nodes, nnodes, root))
-                return TRN_ERR_ARG;
-        uint32_t n{0}, stack[64], sp{0};
-        stack[sp++] = root;
-        while (sp) {
-                const auto &X = nodes[stack[--sp]];
-                if (X.kind == TRN_NODE_TERM) {
-                        if (X.term == kEmptyTerm)
-                                continue;
-                        bool seen{false};
-                        for (uint32_t j = 0; j < n; ++j)
-                                seen |= terms[j] == X.term;
-                        if (!seen) {
-                                if (n == 8)
-                                        return TRN_ERR_ARG;
-                                terms[n++] = X.term;
-                        }
-                } else {
-                        if (X.kind == TRN_NODE_PHRASE)
-                                return TRN_ERR_UNSUPPORTED;
-                        if (X.kind > TRN_NODE_SOME || X.nchildren == 0 || uint32_t(X.first_child) + X.nchildren > nnodes || sp + X.nchildren > 64)
-                                return TRN_ERR_ARG;
-                        for (uint32_t k = 0; k < X.nchildren; ++k)
-                                stack[sp++] = X.first_child + k;
-                }
-        }
-        const TruthVec v = truth_vector(nodes, root, terms, n);
-        uint32_t       nec{n ? (1u << n) - 1u : 0u};
-        for (uint32_t w = 0; w < 8; ++w)
-                table[w] = 0;
-        for (uint32_t a = 0; a < (1u << n); ++a)
-                if ((v.w[a >> 6] >> (a & 63u)) & 1ull) {
-                        table[a >> 5] |= 1u << (a & 31u);
-                        nec &= a;
-                }
-        *nterms    = n;
-        *necessary = nec;
-        return TRN_OK;
-}
-
-// Flat-tree form of a DocumentsOnly step program (k_exec_docs, exec_docs_flat.cuh): every leaf gets a bitmap of its own (slots 0 .. nl-1,
-// announced by one [OP_LEAF M_NONE dst = leaf slot] marker each, at the front of the program) that ONE flat (leaf, block) pass over the tile
-// fills; the rest of the program becomes slot operations on them, the compiler's own slots moved behind the leaf bitmaps.
-// Returns the number of leaves (0: the program stays as it is).
-// Leaf bitmaps are numbered by descending block count: the (leaf, block) list of a tile is then ordered from the frequent terms (blocks
-// of 1-byte deltas, four codes per decoder step) to the rare ones (2-byte deltas, blocks that straddle the tile), so that the 32 lanes
-// of a group mostly walk blocks of the same kind — a rare term's lane among frequent ones kept the whole warp in the loop for its 16-31
-// slow steps (those ran at a few of 32 lanes and were as many instructions as the fast ones).
-// Afterwards the copies are coalesced (flat_tree_coalesce): `SET d <- s` where s is not read again becomes a renaming of d, so a chain
-// like SET t <- leaf; AND t, leaf2; OR acc, t runs in the leaf's own bitmap: fewer operations per tile and — what matters more — fewer
-// bitmaps per warp (13 -> 8 for the 8-term trees of the benchmark), i.e. more resident warps.
-// rootSlot: in = the compiler's root slot, out = the slot that holds the root docset; slotsInUse: out.
-static void     flat_tree_coalesce(std::vector<DevStep> &steps, size_t opsBegin, uint32_t nl, uint32_t &rootSlot, uint32_t &slotsInUse);
-static uint32_t flat_tree_transform(std::vector<DevStep> &steps, size_t begin, uint32_t next_slot, const std::vector<DevTerm> &terms, std::vector<uint32_t> *leafNodes,
-                                    uint32_t &rootSlot, uint32_t &slotsInUse) {
-        uint32_t nl{0};
-        for (size_t i = begin; i < steps.size(); ++i)
-                nl += steps[i].op == OP_LEAF && steps[i].mode != M_NONE;
-        uint32_t nops{nl}; // slot operations of the transformed program: one per decoding leaf + every non-leaf step
-        for (size_t i = begin; i < steps.size(); ++i)
-                nops += steps[i].op != OP_LEAF;
-        if (nl < 2 || nl > 16 || nl + next_slot > 30 || nops > 32)
-                return 0; // (the kernel keeps leaves and slot operations in lane registers: <= 16 leaves, <= 32 operations, slots < 32)
-        for (size_t i = begin; i < steps.size(); ++i)
-                if (steps[i].op == OP_COUNT_GE && steps[i].term > 15u)
-                        return 0;
-        const std::vector<DevStep> prog(steps.begin() + begin, steps.end());
-        steps.resize(begin);
-        std::vector<DevStep> leaves;
-        for (const auto &st : prog)
-                if (st.op == OP_LEAF && st.mode != M_NONE)
-                        leaves.push_back(st);
-        std::vector<uint32_t> order(nl), slotOf(nl); // order[k]: program leaf held by bitmap k; slotOf: its inverse
-        for (uint32_t j = 0; j < nl; ++j)
-                order[j] = j;
-        auto blocksOf = [&](uint32_t j) { return leaves[j].term == kEmptyTerm ? 0u : terms[leaves[j].term].nblocks; };
-        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return blocksOf(a) > blocksOf(b); });
-        for (uint32_t k = 0; k < nl; ++k) {
-                slotOf[order[k]] = k;
-                DevStep L        = leaves[order[k]]; // decode marker: term -> leaf bitmap k
-                L.mode           = M_NONE;
-                L.dst            = uint8_t(k);
-                L.src            = 0;
-                L.flags          = 0;
-                steps.push_back(L);
-        }
-        if (leafNodes && leafNodes->size() == nl) {
-                const std::vector<uint32_t> was(*leafNodes);
-                for (uint32_t k = 0; k < nl; ++k)
-                        (*leafNodes)[k] = was[order[k]];
-        }
-        uint32_t li{0};
-        for (auto st : prog) {
-                if (st.op == OP_LEAF) {
-                        if (st.mode == M_NONE)
-                                continue; // nothing to do in DocumentsOnly mode
-                        DevStep S;
-                        std::memset(&S, 0, sizeof(S));
-                        S.op    = OP_SLOT;
-                        S.mode  = st.mode;
-                        S.dst   = uint8_t(st.dst + nl);
-                        S.src   = uint8_t(slotOf[li++]);
-                        S.flags = st.flags;
-                        steps.push_back(S);
-                        continue;
-                }
-                st.dst = uint8_t(st.dst + nl); // compiler slots live behind the leaf bitmaps
-                if (st.op == OP_SLOT || st.op == OP_COUNT_ADD || st.op == OP_COUNT_GE)
-                        st.src = uint8_t(st.src + nl);
-                steps.push_back(st);
-        }
-        rootSlot += nl;
-        slotsInUse = nl + next_slot;
-        flat_tree_coalesce(steps, begin + nl, nl, rootSlot, slotsInUse);
-        return nl;
-}
-
-static void flat_tree_coalesce(std::vector<DevStep> &steps, size_t opsBegin, uint32_t nl, uint32_t &rootSlot, uint32_t &slotsInUse) {
-        std::vector<DevStep> ops(steps.begin() + std::ptrdiff_t(opsBegin), steps.end());
-        for (const auto &o : ops)
-                if (o.op != OP_SLOT && o.op != OP_CLEAR)
-                        return; // (counter planes address slot RANGES: left alone)
-        auto reads = [](const DevStep &o, uint32_t x) { // does o read slot x?
-                if (o.op != OP_SLOT)
-                        return false;
-                if (o.mode == M_NONE)
-                        return o.dst == x; // emptiness test only
-                return o.src == x || (o.mode != M_SET && o.dst == x);
-        };
-        auto overwrites = [](const DevStep &o, uint32_t x) { return o.dst == x && (o.op == OP_CLEAR || (o.op == OP_SLOT && o.mode == M_SET)); };
-        // x is dead behind operation i: nothing reads it before it is overwritten, and it is not the root
-        auto dead = [&](size_t i, uint32_t x) {
-                for (size_t j = i + 1; j < ops.size(); ++j) {
-                        if (reads(ops[j], x))
-                                return false;
-                        if (overwrites(ops[j], x))
-                                return true;
-                }
-                return x != rootSlot;
-        };
-        // CLEAR d ... OR d, x (nothing touching d in between)  ==  SET d <- x
-        std::vector<uint8_t> drop(ops.size(), 0);
-        for (size_t i = 0; i < ops.size(); ++i) {
-                if (ops[i].op != OP_CLEAR)
-                        continue;
-                const uint32_t d = ops[i].dst;
-                for (size_t j = i + 1; j < ops.size(); ++j) {
-                        const bool touches = ops[j].dst == d || (ops[j].op == OP_SLOT && ops[j].src == d);
-                        if (!touches)
-                                continue;
-                        if (ops[j].op == OP_SLOT && ops[j].mode == M_OR && ops[j].dst == d && ops[j].src != d) {
-                                ops[j].mode = M_SET;
-                                drop[i]     = 1;
-                        }
-                        break;
-                }
-        }
-        // forward renaming: ren[name] = the physical slot that holds it, holder[slot] = the name it holds (the compiler hands slot numbers
-        // out again, so a name that is overwritten must not land in a slot that meanwhile carries another live name)
-        uint32_t ren[32], holder[32];
-        for (uint32_t i = 0; i < 32; ++i)
-                ren[i] = holder[i] = i;
-        auto deadFrom = [&](size_t i, uint32_t x) { // like dead(), operation i included
-                if (x >= 32u)
-                        return true;
-                if (i < ops.size() && reads(ops[i], x))
-                        return false;
-                if (i < ops.size() && overwrites(ops[i], x))
-                        return true;
-                return dead(i, x);
-        };
-        std::vector<DevStep> out;
-        for (size_t i = 0; i < ops.size(); ++i) {
-                if (drop[i])
-                        continue;
-                DevStep o = ops[i];
-                if (o.op == OP_SLOT && o.mode == M_SET && o.src != o.dst && dead(i, o.src)) {
-                        const uint32_t p = ren[o.src];
-                        if (holder[ren[o.dst]] == o.dst)
-                                holder[ren[o.dst]] = 0xffu;
-                        ren[o.dst] = p;
-                        holder[p]  = o.dst;
-                        if (o.flags & F_BREAK_IF_EMPTY) { // the emptiness test stays, on the slot that now carries the name
-                                o.mode = M_NONE;
-                                o.dst  = uint8_t(p);
-                                o.src  = uint8_t(p);
-                                out.push_back(o);
-                        }
-                        continue;
-                }
-                if (o.op == OP_SLOT)
-                        o.src = uint8_t(ren[o.src]);
-                if (o.op == OP_CLEAR || (o.op == OP_SLOT && o.mode == M_SET)) { // a full overwrite: the name needs a slot nobody lives in
-                        uint32_t p = ren[o.dst];
-                        if (holder[p] != o.dst && !deadFrom(i, holder[p])) {
-                                p = 0xffu;
-                                for (uint32_t k = 0; k < 31u && p == 0xffu; ++k) {
-                                        const uint32_t q = k + nl < 31u ? k + nl : k + nl - 31u; // compiler slots first, then leaf bitmaps already consumed
-                                        if (deadFrom(i, holder[q]) && !(o.op == OP_SLOT && q == o.src))
-                                                p = q;
-                                }
-                                if (p == 0xffu)
-                                        return; // (cannot happen: the program had a slot for every live name) leave the program as it was
-                        }
-                        ren[o.dst] = p;
-                        holder[p]  = o.dst;
-                }
-                o.dst = uint8_t(ren[o.dst]);
-                out.push_back(o);
-        }
-        rootSlot = ren[rootSlot];
-        // compiler slots still in use, renumbered densely behind the leaf bitmaps
-        uint32_t map[32];
-        uint32_t next = nl;
-        for (uint32_t i = 0; i < 32; ++i)
-                map[i] = i < nl ? i : 0xffu;
-        auto use = [&](uint32_t x) {
-                if (x >= nl && map[x] == 0xffu)
-                        map[x] = next++;
-        };
-        for (const auto &o : out) {
-                use(o.dst);
-                if (o.op == OP_SLOT)
-                        use(o.src);
-        }
-        use(rootSlot);
-        for (auto &o : out) {
-                o.dst = uint8_t(map[o.dst]);
-                if (o.op == OP_SLOT)
-                        o.src = uint8_t(map[o.src]);
-        }
-        rootSlot   = map[rootSlot];
-        slotsInUse = next;
-        steps.resize(opsBegin);
-        steps.insert(steps.end(), out.begin(), out.end());
-}
-
-// Masked second decode pass of the flat-tree path.  A leaf whose blocks are short in docID terms (a frequent term) does not have to be
-// decoded where the rest of the tree already rules a match out: if x sits under a conjunction next to S, the value of x outside S cannot
-// reach the root (the conjunction is false there whatever x says), and the same holds for the excluded side of a Filter outside its
-// required side, through any number of operators above.  So the frequent leaves are decoded in a SECOND pass, and of their blocks only
-// those whose docID range holds a set bit of a mask bitmap: the conjunction of the constraint subtrees on the leaf's path to the root,
-// evaluated over the first-pass leaf bitmaps (any superset is a valid mask: an operand of a conjunction that is itself second-pass is
-// left out, a disjunction with such an operand is not usable).  This is Conjuction::next's advance() on the longer list
-// (docset_iterators.cpp:282-348) at block granularity.  The tree semantics used here are the compiler's (Compiler::node), from its
-// effective root.  Layout of the program afterwards: [leaf markers] [mask operations, F_MASKOP] [the unchanged slot operations].
-// Returns the number of slots the masks add.
-static uint32_t flat_tree_masks(std::vector<DevStep> &steps, size_t begin, uint32_t nl, uint32_t slotsInUse, const trn_qnode *n, uint32_t nn, uint32_t root,
-                                const std::vector<uint32_t> &leafNodes, const std::vector<DevTerm> &terms, uint32_t tileShift, double width) {
-        if (leafNodes.size() != nl || nl > 16 || width <= 0)
-                return 0;
-        std::vector<int> leafOf(nn, -1), parent(nn, -1);
-        for (uint32_t j = 0; j < nl; ++j)
-                leafOf[leafNodes[j]] = int(j);
-        {
-                std::vector<uint32_t> st{root};
-                while (!st.empty()) {
-                        const uint32_t i = st.back();
-                        st.pop_back();
-                        if (n[i].kind == TRN_NODE_TERM)
-                                continue;
-                        for (uint32_t c = 0; c < n[i].nchildren; ++c) {
-                                parent[n[i].first_child + c] = int(i);
-                                st.push_back(n[i].first_child + c);
-                        }
-                }
-        }
-        auto blocksOf = [&](uint32_t j) -> double {
-                const uint32_t t = n[leafNodes[j]].term;
-                return t == kEmptyTerm ? 0.0 : double(terms[t].nblocks);
-        };
-        auto densOf = [&](uint32_t j) -> double {
-                const uint32_t t = n[leafNodes[j]].term;
-                return t == kEmptyTerm ? 0.0 : std::min(1.0, double(terms[t].documents) / width);
-        };
-        std::vector<uint8_t> masked(nl, 0);
-        // density of the superset of node i computable from first-pass leaves (-1: unusable)
-        std::function<double(uint32_t)> sup = [&](uint32_t i) -> double {
-                const auto &X = n[i];
-                switch (X.kind) {
-                        case TRN_NODE_TERM:
-                                return (leafOf[i] >= 0 && !masked[leafOf[i]]) ? densOf(uint32_t(leafOf[i])) : -1.0;
-                        case TRN_NODE_AND: {
-                                double d{1.0};
-                                bool   any{false};
-                                for (uint32_t c = 0; c < X.nchildren; ++c) {
-                                        const double x = sup(X.first_child + c);
-                                        if (x >= 0) {
-                                                d *= x;
-                                                any = true;
-                                        }
-                                }
-                                return any ? d : -1.0;
-                        }
-                        case TRN_NODE_OR: {
-                                double d{1.0};
-                                for (uint32_t c = 0; c < X.nchildren; ++c) {
-                                        const double x = sup(X.first_child + c);
-                                        if (x < 0)
-                                                return -1.0;
-                                        d *= 1.0 - x;
-                                }
-                                return 1.0 - d;
-                        }
-                        case TRN_NODE_NOT:
-                        case TRN_NODE_OPTIONAL:
-                                return sup(X.first_child);
-                        default:
-                                return -1.0;
-                }
-        };
-        // constraint subtrees of leaf j
-        auto constraints = [&](uint32_t j) {
-                std::vector<uint32_t> out;
-                int                   c = int(leafNodes[j]);
-                while (uint32_t(c) != root && parent[c] >= 0) {
-                        const int   p = parent[c];
-                        const auto &X = n[p];
-                        if (X.kind == TRN_NODE_AND) {
-                                for (uint32_t k = 0; k < X.nchildren; ++k)
-                                        if (int(X.first_child + k) != c)
-                                                out.push_back(X.first_child + k);
-                        } else if (X.kind == TRN_NODE_NOT && int(X.first_child) + 1 == c)
-                                out.push_back(X.first_child);
-                        c = p;
-                }
-                return out;
-        };
-        const double W = double(1ull << tileShift);
-        auto         need = [&](uint32_t j) { // estimated share of leaf j's blocks a mask leaves over
-                double d{1.0};
-                bool   any{false};
-                for (auto cn : constraints(j)) {
-                        const double x = sup(cn);
-                        if (x >= 0) {
-                                d *= x;
-                                any = true;
-                        }
-                }
-                if (!any)
-                        return 1.0;
-                const double span = width / std::max(1.0, blocksOf(j)); // docIDs a block covers
-                return 1.0 - std::pow(1.0 - std::min(d, 1.0), span);
-        };
-        std::vector<uint32_t> order(nl);
-        for (uint32_t j = 0; j < nl; ++j)
-                order[j] = j;
-        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return blocksOf(a) > blocksOf(b); });
-        bool anyMasked{false};
-        for (auto j : order) {
-                if (blocksOf(j) * W / width < 2.0)
-                        break; // (sorted) blocks as wide as the tile: nothing to skip
-                masked[j] = 1;
-                if (need(j) > g_tree_mask_need)
-                        masked[j] = 0;
-                anyMasked |= masked[j] != 0;
-        }
-        for (auto j : order) // a later choice may have taken a constraint away
-                if (masked[j] && need(j) > g_tree_mask_need + 0.15)
-                        masked[j] = 0;
-        if (!anyMasked)
-                return 0;
-        // ---- emission
-        std::vector<DevStep>                      mops;
-        std::unordered_map<uint32_t, int>         slotOfNode;
-        std::map<std::vector<int>, int>           slotOfAnd;
-        uint32_t                                  extra{0};
-        const uint32_t                            kMaxExtra = 6;
-        auto                                      newSlot   = [&]() -> int { return (extra < kMaxExtra && slotsInUse + extra < 30u) ? int(slotsInUse + extra++) : -1; };
-        auto                                      op        = [&](uint8_t mode, int dst, int src) {
-                DevStep S;
-                std::memset(&S, 0, sizeof(S));
-                S.op    = OP_SLOT;
-                S.mode  = mode;
-                S.dst   = uint8_t(dst);
-                S.src   = uint8_t(src);
-                S.flags = F_MASKOP;
-                mops.push_back(S);
-        };
-        std::function<int(uint32_t)> emit = [&](uint32_t i) -> int { // slot holding a superset of node i, -1: unusable (or out of slots)
-                const auto it = slotOfNode.find(i);
-                if (it != slotOfNode.end())
-                        return it->second;
-                const auto &X = n[i];
-                int         r{-1};
-                if (X.kind == TRN_NODE_TERM)
-                        r = (leafOf[i] >= 0 && !masked[leafOf[i]]) ? leafOf[i] : -1;
-                else if (X.kind == TRN_NODE_NOT || X.kind == TRN_NODE_OPTIONAL)
-                        r = emit(X.first_child);
-                else if (X.kind == TRN_NODE_AND || X.kind == TRN_NODE_OR) {
-                        std::vector<int> kids;
-                        bool             ok{true};
-                        for (uint32_t c = 0; c < X.nchildren && ok; ++c) {
-                                const int k = sup(X.first_child + c) >= 0 ? emit(X.first_child + c) : -1;
-                                if (k >= 0)
-                                        kids.push_back(k);
-                                else if (X.kind == TRN_NODE_OR)
-                                        ok = false;
-                        }
-                        if (ok && kids.size() == 1)
-                                r = kids[0];
-                        else if (ok && kids.size() > 1) {
-                                r = newSlot();
-                                if (r >= 0) {
-                                        op(M_SET, r, kids[0]);
-                                        for (size_t k = 1; k < kids.size(); ++k)
-                                                op(X.kind == TRN_NODE_AND ? M_AND : M_OR, r, kids[k]);
-                                }
-                        }
-                }
-                slotOfNode[i] = r;
-                return r;
-        };
-        std::vector<int> maskSlot(nl, -1);
-        for (uint32_t j = 0; j < nl; ++j) {
-                if (!masked[j])
-                        continue;
-                std::vector<int> cs;
-                for (auto cn : constraints(j))
-                        if (sup(cn) >= 0) {
-                                const int k = emit(cn);
-                                if (k >= 0)
-                                        cs.push_back(k);
-                        }
-                std::sort(cs.begin(), cs.end());
-                cs.erase(std::unique(cs.begin(), cs.end()), cs.end());
-                if (cs.empty()) {
-                        masked[j] = 0; // (cannot be relied on by anybody: it was never usable)
-                        continue;
-                }
-                int m;
-                if (cs.size() == 1)
-                        m = cs[0];
-                else {
-                        const auto it = slotOfAnd.find(cs);
-                        if (it != slotOfAnd.end())
-                                m = it->second;
-                        else {
-                                m = newSlot();
-                                if (m >= 0) {
-                                        op(M_SET, m, cs[0]);
-                                        for (size_t k = 1; k < cs.size(); ++k)
-                                                op(M_AND, m, cs[k]);
-                                        slotOfAnd[cs] = m;
-                                } else
-                                        m = cs[0]; // out of slots: one constraint alone is a (weaker) mask
-                        }
-                }
-                maskSlot[j] = m;
-        }
-        if (mops.size() > 32)
-                return 0;
-        anyMasked = false;
-        for (uint32_t j = 0; j < nl; ++j)
-                if (masked[j] && maskSlot[j] >= 0) {
-                        steps[begin + j].flags |= F_MASKED;
-                        steps[begin + j].src = uint8_t(maskSlot[j]);
-                        anyMasked            = true;
-                }
-        if (!anyMasked)
-                return 0;
-        steps.insert(steps.begin() + std::ptrdiff_t(begin + nl), mops.begin(), mops.end());
-        return extra;
-}
-
-extern "C" int trn_debug_compile(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, const trn_qnode *nodes, uint32_t nnodes,
-                                 uint32_t root, int scored, trn_debug_step *out, uint32_t cap, uint32_t *nsteps, uint32_t *root_slot, uint32_t *nslots, char *err,
-                                 size_t errcap) {
-        static_assert(sizeof(trn_debug_step) == sizeof(DevStep), "trn_debug_step mirrors DevStep");
-        auto seterr = [&](const std::string &m, int rc) {
-                if (err && errcap) {
-                        std::strncpy(err, m.c_str(), errcap - 1);
-                        err[errcap - 1] = 0;
-                }
-                return rc;
-        };
-        if (!index || !terms || !nodes || !nnodes || !out || !nsteps || !root_slot || !nslots || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))
-                return seterr("bad arguments", TRN_ERR_ARG);
-        BlockDirectory dir;
-        try {
-                std::vector<term_index_ctx> t(nterms);
-                for (uint32_t i = 0; i < nterms; ++i) {
-                        t[i].documents = terms[i].documents;
-                        t[i].offset    = terms[i].chunk_off;
-                        t[i].size      = terms[i].chunk_len;
-                }
-                build_block_directory(codec == TRN_CODEC_GOOGLE ? Codec::Google : Codec::Lucene, index, nbytes, t.data(), nterms, 1, dir);
-        } catch (const std::exception &e) {
-                return seterr(e.what(), TRN_ERR_FORMAT);
-        }
-        std::vector<DevTerm> ht(nterms);
-        for (uint32_t i = 0; i < nterms; ++i) {
-                ht[i].documents = dir.terms[i].documents;
-                ht[i].dir_begin = dir.terms[i].dir_begin;
-                ht[i].nblocks   = dir.terms[i].nblocks;
-                ht[i].first_doc = dir.terms[i].first_doc;
-                ht[i].last_doc  = dir.terms[i].last_doc;
-                ht[i].chunk_len = terms[i].chunk_len;
-                ht[i].tf_begin  = dir.terms[i].tf_begin;
-                ht[i].tf_base   = dir.terms[i].tf_base;
-                ht[i].tf_shift  = dir.terms[i].tf_shift;
-        }
-        std::vector<DevStep> steps;
-        Compiler             cc(nodes, nnodes, ht, scored == 1, root, steps);
-        int                  rs = cc.run();
-        if (rs < 0)
-                return seterr(cc.err, cc.unsupported ? TRN_ERR_UNSUPPORTED : TRN_ERR_ARG);
-        uint32_t treeLeaves{0};
-        uint32_t maskSlots{0}, treeSlotsInUse{0};
-        if (scored >= 2) { // DocumentsOnly program in its flat-tree form (what the second k_exec_docs launch runs); 3: with the masked second pass
-                uint32_t root2 = uint32_t(rs);
-                treeLeaves     = flat_tree_transform(steps, 0, cc.next_slot, ht, &cc.leaf_nodes, root2, treeSlotsInUse);
-                if (treeLeaves)
-                        rs = int(root2);
-                if (scored == 3 && treeLeaves) {
-                        uint32_t lo{0xffffffffu}, hi{0};
-                        for (const auto &T : ht)
-                                if (T.nblocks) {
-                                        lo = std::min(lo, T.first_doc);
-                                        hi = std::max(hi, T.last_doc);
-                                }
-                        if (hi >= lo)
-                                maskSlots = flat_tree_masks(steps, 0, treeLeaves, treeSlotsInUse, nodes, nnodes, cc.root, cc.leaf_nodes, ht, 12, double(hi) - double(lo) + 1.0);
-                }
-        }
-        if (steps.size() > cap)
-                return seterr("step buffer too small", TRN_ERR_CAPACITY);
-        std::memcpy(out, steps.data(), steps.size() * sizeof(DevStep));
-        *nsteps    = uint32_t(steps.size());
-        *root_slot = uint32_t(rs);
-        *nslots    = (treeLeaves ? treeSlotsInUse + maskSlots : cc.next_slot) + 1; // + the scratch slot of the kernels
-        return TRN_OK;
-}
-
-static void push_step(std::vector<DevStep> &steps, uint8_t op, uint8_t mode, uint32_t dst, uint32_t src, uint8_t flags, uint32_t term, double idf) {
-        DevStep s;
-        std::memset(&s, 0, sizeof(s));
-        s.op    = op;
-        s.mode  = mode;
-        s.dst   = uint8_t(dst);
-        s.src   = uint8_t(src);
-        s.flags = flags;
-        s.term  = term;
-        s.idf   = idf;
-        steps.push_back(s);
-}
-
 // =================================================================================================== exec
-// small device scratch layout (d_small): [0] ticket u32, [2..3] seg_cursor u64, [4] overflow u32, then per-query arrays
-static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out, int set, cudaEvent_t k0, cudaEvent_t k1) {
+// small device scratch layout (d_small): [0] ticket u32, [2..3] seg_cursor u64, [4] overflow u32, then per-query arrays.
+// routes[0 .. nq): the TRN_ROUTE_* of every query (written on success)
+static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out, int set, cudaEvent_t k0, cudaEvent_t k1,
+                            uint8_t *routes) {
         if (!c)
                 return TRN_ERR_ARG;
         if (!c->have_index)
@@ -1703,305 +463,26 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         const bool compact = mode == TRN_MODE_DOCS_COMPACT; // DocumentsOnly with compact result segments; everything else is the same plan
         if (compact)
                 mode = TRN_MODE_DOCS_ONLY;
-        if (c->block_docs != (c->codec == TRN_CODEC_GOOGLE ? 32u : 128u))
+        if (c->block_docs != (c->pc.codec == TRN_CODEC_GOOGLE ? 32u : 128u))
                 return fail(c, TRN_ERR_UNSUPPORTED, "the uploaded index was built with a block size other than the reference format's (decode sweep only)");
         if (mode == TRN_MODE_SCORED_TOPK && (k == 0 || k > kernel_max_k()))
                 return fail(c, TRN_ERR_ARG, "top-k: k must be in [1, 512]");
         CK(cudaSetDevice(c->device));
         const bool scored = mode != TRN_MODE_DOCS_ONLY;
-        // docID tile of this launch: set queries run one warp per tile (k_exec_docs) on larger tiles; scored queries keep a CTA-wide
-        // fp32 score tile (k_exec_tiles).
-        uint32_t execShift = scored ? c->tile_shift : c->docs_shift;
-        execShift          = std::max(execShift, c->tile_shift);
 
-        const double           tCompile0 = now_ms();
-        std::vector<DevQuery>  hq(nq);
-        std::vector<DevStep>   steps;
-        std::vector<FlatQuery> fqs;    // queries k_score_flat runs
-        std::vector<FlatLeaf>  leaves;
-        uint64_t               genItems{0}, genItems2{0}, flatItems{0};
-        uint32_t               treeSlots{1};
-        uint32_t               maxRuns{0};
-        uint32_t              maxSlots{1};
-        bool                  anyCandidate{false}, anyMembership{false}, anyPhrase{false};
-        uint64_t              items{0}, segCap{0}, candTotal{0}, postings{0}, bytes{0};
-        c->call_routes.assign(nq, 0);
-        for (uint32_t q = 0; q < nq; ++q) {
-                const auto &Q = queries[q];
-                if (!Q.nodes || !Q.nnodes)
-                        return fail(c, TRN_ERR_ARG, "empty query");
-                Compiler cc(Q.nodes, Q.nnodes, c->h_terms, scored, Q.root, steps);
-                cc.allow_phrase = c->codec == TRN_CODEC_GOOGLE || c->have_hits; // GOOGLE: inline hits; LUCENE: hits.data uploaded (trn_upload_hits)
-                auto &   dq     = hq[q];
-                dq.step_begin   = uint32_t(steps.size());
-                const int rs    = cc.run();
-                anyPhrase |= cc.has_phrase;
-                if (rs < 0)
-                        return fail(c, cc.unsupported ? TRN_ERR_UNSUPPORTED : TRN_ERR_ARG, "query " + std::to_string(q) + ": " + cc.err);
-                dq.nsteps    = uint32_t(steps.size()) - dq.step_begin;
-                dq.root_slot = uint32_t(rs);
-                dq.flat      = 0;
-                {
-                        // conjunction / disjunction whose operands are all terms (matchallterms / matchanyterms runs)
-                        const auto &R = Q.nodes[cc.root];
-                        if ((R.kind == TRN_NODE_AND || R.kind == TRN_NODE_OR) && R.nchildren <= 16) {
-                                bool allTerms{true};
-                                for (uint32_t ch = 0; ch < R.nchildren; ++ch)
-                                        allTerms &= Q.nodes[R.first_child + ch].kind == TRN_NODE_TERM;
-                                if (allTerms) {
-                                        dq.flat = R.kind == TRN_NODE_AND ? 1u : 2u;
-                                        if (R.kind == TRN_NODE_AND && R.nchildren <= 3)
-                                                maxSlots = std::max<uint32_t>(maxSlots, R.nchildren); // one bitmap per operand
-                                }
-                        }
-                }
-                postings += cc.postings;
-                bytes += cc.bytes;
-                const Range r = cc.range(cc.root); // cc.root: the effective root (see apply_reference_root_filter_quirk)
-                // Flat scored disjunction (a k-term OR / a single term, every leaf scoring with a weight >= +0.0) on the LUCENE codec:
-                // k_score_flat (score_flat.cuh) instead of the step program
-                bool flatScored{false};
-                if (scored && c->flat_scored && c->codec == TRN_CODEC_LUCENE && execShift >= 13) {
-                        const auto &R = Q.nodes[cc.root];
-                        uint32_t    f0{cc.root}, nl{1};
-                        bool        ok = R.kind == TRN_NODE_TERM;
-                        if (R.kind == TRN_NODE_OR && R.nchildren <= score_flat_max_leaves()) {
-                                ok = true;
-                                f0 = R.first_child;
-                                nl = R.nchildren;
-                                for (uint32_t ch = 0; ch < nl; ++ch)
-                                        ok &= Q.nodes[f0 + ch].kind == TRN_NODE_TERM;
-                        }
-                        for (uint32_t ch = 0; ok && ch < nl; ++ch) {
-                                const double w = Q.nodes[f0 + ch].weight;
-                                ok             = std::isfinite(w) && !std::signbit(w); // the -0.0f "untouched" sentinel of the score tile needs contributions >= +0.0
-                        }
-                        if (ok) {
-                                flatScored = true;
-                                steps.resize(dq.step_begin); // no step program
-                                dq.nsteps = 0;
-                                dq.flat   = 4u;
-                                FlatQuery fq;
-                                std::memset(&fq, 0, sizeof(fq));
-                                fq.qid        = q;
-                                fq.leaf_begin = uint32_t(leaves.size());
-                                fq.nleaf      = nl;
-                                for (uint32_t ch = 0; ch < nl; ++ch) {
-                                        FlatLeaf L;
-                                        L.term = Q.nodes[f0 + ch].term;
-                                        L.pad  = 0;
-                                        L.idf  = Q.nodes[f0 + ch].weight;
-                                        leaves.push_back(L);
-                                }
-                                fqs.push_back(fq);
-                        }
-                }
-                const uint32_t planSlots = cc.next_slot + 1; // + scratch slot (applied below, once the path of the query is known)
-                // Candidate-driven evaluation (exec_docs_cand.cuh) when some term that EVERY match must hold is sparse: cost follows that
-                // lead's postings (~cand_cost/2 warp-instructions per 32 candidates and probed term; the crossover was tuned on the and2
-                // workload: 900 beats 450 and 1500) instead of the docID space (~1500 per tile + ~27 per block in it).
-                // The boolean function of the tree over its (<= 8 distinct) terms is tabulated here; the device probes every term for
-                // each candidate and looks the membership bits up.
-                bool candidate{false};
-                if (!scored && c->codec == TRN_CODEC_GOOGLE && c->cand_cost > 0 && !r.empty() && !cc.has_phrase) {
-                        // distinct non-empty terms below the effective root (at most 8)
-                        uint32_t tv[8];
-                        uint32_t n{0};
-                        bool     small{true};
-                        {
-                                uint32_t stack[64], sp{0};
-                                stack[sp++] = cc.root;
-                                while (sp && small) {
-                                        const auto &X = Q.nodes[stack[--sp]];
-                                        if (X.kind == TRN_NODE_TERM) {
-                                                if (X.term == kEmptyTerm || !c->h_terms[X.term].nblocks)
-                                                        continue;
-                                                bool seen{false};
-                                                for (uint32_t j = 0; j < n; ++j)
-                                                        seen |= tv[j] == X.term;
-                                                if (!seen) {
-                                                        if (n == 8)
-                                                                small = false;
-                                                        else
-                                                                tv[n++] = X.term;
-                                                }
-                                        } else if (sp + X.nchildren > 64)
-                                                small = false;
-                                        else
-                                                for (uint32_t k = 0; k < X.nchildren; ++k)
-                                                        stack[sp++] = X.first_child + k;
-                                }
-                        }
-                        small = small && n >= 2;
-                        if (small) {
-                                // truth vectors: bit `bits` of vec(node) = value of the node under the term assignment `bits` (bit j = tv[j])
-                                uint8_t  truth[256];
-                                uint32_t necessary{(1u << n) - 1u};
-                                bool     any{false};
-                                if (dq.flat == 1u && n == Q.nodes[cc.root].nchildren) { // all-term conjunction: only the all-ones assignment matches
-                                        std::memset(truth, 0, sizeof(truth));
-                                        truth[(1u << n) - 1u] = 1;
-                                        any                   = true;
-                                } else {
-                                        const TruthVec tvec = truth_vector(Q.nodes, cc.root, tv, n);
-                                        for (uint32_t bits = 0; bits < (1u << n); ++bits) {
-                                                truth[bits] = uint8_t((tvec.w[bits >> 6] >> (bits & 63u)) & 1ull);
-                                                if (truth[bits]) {
-                                                        necessary &= bits;
-                                                        any = true;
-                                                }
-                                        }
-                                }
-                                if (any && necessary) {
-                                        // probe order: the lead (rarest necessary term), the other necessary terms rarest first (they filter),
-                                        // then the rest
-                                        uint32_t order[8], nn{0}, no{0};
-                                        for (uint32_t j = 0; j < n; ++j)
-                                                if ((necessary >> j) & 1u)
-                                                        order[no++] = j;
-                                        nn = no;
-                                        for (uint32_t j = 0; j < n; ++j)
-                                                if (!((necessary >> j) & 1u))
-                                                        order[no++] = j;
-                                        auto byBlocks = [&](uint32_t x, uint32_t y) { return c->h_terms[tv[x]].nblocks < c->h_terms[tv[y]].nblocks; };
-                                        std::sort(order, order + nn, byBlocks);
-                                        std::sort(order + nn, order + n, byBlocks);
-                                        const uint32_t lead = tv[order[0]];
-                                        double         blocks{0};
-                                        for (uint32_t j = 0; j < n; ++j)
-                                                blocks += c->h_terms[tv[j]].nblocks;
-                                        const double width   = double(c->max_docid) - double(std::min(c->min_docid, c->max_docid)) + 1.0; // docID span of THIS source
-                                        const double perTile = double(1ull << execShift) / width;
-                                        const double lhs     = double(n - 1) * c->h_terms[lead].nblocks * perTile * double(c->cand_cost);
-                                        const double rhs     = 1500.0 + (dq.flat == 1u ? 0.0 : 150.0 * n) + blocks * perTile * (dq.flat == 1u ? 27.0 : 35.0);
-                                        if (lhs < rhs) {
-                                                // replace the step program: terms in probe order, then the truth table re-indexed to probe positions
-                                                steps.resize(dq.step_begin);
-                                                for (uint32_t j = 0; j < n; ++j)
-                                                        push_step(steps, OP_LEAF, M_NONE, 0, 0, 0, tv[order[j]], 0.0);
-                                                uint32_t words[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-                                                for (uint32_t pb = 0; pb < (1u << n); ++pb) { // pb: bit j = term at probe position j
-                                                        uint32_t bits{0};
-                                                        for (uint32_t j = 0; j < n; ++j)
-                                                                if ((pb >> j) & 1u)
-                                                                        bits |= 1u << order[j];
-                                                        if (truth[bits])
-                                                                words[pb >> 5] |= 1u << (pb & 31u);
-                                                }
-                                                for (uint32_t w = 0; w < 8; w += 4) {
-                                                        DevStep st;
-                                                        std::memset(&st, 0, sizeof(st));
-                                                        st.op   = OP_TABLE;
-                                                        st.dst  = uint8_t(w);
-                                                        st.term = words[w];
-                                                        st.pad2 = words[w + 1];
-                                                        uint64_t hi = uint64_t(words[w + 2]) | (uint64_t(words[w + 3]) << 32);
-                                                        std::memcpy(&st.idf, &hi, 8);
-                                                        steps.push_back(st);
-                                                }
-                                                dq.nsteps    = uint32_t(steps.size()) - dq.step_begin;
-                                                dq.root_slot = nn;
-                                                candidate    = true;
-                                                dq.flat      = 3u;
-                                                dq.tile_lo   = 0;
-                                                dq.ntiles    = (c->h_terms[lead].nblocks + 31u) / 32u;
-                                                anyCandidate = true;
-                                                anyMembership |= nn < n;
-                                        }
-                                }
-                        }
-                }
-                // Flat-tree path (exec_docs_flat.cuh): a DocumentsOnly tree that is neither an all-term run nor candidate-driven decodes ALL its
-                // leaves of a tile in one flat (leaf, block) pass — each leaf into a bitmap of its own — and then runs slot operations only.
-                // The per-leaf groups of the step-program path ran at a third of the lanes with up to 8 live bitmaps per warp; here
-                // the lanes are packed across leaves, and a smaller tile pays for the extra bitmaps.
-                bool treeFlat{false};
-                if (!scored && !candidate && dq.flat == 0u && c->codec == TRN_CODEC_GOOGLE && c->tree_shift && !r.empty() && !cc.has_phrase) {
-                        uint32_t       root2 = dq.root_slot, inUse{0};
-                        const uint32_t nl    = flat_tree_transform(steps, dq.step_begin, cc.next_slot, c->h_terms, &cc.leaf_nodes, root2, inUse);
-                        if (nl) {
-                                uint32_t extra{0};
-                                if (c->tree_masks) {
-                                        const double width = double(c->max_docid) - double(std::min(c->min_docid, c->max_docid)) + 1.0; // docID span of THIS source
-                                        extra = flat_tree_masks(steps, dq.step_begin, nl, inUse, Q.nodes, Q.nnodes, cc.root, cc.leaf_nodes, c->h_terms, c->tree_shift, width);
-                                }
-                                dq.nsteps = uint32_t(steps.size()) - dq.step_begin;
-                                dq.root_slot = root2;
-                                dq.flat      = 5u;
-                                treeSlots    = std::max(treeSlots, inUse + extra);
-                                treeFlat  = true;
-                        }
-                }
-                if (!flatScored && !treeFlat)
-                        maxSlots = std::max(maxSlots, planSlots);
-                // the path this query takes (trn_debug_last_routes): scored plans run k_score_flat or k_exec_tiles; the LUCENE
-                // instantiation of k_exec_docs has no flat AND / OR form and runs those plans as step programs
-                if (scored)
-                        c->call_routes[q] = flatScored ? TRN_ROUTE_SCORE_FLAT : TRN_ROUTE_EXEC_TILES;
-                else if (c->codec == TRN_CODEC_LUCENE && (dq.flat == 1u || dq.flat == 2u))
-                        c->call_routes[q] = TRN_ROUTE_STEPS;
-                else
-                        c->call_routes[q] = uint8_t(dq.flat); // 0 steps, 1 flat AND, 2 flat OR, 3 candidate-driven, 5 flat-tree (== TRN_ROUTE_*)
-                if (candidate) {
-                } else if (r.empty()) {
-                        dq.tile_lo = 0;
-                        dq.ntiles  = 0;
-                } else {
-                        const uint32_t qshift = flatScored ? c->scored_shift : (treeFlat ? c->tree_shift : execShift); // per-path tile
-                        dq.tile_lo            = r.lo >> qshift;
-                        dq.ntiles             = (r.hi >> qshift) - dq.tile_lo + 1;
-                }
-                dq.item_base = uint32_t(items);
-                dq.gen_base  = uint32_t(genItems);
-                dq.gen_base2 = uint32_t(genItems2);
-                items += dq.ntiles;
-                if (treeFlat)
-                        genItems2 += dq.ntiles;
-                else if (!flatScored)
-                        genItems += dq.ntiles;
-                if (items >= (1ull << 32))
-                        return fail(c, TRN_ERR_CAPACITY, "batch has more than 2^32 (query, tile) work items; split it");
-                const uint64_t width = r.empty() ? 0 : uint64_t(r.hi) - r.lo + 1;
-                segCap += std::min(cc.bound(cc.root), width);
-                dq.cand_base = uint32_t(candTotal);
-                dq.cand_cap  = uint32_t(std::min<uint64_t>(uint64_t(dq.ntiles) * k, 0xffffffffull));
-                if (flatScored) {
-                        auto &fq      = fqs.back();
-                        fq.tile_lo    = dq.tile_lo;
-                        fq.ntiles     = dq.ntiles;
-                        fq.nruns      = (dq.ntiles + c->run_tiles - 1u) / c->run_tiles;
-                        fq.item_base  = dq.item_base;
-                        fq.local_base = uint32_t(flatItems);
-                        flatItems += dq.ntiles;
-                        maxRuns     = std::max(maxRuns, fq.nruns);
-                        dq.cand_cap = uint32_t(std::min<uint64_t>(uint64_t(fq.nruns) * k, 0xffffffffull));
-                        fq.cand_base = dq.cand_base;
-                        fq.cand_cap  = dq.cand_cap;
-                }
-                if (mode == TRN_MODE_SCORED_TOPK) {
-                        candTotal += dq.cand_cap;
-                        if (candTotal >= (1ull << 32))
-                                return fail(c, TRN_ERR_CAPACITY, "top-k candidate space exceeds 2^32 entries; split the batch");
-                }
-        }
+        const double tCompile0 = now_ms();
+        c->pc.allow_phrase     = c->pc.codec == TRN_CODEC_GOOGLE || c->have_hits; // GOOGLE: inline hits; LUCENE: hits.data uploaded (trn_upload_hits)
+        BatchPlan   plan;
+        std::string perr;
+        const int   prc = plan_batch(c->pc, c->h_terms, queries, nq, mode, k, plan, perr);
+        if (prc != TRN_OK)
+                return fail(c, prc, perr);
         c->tm.host_compile_ms += float(now_ms() - tCompile0);
         const double   tEnqueue0  = now_ms();
-        const uint32_t totalItems = uint32_t(items);
-        if (anyCandidate) { // the candidate array + one gather buffer must fit a warp's share of shared memory
-                const uint32_t slotBytes = (1u << execShift) / 8u, stageB = exec_docs_stage_bytes(), need = exec_docs_cand_smem_bytes(anyMembership);
-                if (need > stageB)
-                        maxSlots = std::max(maxSlots, (need - stageB + slotBytes - 1u) / slotBytes);
-        }
-        // a flat conjunction keeps one bitmap per operand: with more operands than the launch has slots, flat_exec_google hands every
-        // tile to the step program (the launch's slot count is final only here)
-        for (uint32_t q = 0; q < nq; ++q)
-                if (c->call_routes[q] == TRN_ROUTE_FLAT_AND) {
-                        uint32_t nleaf{0};
-                        for (uint32_t si = 0; si < hq[q].nsteps; ++si)
-                                nleaf += steps[hq[q].step_begin + si].op == OP_LEAF;
-                        if (nleaf > maxSlots)
-                                c->call_routes[q] = TRN_ROUTE_STEPS;
-                }
+        const uint32_t totalItems = uint32_t(plan.items);
+        const uint32_t execShift  = plan.exec_shift;
+        const uint64_t segCap     = plan.seg_cap;
+        const auto &   steps      = plan.steps;
 
         // ---- result staging must fit the device: a caller (trn_exec_batch) reacts to TRN_ERR_CAPACITY by splitting the batch
         if (mode != TRN_MODE_SCORED_TOPK) {
@@ -2032,18 +513,18 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         CK(c->d_out_scores[set].ensure(std::max<size_t>(4, segCap * 4)));
                 }
         } else {
-                CK(c->d_cand.ensure(std::max<size_t>(8, candTotal * 8)));
+                CK(c->d_cand.ensure(std::max<size_t>(8, plan.cand_total * 8)));
                 CK(c->d_topk_docids.ensure(size_t(nq) * k * 4));
                 CK(c->d_topk_scores.ensure(size_t(nq) * k * 4));
                 CK(c->d_topk_counts.ensure(size_t(nq) * 4));
         }
-        const uint32_t nflat = uint32_t(fqs.size());
+        const uint32_t nflat = uint32_t(plan.flat.size());
         if (nflat) {
-                CK(c->d_fq.ensure(fqs.size() * sizeof(FlatQuery)));
-                CK(c->d_leaves.ensure(leaves.size() * sizeof(FlatLeaf)));
-                CK(c->d_luts.ensure(leaves.size() * 64 * sizeof(float)));
-                CK(cudaMemcpyAsync(c->d_fq.p, fqs.data(), fqs.size() * sizeof(FlatQuery), cudaMemcpyHostToDevice, c->stream));
-                CK(cudaMemcpyAsync(c->d_leaves.p, leaves.data(), leaves.size() * sizeof(FlatLeaf), cudaMemcpyHostToDevice, c->stream));
+                CK(c->d_fq.ensure(plan.flat.size() * sizeof(FlatQuery)));
+                CK(c->d_leaves.ensure(plan.leaves.size() * sizeof(FlatLeaf)));
+                CK(c->d_luts.ensure(plan.leaves.size() * 64 * sizeof(float)));
+                CK(cudaMemcpyAsync(c->d_fq.p, plan.flat.data(), plan.flat.size() * sizeof(FlatQuery), cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(c->d_leaves.p, plan.leaves.data(), plan.leaves.size() * sizeof(FlatLeaf), cudaMemcpyHostToDevice, c->stream));
         }
         uint8_t *small        = c->d_small[set].as<uint8_t>();
         auto *   ticket       = reinterpret_cast<uint32_t *>(small);
@@ -2061,11 +542,11 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 auto &qi = c->qitems_set[set];
                 qi.resize(nq);
                 for (uint32_t q = 0; q < nq; ++q) {
-                        const DevQuery &dq = hq[q];
-                        qi[q] = trn_qitems{dq.item_base, dq.ntiles, dq.tile_lo, dq.flat == 5u ? c->tree_shift : execShift};
+                        const DevQuery &dq = plan.queries[q];
+                        qi[q] = trn_qitems{dq.item_base, dq.ntiles, dq.tile_lo, dq.route == TRN_ROUTE_FLAT_TREE ? c->pc.tree_shift : execShift};
                 }
         }
-        CK(cudaMemcpyAsync(c->d_queries.p, hq.data(), nq * sizeof(DevQuery), cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(c->d_queries.p, plan.queries.data(), nq * sizeof(DevQuery), cudaMemcpyHostToDevice, c->stream));
         if (!steps.empty())
                 CK(cudaMemcpyAsync(c->d_steps.p, steps.data(), steps.size() * sizeof(DevStep), cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemsetAsync(small, 0, smallBytes, c->stream));
@@ -2077,11 +558,11 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         P.steps        = c->d_steps.as<DevStep>();
         P.nq           = nq;
         P.total_items  = totalItems;
-        P.gen_items    = uint32_t(genItems);
-        P.has_phrase   = anyPhrase ? 1u : 0u;
-        P.nslots       = maxSlots;
+        P.gen_items    = uint32_t(plan.gen_items);
+        P.has_phrase   = plan.any_phrase ? 1u : 0u;
+        P.nslots       = plan.nslots;
         P.exec_shift   = execShift;
-        P.stage_bytes  = exec_stage_bytes(c->codec);
+        P.stage_bytes  = exec_stage_bytes(c->pc.codec);
         P.docs_stage_bytes = exec_docs_stage_bytes();
         P.mode         = mode;
         P.k            = k;
@@ -2103,9 +584,9 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         uint32_t launches{0};
         if (totalItems) {
                 const bool     warpKernel = !scored;
-                const uint64_t ownItems   = genItems; // tickets of the step-program launch
+                const uint64_t ownItems   = plan.gen_items; // tickets of the step-program launch
                 CK(cudaEventRecord(k0, c->stream));
-                if (nflat && flatItems) {
+                if (nflat && plan.flat_items) {
                         // flat scored disjunctions: per-leaf BM25 tables once per batch, then k_score_flat
                         ScoreParams S;
                         std::memset(&S, 0, sizeof(S));
@@ -2114,9 +595,9 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         S.leaves       = c->d_leaves.as<FlatLeaf>();
                         S.luts         = c->d_luts.as<float>();
                         S.nflat        = nflat;
-                        S.run_tiles    = c->run_tiles;
-                        S.total_items  = mode == TRN_MODE_SCORED_TOPK ? uint32_t(std::min<uint64_t>(uint64_t(maxRuns) * nflat, 0xffffffffull)) : uint32_t(flatItems);
-                        S.tile_shift   = c->scored_shift;
+                        S.run_tiles    = c->pc.run_tiles;
+                        S.total_items  = mode == TRN_MODE_SCORED_TOPK ? uint32_t(std::min<uint64_t>(uint64_t(plan.max_runs) * nflat, 0xffffffffull)) : uint32_t(plan.flat_items);
+                        S.tile_shift   = c->pc.scored_shift;
                         S.mode         = mode;
                         S.k            = k;
                         S.ticket       = reinterpret_cast<uint32_t *>(small + 4);
@@ -2131,14 +612,12 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         S.item_off     = P.item_off;
                         S.item_cnt     = P.item_cnt;
                         S.overflow     = overflow;
-                        if (uint64_t(maxRuns) * nflat >= (1ull << 32))
-                                return fail(c, TRN_ERR_CAPACITY, "batch has more than 2^32 (run, query) work items; split it");
-                        CK(launch_build_luts(S.leaves, uint32_t(leaves.size()), c->d_luts.as<float>(), c->stream));
+                        CK(launch_build_luts(S.leaves, uint32_t(plan.leaves.size()), c->d_luts.as<float>(), c->stream));
                         CK(launch_score_flat(S, c->flat_threads, c->num_sms, c->stream));
                         launches += 2;
                 }
                 if (ownItems) {
-                        const int perSM = warpKernel ? exec_docs_max_ctas_per_sm(execShift, maxSlots, exec_docs_stage_bytes(), false, c->codec == TRN_CODEC_LUCENE) : exec_max_ctas_per_sm(execShift, maxSlots, mode, c->codec);
+                        const int perSM = warpKernel ? exec_docs_max_ctas_per_sm(execShift, plan.nslots, exec_docs_stage_bytes(), false, c->pc.codec == TRN_CODEC_LUCENE) : exec_max_ctas_per_sm(execShift, plan.nslots, mode, c->pc.codec);
                         if (perSM <= 0)
                                 return fail(c, TRN_ERR_CUDA, "the exec kernel does not fit on an SM with this many docset slots");
                         const uint64_t workers = warpKernel ? (ownItems + 3) / 4 : ownItems; // 4 warp-workers per CTA
@@ -2149,17 +628,17 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                                 CK(launch_exec_tiles(P, grid, c->stream));
                         ++launches;
                 }
-                if (warpKernel && genItems2) { // flat-tree plans: same kernel, own tile size / slot count / ticket space
+                if (warpKernel && plan.gen_items2) { // flat-tree plans: same kernel, own tile size / slot count / ticket space
                         ExecParams P2 = P;
-                        P2.exec_shift = c->tree_shift;
-                        P2.nslots     = treeSlots;
-                        P2.gen_items  = uint32_t(genItems2);
+                        P2.exec_shift = c->pc.tree_shift;
+                        P2.nslots     = plan.tree_slots;
+                        P2.gen_items  = uint32_t(plan.gen_items2);
                         P2.gen_sel    = 1;
                         P2.ticket     = reinterpret_cast<uint32_t *>(small + 4);
                         const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true);
                         if (perSM <= 0)
                                 return fail(c, TRN_ERR_CUDA, "the flat-tree launch does not fit on an SM with this many docset slots");
-                        const int grid = int(std::min<uint64_t>(uint64_t(c->num_sms) * perSM, std::max<uint64_t>(1, (genItems2 + 3) / 4)));
+                        const int grid = int(std::min<uint64_t>(uint64_t(c->num_sms) * perSM, std::max<uint64_t>(1, (plan.gen_items2 + 3) / 4)));
                         CK(launch_exec_docs(P2, grid, c->stream));
                         ++launches;
                 }
@@ -2189,15 +668,17 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         c->last_nq       = nq;
         c->last_k        = k;
         c->last_launches = launches;
-        c->last_postings = postings;
-        c->last_bytes    = bytes;
+        c->last_postings = plan.postings;
+        c->last_bytes    = plan.bytes;
         if (out) {
                 std::memset(out, 0, sizeof(*out));
                 out->nq                  = nq;
-                out->postings_scanned    = postings;
-                out->index_bytes_touched = bytes;
+                out->postings_scanned    = plan.postings;
+                out->index_bytes_touched = plan.bytes;
                 out->kernel_launches     = launches;
         }
+        for (uint32_t q = 0; q < nq; ++q)
+                routes[q] = uint8_t(plan.queries[q].route);
         return TRN_OK;
 }
 
@@ -2210,11 +691,12 @@ extern "C" int trn_exec_batch_device(trn_ctx *c, const trn_query *queries, uint3
         c->last_routes.clear();
         const double t0       = now_ms();
         CK(cudaEventRecord(c->ev0, c->stream));
-        const int r = exec_device_impl(c, queries, nq, mode, k, out, 0, c->evk0, c->evk1);
+        std::vector<uint8_t> routes(nq);
+        const int            r = exec_device_impl(c, queries, nq, mode, k, out, 0, c->evk0, c->evk1, routes.data());
         c->tm.total_ms = float(now_ms() - t0);
         if (r != TRN_OK)
                 return r;
-        c->last_routes = c->call_routes;
+        c->last_routes = std::move(routes);
         CK(cudaEventRecord(c->ev1, c->stream));
         return TRN_OK;
 }
@@ -2463,7 +945,7 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
                 if (i >= 2)
                         CK(cudaStreamWaitEvent(c->stream, c->ev_d2h[set], 0)); // the set's previous results have left the device
                 trn_result part;
-                const int  r = exec_device_impl(c, queries + ch[i].q0, ch[i].n, mode, k, &part, set, c->ev_ck0[i % 16], c->ev_ck1[i % 16]);
+                const int  r = exec_device_impl(c, queries + ch[i].q0, ch[i].n, mode, k, &part, set, c->ev_ck0[i % 16], c->ev_ck1[i % 16], routes.data() + ch[i].q0);
                 if (r == TRN_ERR_CAPACITY && ch[i].n > 1) {
                         // the upper bound of this chunk's matches does not fit the device: halve it and retry (nothing was launched)
                         const Chunk a{ch[i].q0, ch[i].n / 2}, b{ch[i].q0 + ch[i].n / 2, ch[i].n - ch[i].n / 2};
@@ -2474,7 +956,6 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
                 }
                 if (r != TRN_OK)
                         return r;
-                std::copy(c->call_routes.begin(), c->call_routes.end(), routes.begin() + ch[i].q0);
                 CK(cudaEventRecord(c->ev_done[set], c->stream));
                 if (compact) {
                         if (chunkItems.size() <= i) {
@@ -2549,6 +1030,42 @@ extern "C" int trn_debug_last_routes(trn_ctx *c, uint8_t *out, uint32_t cap, uin
                 return fail(c, TRN_ERR_CAPACITY, "trn_debug_last_routes: buffer too small");
         if (*n)
                 std::memcpy(out, c->last_routes.data(), *n);
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                              const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap) {
+        auto seterr = [&](const std::string &m, int rc) {
+                if (err && errcap) {
+                        std::strncpy(err, m.c_str(), errcap - 1);
+                        err[errcap - 1] = 0;
+                }
+                return rc;
+        };
+        if (!index || !terms || !queries || !nq || !routes || !nslots || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || mode < 0 || mode > 3)
+                return seterr("bad arguments", TRN_ERR_ARG);
+        BlockDirectory       dir;
+        std::vector<DevTerm> ht;
+        try {
+                build_directory(codec, index, nbytes, terms, nterms, 1, dir);
+                ht = dev_terms(dir, terms, nterms);
+        } catch (const std::exception &e) {
+                return seterr(e.what(), TRN_ERR_FORMAT);
+        }
+        PlanConfig pc   = initial_plan_config();
+        pc.codec        = codec;
+        pc.allow_phrase = codec == TRN_CODEC_GOOGLE;
+        docid_span(ht, pc.min_docid, max_docid);
+        pc.max_docid = max_docid;
+        BatchPlan   plan;
+        std::string perr;
+        const int   rc = plan_batch(pc, ht, queries, nq, mode, k, plan, perr);
+        if (rc != TRN_OK)
+                return seterr(perr, rc);
+        for (uint32_t q = 0; q < nq; ++q)
+                routes[q] = uint8_t(plan.queries[q].route);
+        nslots[0] = plan.nslots;
+        nslots[1] = plan.tree_slots;
         return TRN_OK;
 }
 
@@ -2725,7 +1242,7 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
         // TRN_DECODE_KERNEL=legacy | single-pass: the round-1 kernels (register-staged span copy / cp.async lane gather), kept for A/B runs;
         // default: the bulk-copy streaming kernels of decode_stream.cuh
         static const std::string decodeKernel = getenv("TRN_DECODE_KERNEL") ? getenv("TRN_DECODE_KERNEL") : "";
-        const bool               legacyDecode = (decodeKernel == "legacy" || decodeKernel == "single-pass") && c->block_docs == (c->codec == TRN_CODEC_GOOGLE ? 32u : 128u);
+        const bool               legacyDecode = (decodeKernel == "legacy" || decodeKernel == "single-pass") && c->block_docs == (c->pc.codec == TRN_CODEC_GOOGLE ? 32u : 128u);
         std::vector<uint32_t> unit_base(nterms + 1);
         std::vector<uint64_t> out_base(nterms + 1), host_base(nterms + 1);
         uint64_t              units{0}, posts{0}, padded{0};
@@ -2736,7 +1253,7 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                 unit_base[i]  = uint32_t(units);
                 out_base[i]   = padded; // device rows start on a 128-entry boundary (16-byte vector stores)
                 host_base[i]  = posts;
-                units += (legacyDecode && c->codec == TRN_CODEC_LUCENE) ? t.nblocks : (t.nblocks + 31) / 32;
+                units += (legacyDecode && c->pc.codec == TRN_CODEC_LUCENE) ? t.nblocks : (t.nblocks + 31) / 32;
                 posts += t.documents;
                 padded += (uint64_t(t.documents) + 127) / 128 * 128;
                 if (units >= (1ull << 32))
@@ -2756,8 +1273,8 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                                 D.cnt         = std::min(32u, t.nblocks - g0);
                                 D.term_start  = g0 == 0;
                                 const uint32_t lastN = t.documents - bd * (t.nblocks - 1u); // documents of the term's last block
-                                D.last_n      = (g0 + D.cnt == t.nblocks && (c->codec == TRN_CODEC_GOOGLE ? true : lastN != bd)) ? lastN : 0u;
-                                if (c->codec == TRN_CODEC_LUCENE && (t.documents & 127u) == 0u)
+                                D.last_n      = (g0 + D.cnt == t.nblocks && (c->pc.codec == TRN_CODEC_GOOGLE ? true : lastN != bd)) ? lastN : 0u;
+                                if (c->pc.codec == TRN_CODEC_LUCENE && (t.documents & 127u) == 0u)
                                         D.last_n = 0;
                                 D.ti   = i;
                                 D.g0   = g0;
@@ -2791,7 +1308,7 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                         CK(launch_decode_stream(dev_index(c), c->d_dec_units.as<DecUnit>(), c->d_dec_c.as<uint64_t>(), uint32_t(units),
                                                 materialise ? c->d_dec_docids.as<uint32_t>() : nullptr, materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr,
                                                 c->d_dec_sums.as<unsigned long long>(), c->num_sms, c->stream));
-                else if (c->codec == TRN_CODEC_GOOGLE && (materialise || forceNew))
+                else if (c->pc.codec == TRN_CODEC_GOOGLE && (materialise || forceNew))
                         CK(launch_decode_google(dev_index(c), c->d_dec_a.as<uint32_t>(), c->d_dec_b.as<uint32_t>(), c->d_dec_c.as<uint64_t>(), nterms,
                                                 uint32_t(units), materialise ? c->d_dec_docids.as<uint32_t>() : nullptr,
                                                 materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr, c->d_dec_sums.as<unsigned long long>(), grid, c->stream));

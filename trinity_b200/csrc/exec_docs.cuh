@@ -2,7 +2,7 @@
 //
 // A work item is a (query, docID tile) pair for the bitmap paths (general step programs here, all-term conjunctions / disjunctions in
 // exec_docs_flat.cuh) or a 32-block group of a lead term for the candidate-driven path (exec_docs_cand.cuh); the host picks the path
-// per query (engine.cu, exec_device_impl).
+// per query (planner.cpp, plan_batch: DevQuery::route).
 //
 // Why a second kernel: the ncu capture of the CTA-per-tile kernel on the 2-term AND workload showed DRAM far from
 // peak, low issue utilisation and half of all stall samples on CTA barriers — 4 warps waiting for the slowest lane-serial block
@@ -618,7 +618,7 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 }
                 const uint32_t item = Q.item_base + (gitem - qgen); // batch-wide (query, tile) item: index of the segment arrays
                 if constexpr (!TREE && !LUC) {
-                        if (Q.flat == 3u) { // candidate-driven conjunction: the work item is a 32-block group of the lead term
+                        if (Q.route == TRN_ROUTE_CANDIDATE) { // candidate-driven conjunction: the work item is a 32-block group of the lead term
                                 __syncwarp();
                                 cand_exec_google(P, Q, curq, item, item - Q.item_base, slots, lane);
                                 continue;
@@ -630,7 +630,7 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 int            handled = 0;
                 if constexpr (TREE) { // flat-tree plan: its leaves in (at most) two decode passes, then its slot operations
                         handled = tree_exec_google(P, Q, TS, lo, W, NW, slots, stage, lane) ? 2 : 1;
-                } else if (!LUC && Q.flat)
+                } else if (!LUC && Q.route != TRN_ROUTE_STEPS) // (the flat AND / OR plans: the other routes never reach this launch)
                         handled = flat_exec_google(P, Q, lo, W, NW, slots, stage, lane);
                 if (handled == 2)
                         dead = true;

@@ -22,7 +22,7 @@ struct FlatLane { // per-lane description of one (term, block) work unit
 
 // returns 0 = not applicable (use the step program), 1 = handled (root docset in slot Q.root_slot), 2 = handled, result empty
 __device__ int flat_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t lo, uint32_t W, uint32_t NW, uint32_t *slots, uint8_t *stage, int lane) {
-        const bool isAnd = Q.flat == 1u;
+        const bool isAnd = Q.route == TRN_ROUTE_FLAT_AND;
         // lane j adopts the j-th leaf of the plan
         uint32_t nleaf = 0, myTerm = kEmptyTerm;
         for (uint32_t si = 0; si < Q.nsteps; ++si) {
@@ -180,7 +180,7 @@ __device__ void google_leaf_own(const DevIndex &ix, const DevTerm &T, uint32_t b
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------------
-// Flat-tree plans (DevQuery::flat == 5): a DocumentsOnly tree that is neither an all-term run nor candidate-driven.  The host puts one
+// Flat-tree plans (DevQuery::route == TRN_ROUTE_FLAT_TREE): a DocumentsOnly tree that is neither an all-term run nor candidate-driven.  The host puts one
 // [OP_LEAF M_NONE dst = j] marker per leaf at the front of the program (leaf j owns bitmap slot j) and turns the rest into slot operations.
 // Per tile: ONE flat (leaf, block) pass decodes every leaf's blocks into its own bitmap with the plain-store word builder (lanes packed
 // across leaves: the per-leaf groups of the step-program path ran at a third of the lanes), then the slot operations run as
@@ -237,7 +237,7 @@ __device__ void tree_load(const ExecParams &P, const DevQuery &Q, TreeState &S, 
 }
 
 // returns true when the plan's F_BREAK_IF_EMPTY fired (the tile matches nothing); else the root docset is in slot Q.root_slot.
-// Two decode passes (engine.cu: flat_tree_masks): pass 0 decodes the first-pass leaves and runs the mask section; pass 1 decodes, of the
+// Two decode passes (planner.cpp: flat_tree_masks): pass 0 decodes the first-pass leaves and runs the mask section; pass 1 decodes, of the
 // masked leaves, only the blocks whose docID range holds a set bit of their mask bitmap, and runs the plan's own slot operations.
 __device__ bool tree_exec_google(const ExecParams &P, const DevQuery &Q, const TreeState &S, uint32_t lo, uint32_t W, uint32_t NW, uint32_t *slots, uint8_t *stage, int lane) {
         const uint32_t nleaf = S.nleaf;

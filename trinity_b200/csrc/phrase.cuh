@@ -1,7 +1,7 @@
 // Positions on the device (SURVEY.md 8f row 3) — GOOGLE codec: the inline hit streams of google_codec.cpp:533-594 (materialize_hits) and
 // Phrase::consider_phrase_match (docset_iterators.cpp:66-158).  (Included by kernels.cu.)
 //
-// A phrase node "t0 t1 ... t(k-1)" is compiled (engine.cu, Compiler::phrase_leaf) into
+// A phrase node "t0 t1 ... t(k-1)" is compiled (planner.cpp, Compiler::phrase_leaf) into
 //     [OP_LEAF SET t(a) -> s] [OP_LEAF AND t(b) -> s] ...     the conjunction of its distinct terms: the documents that CAN match
 //     [OP_PHRASE mode = k, dst = s, idf = sum of the terms' idf] [OP_ARG ...]       the position check, in place, over the survivors
 // so the docset part runs on the existing leaf decoders (incl. their block skipping), and only the surviving candidates pay for positions.
