@@ -220,6 +220,10 @@ typedef struct trn_index_info {
         int      codec;
         uint32_t nterms, max_docid, tile_docs, ntiles, block_docs;
         uint64_t index_bytes, directory_bytes, total_blocks, total_postings;
+        /* resident docID bitmaps of the dense terms (GOOGLE; trn_debug_dense_terms): how many terms have one and their bytes in HBM.  Not
+         * counted in directory_bytes.  0 when TRN_DENSE_BITMAPS=0, for LUCENE sources, or when the upload could not allocate them
+         * (trn_last_error then says so; the upload itself succeeds). */
+        uint64_t dense_terms, dense_bitmap_bytes;
 } trn_index_info;
 int trn_index_info_get(trn_ctx *, trn_index_info *out);
 
@@ -326,6 +330,18 @@ int trn_debug_last_routes(trn_ctx *, uint8_t *out, uint32_t cap, uint32_t *n);
  * flat-tree launch of k_exec_docs.  LUCENE phrase plans are refused as on a context without trn_upload_hits. */
 int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
                    uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap);
+
+/* Host-only view of the dense-term selection (tests, tooling; no GPU needed): the terms trn_upload_index would keep a resident docID
+ * bitmap for on a context that trn_create made with this environment (TRN_DENSE_BITMAPS, TRN_DENSE_BUDGET).  A GOOGLE term qualifies when
+ * its bitmap — one bit per docID of its own span, both ends aligned to 2^17 docIDs — is no larger than its chunk; qualifying terms are
+ * taken densest first while the bitmaps fit into the budget (default: 25 % of the index bytes).  offsets[0..nterms) receives every term's
+ * first 32-bit word in the bitmap array (0xffffffff: none), *nselected the number of terms with a bitmap, *bitmap_bytes their bytes. */
+int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets, uint32_t *nselected,
+                          uint64_t *bitmap_bytes, char *err, size_t errcap);
+
+/* Debug view (tests, tooling): the resident bitmap of `term` as the upload built it.  *nwords = its 32-bit words (0: the term has none),
+ * bit b of word w = docID *base + 32 w + b; the words go to out[0..cap) (TRN_ERR_CAPACITY if cap is smaller). */
+int trn_debug_dense_bitmap(trn_ctx *, uint32_t term, uint32_t *out, uint64_t cap, uint64_t *base, uint64_t *nwords);
 
 /* Split form used by bench.py / multi-GPU: run on device only, results stay in HBM ... */
 int trn_exec_batch_device(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out_counts_only);

@@ -21,6 +21,7 @@ NODE_TERM, NODE_AND, NODE_OR, NODE_NOT, NODE_OPTIONAL, NODE_SOME, NODE_PHRASE = 
 # the path a query ran (GpuIndexSource.last_routes, == TRN_ROUTE_* of include/trinity_b200.h)
 ROUTE_STEPS, ROUTE_FLAT_AND, ROUTE_FLAT_OR, ROUTE_CANDIDATE, ROUTE_SCORE_FLAT, ROUTE_FLAT_TREE, ROUTE_EXEC_TILES = 0, 1, 2, 3, 4, 5, 6
 EMPTY_TERM = 0xFFFFFFFF
+DENSE_NONE = 0xFFFFFFFF  # debug_dense_terms: the term has no resident bitmap
 DOC_IDS_END = 0xFFFFFFFF  # DocIDsEND, common.h:43
 
 
@@ -291,6 +292,22 @@ def debug_plan(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequen
     return routes[: len(queries)].copy(), (int(slots[0]), int(slots[1]))
 
 
+def debug_dense_terms(codec: int, index: np.ndarray, terms: np.ndarray):
+    """(offsets, bitmap_bytes): the first 32-bit word of every term's resident docID bitmap (DENSE_NONE: none) and the bytes of all of them,
+    selected on the host as a GpuIndexSource created with this environment would on upload (no GPU needed)"""
+    index = np.ascontiguousarray(index, dtype=np.uint8)
+    terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)
+    off = np.zeros(max(len(terms), 1), np.uint32)
+    n, nbytes = C.c_uint32(), C.c_uint64()
+    err = C.create_string_buffer(256)
+    rc = lib().trn_debug_dense_terms(codec, _ptr(index), index.size, _ptr(terms), len(terms), _ptr(off), C.byref(n), C.byref(nbytes), err, 256)
+    if rc != 0:
+        raise TrinityError(err.value.decode("utf-8", "replace") or f"rc={rc}")
+    off = off[: len(terms)].copy()
+    assert int(np.count_nonzero(off != DENSE_NONE)) == n.value
+    return off, int(nbytes.value)
+
+
 def bm25_idf(doc_freq: int, docs_cnt: int) -> float:
     return float(lib().trn_bm25_idf(doc_freq, docs_cnt))
 
@@ -473,6 +490,17 @@ class GpuIndexSource:
         t = TrnTimings()
         self._ck(self._L.trn_last_timings(self._h, C.byref(t)))
         return {n: float(getattr(t, n)) for n, _ in TrnTimings._fields_}
+
+    def dense_bitmap(self, term: int):
+        """debug: (base docID, words) of the term's resident bitmap as the upload built it (bit b of word w = docID base + 32 w + b), or None"""
+        base, n = C.c_uint64(), C.c_uint64()
+        rc = self._L.trn_debug_dense_bitmap(self._h, term, None, 0, C.byref(base), C.byref(n))  # sizes it (TRN_ERR_CAPACITY when it exists)
+        if n.value == 0:
+            self._ck(rc)
+            return None
+        out = np.zeros(n.value, np.uint32)
+        self._ck(self._L.trn_debug_dense_bitmap(self._h, term, _ptr(out), n.value, C.byref(base), C.byref(n)))
+        return int(base.value), out
 
     def last_routes(self) -> np.ndarray:
         """debug: the path (ROUTE_*) every query of the last exec_batch / exec_batch_device call ran"""

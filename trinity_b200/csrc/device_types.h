@@ -9,6 +9,9 @@ namespace trn {
 struct HitTerm;
 
 static constexpr uint32_t kEmptyTerm = 0xffffffffu;
+// resident bitmaps of dense terms (DevIndex::dense): both ends of a term's bitmap aligned to 2^17 docIDs, the largest k_exec_docs tile
+static constexpr uint32_t kDenseAlignShift = 17;
+static constexpr uint32_t kDenseNone       = 0xffffffffu;
 
 // one per dictionary term (36 B)
 struct DevTerm {
@@ -44,6 +47,10 @@ struct DevIndex {
         const uint32_t *hit_base; // parallel to blk_last: hits of the term's documents before the block
         const uint32_t *hblk_off; // per term: byte offsets of its 128-hit blocks in hits.data, then of its varbyte tail, then the end
         const struct HitTerm *hit_term; // per term: {first entry in hblk_off, sumHits} (hitcursor.h)
+        // resident docID bitmaps of dense GOOGLE terms (planner.h select_dense_terms; null when the source has none): term t's bitmap starts
+        // at word dense_off[t] of `dense` (kDenseNone: no bitmap) and covers docIDs from first_doc rounded down to 2^kDenseAlignShift
+        const uint32_t *dense;
+        const uint32_t *dense_off;
 };
 
 // ---- per-query step program (built on the host from the trn_qnode tree) ----

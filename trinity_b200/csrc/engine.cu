@@ -96,6 +96,10 @@ struct trn_ctx {
         uint64_t             index_bytes{0}, dir_bytes{0}, total_blocks{0}, total_postings{0};
         DevBuf               d_index, d_blk_last, d_blk_off, d_terms, d_tile_first, d_masked;
         bool                 have_masked{false};
+        DevBuf               d_dense, d_dense_off; // resident bitmaps of the dense terms (select_dense_terms) and each term's first word in them
+        uint32_t             dense_terms{0};       // terms with a bitmap (0: none, d_dense unused)
+        uint64_t             dense_bytes{0};
+        std::vector<uint32_t> h_dense_off;          // host copy of d_dense_off (trn_debug_dense_bitmap)
         std::vector<DevTerm> h_terms;
         // batch scratch (grow-only)
         DevBuf d_queries, d_steps, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
@@ -147,6 +151,8 @@ struct trn_ctx {
 static inline double now_ms() {
         return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
+
+static DevIndex dev_index(trn_ctx *c);
 
 static int fail(trn_ctx *c, int code, const std::string &m) {
         c->err = m;
@@ -222,7 +228,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_queries, &c->d_steps, &c->d_small[0], &c->d_small[1], &c->d_item_off,
+        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_a, &c->d_dec_b, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores})
@@ -255,6 +261,68 @@ extern "C" int trn_set_stream(trn_ctx *c, void *s) {
 }
 
 // =================================================================================================== upload
+// The resident docID bitmaps of the dense terms of the index just copied (select_dense_terms), built on the device from the doc-delta
+// sections: exact copies of the terms' docID sets, like the block directory.  Not being able to allocate them does not fail the upload:
+// the source then runs without them, and trn_last_error says why.
+static int upload_dense(trn_ctx *c) {
+        c->dense_terms = 0;
+        c->dense_bytes = 0;
+        c->h_dense_off.clear();
+        DenseSelection                  s;
+        std::vector<unsigned long long> prefix;
+        try {
+                s = select_dense_terms(c->pc, c->h_terms, c->index_bytes);
+                prefix.assign(s.order.size() + 1, 0ull);
+                for (size_t i = 0; i < s.order.size(); ++i)
+                        prefix[i + 1] = prefix[i] + c->h_terms[s.order[i]].nblocks;
+        } catch (const std::bad_alloc &) {
+                s = DenseSelection{};
+                c->err = "dense-term bitmaps off for this index: out of host memory";
+        }
+        DevBuf sel, pre;
+        cudaError_t e = cudaSuccess;
+        if (!s.order.empty()) {
+                e = c->d_dense.ensure(s.words * 4);
+                if (e == cudaSuccess)
+                        e = c->d_dense_off.ensure(std::max<size_t>(4, s.off.size() * 4));
+                if (e == cudaSuccess)
+                        e = sel.ensure(s.order.size() * 4);
+                if (e == cudaSuccess)
+                        e = pre.ensure(prefix.size() * 8);
+        }
+        if (s.order.empty() || e != cudaSuccess) {
+                if (e != cudaSuccess) {
+                        (void)cudaGetLastError(); // an allocation failure is not sticky: clear it
+                        c->err = std::string("dense-term bitmaps off for this index: ") + cudaGetErrorString(e);
+                }
+                c->d_dense.release();
+                c->d_dense_off.release();
+                sel.release();
+                pre.release();
+                return TRN_OK;
+        }
+        CK(cudaMemsetAsync(c->d_dense.p, 0, s.words * 4, c->stream));
+        CK(cudaMemcpyAsync(c->d_dense_off.p, s.off.data(), s.off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(sel.p, s.order.data(), s.order.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(pre.p, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, c->stream));
+        c->dense_terms = uint32_t(s.order.size()); // dev_index hands the bitmaps out from here on
+        // the launch check reads the thread's last error: drop one a failed call elsewhere left behind (e.g. trn_destroy's cudaSetDevice
+        // of a context created for a device that does not exist)
+        (void)cudaGetLastError();
+        const cudaError_t le = launch_build_dense(dev_index(c), sel.as<uint32_t>(), pre.as<unsigned long long>(), uint32_t(s.order.size()), prefix.back(),
+                                                  c->d_dense.as<uint32_t>(), c->stream);
+        const cudaError_t se = cudaStreamSynchronize(c->stream);
+        sel.release();
+        pre.release();
+        if (le != cudaSuccess || se != cudaSuccess) {
+                c->dense_terms = 0;
+                return fail(c, TRN_ERR_CUDA, std::string("building the dense-term bitmaps: ") + cudaGetErrorString(le != cudaSuccess ? le : se));
+        }
+        c->dense_bytes = s.words * 4;
+        c->h_dense_off = std::move(s.off);
+        return TRN_OK;
+}
+
 extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid) {
         if (!c || !index || !terms || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))
                 return c ? fail(c, TRN_ERR_ARG, "trn_upload_index: bad arguments") : TRN_ERR_ARG;
@@ -311,6 +379,8 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         CK(cudaStreamSynchronize(c->stream));
         c->index_bytes = nbytes;
         c->dir_bytes   = dir.bytes();
+        if (const int rc = upload_dense(c); rc != TRN_OK)
+                return rc;
         c->have_index  = true;
         c->have_hits   = false; // positions belong to the index they were uploaded for
         c->h_dir       = BlockDirectory{};
@@ -425,6 +495,8 @@ extern "C" int trn_index_info_get(trn_ctx *c, trn_index_info *o) {
         o->directory_bytes = c->dir_bytes;
         o->total_blocks    = c->total_blocks;
         o->total_postings  = c->total_postings;
+        o->dense_terms        = c->dense_terms;
+        o->dense_bitmap_bytes = c->dense_bytes;
         return TRN_OK;
 }
 
@@ -446,6 +518,8 @@ static DevIndex dev_index(trn_ctx *c) {
         ix.hit_base   = c->have_hits ? c->d_hit_base.as<uint32_t>() : nullptr;
         ix.hblk_off   = c->have_hits ? c->d_hblk_off.as<uint32_t>() : nullptr;
         ix.hit_term   = c->have_hits ? c->d_hit_term.as<HitTerm>() : nullptr;
+        ix.dense      = c->dense_terms ? c->d_dense.as<uint32_t>() : nullptr;
+        ix.dense_off  = c->dense_terms ? c->d_dense_off.as<uint32_t>() : nullptr;
         return ix;
 }
 
@@ -1066,6 +1140,53 @@ extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, 
                 routes[q] = uint8_t(plan.queries[q].route);
         nslots[0] = plan.nslots;
         nslots[1] = plan.tree_slots;
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,
+                                     uint32_t *nselected, uint64_t *bitmap_bytes, char *err, size_t errcap) {
+        auto seterr = [&](const std::string &m, int rc) {
+                if (err && errcap) {
+                        std::strncpy(err, m.c_str(), errcap - 1);
+                        err[errcap - 1] = 0;
+                }
+                return rc;
+        };
+        if (!index || !terms || (nterms && !offsets) || !nselected || !bitmap_bytes || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))
+                return seterr("bad arguments", TRN_ERR_ARG);
+        DenseSelection s;
+        try {
+                BlockDirectory dir;
+                build_directory(codec, index, nbytes, terms, nterms, 1, dir);
+                PlanConfig pc = initial_plan_config();
+                pc.codec      = codec;
+                s             = select_dense_terms(pc, dev_terms(dir, terms, nterms), nbytes);
+        } catch (const std::exception &e) {
+                return seterr(e.what(), TRN_ERR_FORMAT);
+        }
+        if (nterms)
+                std::memcpy(offsets, s.off.data(), nterms * 4);
+        *nselected    = uint32_t(s.order.size());
+        *bitmap_bytes = s.words * 4;
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_dense_bitmap(trn_ctx *c, uint32_t term, uint32_t *out, uint64_t cap, uint64_t *base, uint64_t *nwords) {
+        if (!c || !base || !nwords)
+                return TRN_ERR_ARG;
+        if (!c->have_index)
+                return fail(c, TRN_ERR_STATE, "no index uploaded");
+        if (term >= c->nterms)
+                return fail(c, TRN_ERR_ARG, "trn_debug_dense_bitmap: no such term");
+        *base   = 0;
+        *nwords = 0;
+        if (!c->dense_terms || c->h_dense_off[term] == kDenseNone)
+                return TRN_OK;
+        dense_span(c->h_terms[term], *base, *nwords);
+        if (cap < *nwords || !out)
+                return fail(c, TRN_ERR_CAPACITY, "trn_debug_dense_bitmap: buffer too small");
+        CK(cudaSetDevice(c->device));
+        CK(cudaMemcpy(out, c->d_dense.as<uint32_t>() + c->h_dense_off[term], *nwords * 4, cudaMemcpyDeviceToHost));
         return TRN_OK;
 }
 

@@ -141,9 +141,11 @@ __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_
                 }
         }
         const uint32_t nnec = Q.root_slot; // necessary terms incl. the lead
-        uint32_t mydir = 0, mynb = 0, mydocs = 0, myfirst = 0, mylast = 0, mytfb = 0, mytfbase = 0, mytfs = 32;
+        uint32_t mydir = 0, mynb = 0, mydocs = 0, myfirst = 0, mylast = 0, mytfb = 0, mytfbase = 0, mytfs = 32, mydense = kDenseNone;
         if (uint32_t(lane) < nleaf && myTerm != kEmptyTerm) {
                 const DevTerm T = P.ix.terms[myTerm];
+                if (P.ix.dense_off)
+                        mydense = __ldg(P.ix.dense_off + myTerm);
                 mydir           = T.dir_begin;
                 mynb            = T.nblocks;
                 mydocs          = T.documents;
@@ -185,6 +187,10 @@ __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_
                 const uint32_t  firstt = __shfl_sync(0xffffffffu, myfirst, int(t)), lastt = __shfl_sync(0xffffffffu, mylast, int(t));
                 const uint32_t  tfbt = __shfl_sync(0xffffffffu, mytfb, int(t)), tfbaset = __shfl_sync(0xffffffffu, mytfbase, int(t)), tfst = __shfl_sync(0xffffffffu, mytfs, int(t));
                 const uint32_t *bl = P.ix.blk_last + dirt, *bo = P.ix.blk_off + dirt;
+                // a term with a resident bitmap: the probe is one word load and a bit test
+                const uint32_t  denset = __shfl_sync(0xffffffffu, mydense, int(t));
+                const uint32_t *bmt    = denset != kDenseNone ? P.ix.dense + denset : nullptr;
+                const uint32_t  baset  = (firstt >> kDenseAlignShift) << kDenseAlignShift;
                 uint32_t        alive = 0;
                 for (uint32_t j = 0; j < rounds; ++j) {
                         const uint32_t nj = __shfl_sync(0xffffffffu, n, int(j));
@@ -194,7 +200,10 @@ __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_
                                 continue;
                         bool     hit = false, need = false;
                         uint32_t off = 0, prev = 0, nblk = 0;
-                        if (valid && nbt) {
+                        if (bmt) {
+                                if (valid && c >= firstt && c <= lastt)
+                                        hit = (__ldg(bmt + ((c - baset) >> 5)) >> (c & 31u)) & 1u;
+                        } else if (valid && nbt) {
                                 // the one block that can hold c: first block whose last document is >= c
                                 const uint32_t lo = first_block_ge(P.ix, dirt, nbt, firstt, lastt, tfbt, tfbaset, tfst, c);
                                 if (lo < nbt) {

@@ -35,7 +35,7 @@ __device__ int flat_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t
         }
         if (nleaf == 0 || nleaf > kFlatMaxLeaves || (isAnd && nleaf > P.nslots))
                 return 0;
-        uint32_t mybA = 0, mycnt = 0, mydir = 0, mynb = 0, mydocs = 0;
+        uint32_t mybA = 0, mycnt = 0, mydir = 0, mynb = 0, mydocs = 0, mydense = kDenseNone;
         if (uint32_t(lane) < nleaf && myTerm != kEmptyTerm) {
                 const DevTerm T = P.ix.terms[myTerm];
                 mydir           = T.dir_begin;
@@ -46,24 +46,40 @@ __device__ int flat_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t
                 if (a <= b) {
                         mybA  = a;
                         mycnt = b - a + 1u;
+                        // a conjunction's operand with a resident bitmap: the tile's words come from it (the tile lies inside the bitmap's span)
+                        if (isAnd && P.ix.dense_off) {
+                                const uint32_t o = __ldg(P.ix.dense_off + myTerm);
+                                if (o != kDenseNone)
+                                        mydense = o + ((lo - ((T.first_doc >> kDenseAlignShift) << kDenseAlignShift)) >> 5);
+                        }
                 }
+        }
+        unsigned dmask = 0; // conjunctions: the operands read from their bitmaps (not decoded)
+        if (isAnd) {
+                if (__ballot_sync(0xffffffffu, uint32_t(lane) < nleaf && mycnt == 0u))
+                        return 2; // an operand has no posting in this tile
+                dmask = __ballot_sync(0xffffffffu, mydense != kDenseNone);
+                if (mydense != kDenseNone)
+                        mycnt = 0;
         }
         const uint32_t incl  = warp_incl_scan(uint32_t(lane) < nleaf ? mycnt : 0u, lane);
         const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
         if (isAnd) {
-                if (__ballot_sync(0xffffffffu, uint32_t(lane) < nleaf && mycnt == 0u))
-                        return 2; // an operand has no posting in this tile
-                // rarest term (operands are sorted by df) sparse in this tile => skipping beats packing
-                const uint32_t cnt0 = __shfl_sync(0xffffffffu, mycnt, 0);
-                if (64u * cnt0 < total - cnt0)
-                        return 0;
+                // rarest decoded term (operands are sorted by df) sparse in this tile => skipping beats packing
+                const unsigned dec = ~dmask & ((2u << (nleaf - 1u)) - 1u);
+                if (dec) {
+                        const uint32_t cnt0 = __shfl_sync(0xffffffffu, mycnt, __ffs(int(dec)) - 1);
+                        if (64u * cnt0 < total - cnt0)
+                                return 0;
+                }
         } else if (total == 0u)
                 return 2;
 
         uint32_t *     root   = slots + size_t(Q.root_slot) * NW;
-        const uint32_t nclear = isAnd ? nleaf : 1u;
+        const uint32_t nclear = isAnd ? nleaf : 1u, lnw = P.exec_shift - 5u;
         for (uint32_t i = lane; i < nclear * NW; i += 32)
-                (isAnd ? slots : root)[i] = 0;
+                if (!((dmask >> (i >> lnw)) & 1u)) // (the bitmap operands' slots are never read)
+                        (isAnd ? slots : root)[i] = 0;
 
         // lane assignment of group g
         auto assign = [&](uint32_t g) {
@@ -131,12 +147,17 @@ __device__ int flat_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t
                 asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(tail_a), "r"(tail_bits) : "memory");
         __syncwarp();
         if (isAnd) {
-                // operand i lives in slot i; the root of an all-term conjunction is slot 0
-                for (uint32_t i = lane; i < NW; i += 32) {
-                        uint32_t w = slots[i];
-                        for (uint32_t k = 1; k < nleaf; ++k)
-                                w &= slots[size_t(k) * NW + i];
-                        root[i] = w;
+                // operand i lives in slot i, or in its bitmap; the root of an all-term conjunction is slot 0
+                const uint32_t NW4 = NW >> 2;
+                const uint4 *  s4  = reinterpret_cast<const uint4 *>(slots);
+                for (uint32_t i = lane; i < NW4; i += 32) {
+                        uint4 w = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
+                        for (uint32_t k = 0; k < nleaf; ++k) {
+                                const uint32_t dk = __shfl_sync(0xffffffffu, mydense, int(k));
+                                const uint4    v  = dk != kDenseNone ? __ldg(reinterpret_cast<const uint4 *>(P.ix.dense + dk) + i) : s4[size_t(k) * NW4 + i];
+                                w                 = make_uint4(w.x & v.x, w.y & v.y, w.z & v.z, w.w & v.w);
+                        }
+                        reinterpret_cast<uint4 *>(root)[i] = w;
                 }
                 __syncwarp();
         }
@@ -189,6 +210,7 @@ __device__ void google_leaf_own(const DevIndex &ix, const DevTerm &T, uint32_t b
 struct TreeState {
         uint32_t dir, nb, docs, first, last, tfb, tfbase; // lane j < nleaf: leaf j
         uint32_t tfs;                                      // bits 0-7: tf_shift; 8-12: mask slot; 16: decoded in the masked second pass
+        uint32_t dense;                                    // lane j < nleaf: first word of leaf j's resident bitmap (kDenseNone: decoded)
         uint32_t op, mop;                                  // lane k < nops / nmops: packed slot operation k of the main / mask section
         uint32_t nleaf, nops, nmops, nmasked;              // (uniform)
 };
@@ -201,6 +223,7 @@ __device__ void tree_load(const ExecParams &P, const DevQuery &Q, TreeState &S, 
         S.nleaf = S.nops = S.nmops = S.nmasked = 0;
         S.dir = S.nb = S.docs = S.first = S.last = S.tfb = S.tfbase = 0;
         S.tfs = 32;
+        S.dense = kDenseNone;
         S.op = S.mop = 0;
         uint32_t myTerm = kEmptyTerm, myMask = 0;
         for (uint32_t si = 0; si < Q.nsteps; ++si) {
@@ -232,6 +255,8 @@ __device__ void tree_load(const ExecParams &P, const DevQuery &Q, TreeState &S, 
                 S.tfb    = T.tf_begin;
                 S.tfbase = T.tf_base;
                 S.tfs    = T.tf_shift;
+                if (P.ix.dense_off)
+                        S.dense = __ldg(P.ix.dense_off + myTerm);
         }
         S.tfs |= myMask;
 }
@@ -257,9 +282,20 @@ __device__ bool tree_exec_google(const ExecParams &P, const DevQuery &Q, const T
         for (uint32_t pass = 0; pass < 2u; ++pass) {
                 const bool masked = pass != 0u;
                 if (!masked || S.nmasked) {
-                        // ---- the tile's blocks of every leaf of this pass
+                        // ---- leaves of this pass with a resident bitmap: a vector copy of the tile's words (the tile lies inside the bitmap's span)
+                        const bool inTile = uint32_t(lane) < nleaf && S.nb && ((S.tfs >> 16) & 1u) == pass && lo <= S.last && lo + (W - 1u) >= S.first;
+                        for (unsigned dm = __ballot_sync(0xffffffffu, inTile && S.dense != kDenseNone); dm; dm &= dm - 1u) {
+                                const int      j  = __ffs(int(dm)) - 1;
+                                const uint32_t f  = __shfl_sync(0xffffffffu, S.first, j);
+                                const uint4 *  s4 = reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, S.dense, j) +
+                                                                                   ((lo - ((f >> kDenseAlignShift) << kDenseAlignShift)) >> 5));
+                                uint4 *d4 = reinterpret_cast<uint4 *>(slots) + size_t(j) * NW4;
+                                for (uint32_t i = lane; i < NW4; i += 32)
+                                        d4[i] = __ldg(s4 + i);
+                        }
+                        // ---- the tile's blocks of every other leaf of this pass
                         uint32_t mybA = 0, mycnt = 0;
-                        if (uint32_t(lane) < nleaf && S.nb && ((S.tfs >> 16) & 1u) == pass && lo <= S.last && lo + (W - 1u) >= S.first) {
+                        if (inTile && S.dense == kDenseNone) {
                                 const uint32_t tfs = S.tfs & 0xffu;
                                 const uint32_t a   = first_block_ge(P.ix, S.dir, S.nb, S.first, S.last, S.tfb, S.tfbase, tfs, lo);
                                 if (a < S.nb) {

@@ -1149,6 +1149,49 @@ cudaError_t launch_decode_terms(const DevIndex &ix, const uint32_t *term_ids, co
         return cudaGetLastError();
 }
 
+// Load time: the bitmaps of the dense terms (DevIndex::dense, zeroed by the caller).  One thread per block of a selected term: it walks the
+// block's doc-delta section (the deltas of documents 2..n, the block's last docID comes from the directory) and ORs one word per 32
+// docIDs it touched.  blk_prefix[s] = blocks of the selected terms before sel[s] (nsel + 1 entries).
+__global__ void __launch_bounds__(kThreads) k_build_dense(DevIndex ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel,
+                                                           unsigned long long total_blocks, uint32_t *dense) {
+        const unsigned long long g = blockIdx.x * 1ull * blockDim.x + threadIdx.x;
+        if (g >= total_blocks)
+                return;
+        uint32_t lo = 0, hi = nsel; // the selected term whose blocks hold g: blk_prefix[lo] <= g < blk_prefix[lo + 1]
+        while (hi - lo > 1u) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (blk_prefix[mid] <= g) lo = mid;
+                else hi = mid;
+        }
+        const uint32_t  t = sel[lo], b = uint32_t(g - blk_prefix[lo]);
+        const DevTerm   T = ix.terms[t];
+        const uint32_t *bl = ix.blk_last + T.dir_begin;
+        const uint32_t  base = (T.first_doc >> kDenseAlignShift) << kDenseAlignShift;
+        uint32_t *      bm   = dense + ix.dense_off[t];
+        const uint32_t  n    = (b + 1u == T.nblocks) ? (T.documents - 32u * (T.nblocks - 1u)) : 32u;
+        const uint8_t * p    = ix.index + ix.blk_off[T.dir_begin + b];
+        uint32_t        doc = b ? bl[b - 1] : 0u, cw = 0xffffffffu, cur = 0;
+        for (uint32_t i = 0; i < n; ++i) {
+                doc               = i + 1u < n ? doc + varbyte_get(p) : bl[b];
+                const uint32_t w  = (doc - base) >> 5;
+                if (w != cw && cur)
+                        atomicOr(bm + cw, cur);
+                cur = (w != cw ? 0u : cur) | (1u << (doc & 31u));
+                cw  = w;
+        }
+        if (cur)
+                atomicOr(bm + cw, cur);
+}
+
+cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
+                               uint32_t *dense, cudaStream_t stream) {
+        if (!total_blocks)
+                return cudaSuccess;
+        const unsigned grid = unsigned((total_blocks + kThreads - 1) / kThreads);
+        k_build_dense<<<grid, kThreads, 0, stream>>>(ix, sel, blk_prefix, nsel, total_blocks, dense);
+        return cudaGetLastError();
+}
+
 uint32_t kernel_max_k() {
         return kMaxK;
 }

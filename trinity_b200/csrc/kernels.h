@@ -36,4 +36,6 @@ cudaError_t launch_enc_google_sizes(const EncParams &E, cudaStream_t stream);
 cudaError_t launch_enc_term_sizes(const EncParams &E, unsigned long long *chunk_bytes, cudaStream_t stream);
 cudaError_t launch_enc_google_write(const EncParams &E, cudaStream_t stream);
 uint32_t    kernel_max_k();
+cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
+                               uint32_t *dense, cudaStream_t stream);
 } // namespace trn

@@ -1211,7 +1211,46 @@ PlanConfig trn::plan_config_from_env() {
                 if (v == 13 || v == 14)
                         pc.scored_shift = uint32_t(v);
         }
+        if (const char *e = getenv("TRN_DENSE_BITMAPS"))
+                pc.dense_bitmaps = atoi(e) != 0;
+        if (const char *e = getenv("TRN_DENSE_BUDGET")) {
+                const double v = atof(e);
+                if (v >= 0.0 && v <= 1.0)
+                        pc.dense_budget = v;
+        }
         return pc;
+}
+
+void trn::dense_span(const DevTerm &T, uint64_t &base, uint64_t &words) {
+        base             = (uint64_t(T.first_doc) >> kDenseAlignShift) << kDenseAlignShift;
+        const uint64_t e = ((uint64_t(T.last_doc) >> kDenseAlignShift) + 1) << kDenseAlignShift; // 2^32 for a term in the top tile
+        words            = (e - base) >> 5;
+}
+
+trn::DenseSelection trn::select_dense_terms(const PlanConfig &cfg, const std::vector<DevTerm> &terms, uint64_t index_bytes) {
+        DenseSelection s;
+        s.off.assign(terms.size(), kDenseNone);
+        if (cfg.codec != TRN_CODEC_GOOGLE || !cfg.dense_bitmaps)
+                return s;
+        std::vector<uint32_t> cand;
+        for (uint32_t t = 0; t < terms.size(); ++t) {
+                uint64_t base, words;
+                dense_span(terms[t], base, words);
+                if (terms[t].nblocks && words * 4 <= terms[t].chunk_len)
+                        cand.push_back(t);
+        }
+        std::stable_sort(cand.begin(), cand.end(), [&](uint32_t a, uint32_t b) { return terms[a].documents > terms[b].documents; });
+        const double budget = cfg.dense_budget * double(index_bytes);
+        for (uint32_t t : cand) {
+                uint64_t base, words;
+                dense_span(terms[t], base, words);
+                if (double((s.words + words) * 4) > budget)
+                        break;
+                s.off[t] = uint32_t(s.words);
+                s.order.push_back(t);
+                s.words += words;
+        }
+        return s;
 }
 
 void trn::build_directory(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, int threads, BlockDirectory &dir) {

@@ -31,6 +31,8 @@ struct PlanConfig {
                                     // take resident warps from every query.)
         double   tree_mask_need{0.6}; // TRN_TREE_MASK_NEED: a leaf is decoded in the masked pass when at most this share of its blocks is expected to survive its mask
         bool     allow_phrase{false}; // the kernels execute OP_PHRASE (GOOGLE: inline hits; LUCENE: once hits.data is uploaded)
+        bool     dense_bitmaps{true}; // TRN_DENSE_BITMAPS=0: no resident docID bitmaps of dense terms (select_dense_terms)
+        double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
         // kernel limits (kernels.h)
         uint32_t score_flat_max_leaves{0};          // leaves of a k_score_flat query
         uint32_t docs_stage_bytes{0};               // per-warp staging bytes of k_exec_docs
@@ -61,6 +63,20 @@ struct BatchPlan {
 // TRN_ERR_UNSUPPORTED for a plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.
 int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &out,
                std::string &err);
+
+// Resident docID bitmaps of dense terms (GOOGLE sources; LUCENE sources get none).  A selected term owns one bitmap over its own docID
+// span, both ends aligned to 2^kDenseAlignShift docIDs — the largest tile of any k_exec_docs launch — so every tile of every launch lies
+// wholly inside the bitmap or holds none of the term's documents (kDenseAlignShift, kDenseNone: device_types.h).
+struct DenseSelection {
+        std::vector<uint32_t> off;  // per term: its first word in the bitmap array, kDenseNone when it has no bitmap
+        std::vector<uint32_t> order; // the selected terms, densest first (the order their bitmaps are laid out in)
+        uint64_t              words{0};
+};
+// first docID and 32-bit words of term T's bitmap (64-bit arithmetic: the span of a term ending at 2^32 - 2 ends at 2^32)
+void dense_span(const DevTerm &T, uint64_t &base, uint64_t &words);
+// A term qualifies when its bitmap is no larger than its chunk (chunk_len); qualifying terms are taken densest first (ties: lower term
+// id) while their bitmaps fit into cfg.dense_budget x index_bytes.  Reads the term records and the config only.
+DenseSelection select_dense_terms(const PlanConfig &cfg, const std::vector<DevTerm> &terms, uint64_t index_bytes);
 
 // the block directory of an index (throws what build_block_directory throws)
 void build_directory(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, int threads, BlockDirectory &dir);
