@@ -330,6 +330,12 @@ int trn_debug_last_routes(trn_ctx *, uint8_t *out, uint32_t cap, uint32_t *n);
  * flat-tree launch of k_exec_docs.  LUCENE phrase plans are refused as on a context without trn_upload_hits. */
 int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
                    uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap);
+/* The same plan's run-major tickets of the all-bitmap flat ANDs (TRN_ROUTE_FLAT_AND plans whose operands all have a resident bitmap; they
+ * run in front of the other tickets of the step-program launch; TRN_DENSE_RUNS=0 turns them off).  qtiles[2q], qtiles[2q + 1]: the tile_lo and
+ * ntiles of query q; *n = the number of such tickets (TRN_ERR_CAPACITY if cap is smaller), ticket t = tickets[3t .. 3t + 2]: the query, the
+ * first tile and the end tile (exclusive) it covers, all inside one 2^17-docID run. */
+int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
+                         uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n, char *err, size_t errcap);
 
 /* Host-only view of the dense-term selection (tests, tooling; no GPU needed): the terms trn_upload_index would keep a resident docID
  * bitmap for on a context that trn_create made with this environment (TRN_DENSE_BITMAPS, TRN_DENSE_BUDGET).  A GOOGLE term qualifies when

@@ -102,7 +102,7 @@ struct trn_ctx {
         std::vector<uint32_t> h_dense_off;          // host copy of d_dense_off (trn_debug_dense_bitmap)
         std::vector<DevTerm> h_terms;
         // batch scratch (grow-only)
-        DevBuf d_queries, d_steps, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
+        DevBuf d_queries, d_steps, d_dense_runs, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
             d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_a, d_dec_b, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
         PinBuf h_offsets, h_docids, h_scores, h_counts, h_small, h_chunk, h_item_desc;
         DevBuf d_hits, d_hit_base, d_hblk_off, d_hit_term; // LUCENE positions (trn_upload_hits)
@@ -228,7 +228,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_small[0], &c->d_small[1], &c->d_item_off,
+        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs,&c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_a, &c->d_dec_b, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores})
@@ -548,7 +548,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         c->pc.allow_phrase     = c->pc.codec == TRN_CODEC_GOOGLE || c->have_hits; // GOOGLE: inline hits; LUCENE: hits.data uploaded (trn_upload_hits)
         BatchPlan   plan;
         std::string perr;
-        const int   prc = plan_batch(c->pc, c->h_terms, queries, nq, mode, k, plan, perr);
+        const int   prc = plan_batch(c->pc, c->h_terms, c->dense_terms ? c->h_dense_off.data() : nullptr, queries, nq, mode, k, plan, perr);
         if (prc != TRN_OK)
                 return fail(c, prc, perr);
         c->tm.host_compile_ms += float(now_ms() - tCompile0);
@@ -623,6 +623,11 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         CK(cudaMemcpyAsync(c->d_queries.p, plan.queries.data(), nq * sizeof(DevQuery), cudaMemcpyHostToDevice, c->stream));
         if (!steps.empty())
                 CK(cudaMemcpyAsync(c->d_steps.p, steps.data(), steps.size() * sizeof(DevStep), cudaMemcpyHostToDevice, c->stream));
+        const uint32_t denseItems = uint32_t(plan.dense_runs.size());
+        if (denseItems) {
+                CK(c->d_dense_runs.ensure(size_t(denseItems) * sizeof(uint2)));
+                CK(cudaMemcpyAsync(c->d_dense_runs.p, plan.dense_runs.data(), size_t(denseItems) * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+        }
         CK(cudaMemsetAsync(small, 0, smallBytes, c->stream));
 
         ExecParams P;
@@ -633,6 +638,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         P.nq           = nq;
         P.total_items  = totalItems;
         P.gen_items    = uint32_t(plan.gen_items);
+        P.dense_runs   = denseItems ? c->d_dense_runs.as<uint2>() : nullptr;
+        P.dense_items  = denseItems;
         P.has_phrase   = plan.any_phrase ? 1u : 0u;
         P.nslots       = plan.nslots;
         P.exec_shift   = execShift;
@@ -658,7 +665,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         uint32_t launches{0};
         if (totalItems) {
                 const bool     warpKernel = !scored;
-                const uint64_t ownItems   = plan.gen_items; // tickets of the step-program launch
+                const uint64_t ownItems   = plan.gen_items + denseItems; // tickets of the step-program launch
                 CK(cudaEventRecord(k0, c->stream));
                 if (nflat && plan.flat_items) {
                         // flat scored disjunctions: per-leaf BM25 tables once per batch, then k_score_flat
@@ -708,6 +715,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         P2.nslots     = plan.tree_slots;
                         P2.gen_items  = uint32_t(plan.gen_items2);
                         P2.gen_sel    = 1;
+                        P2.dense_runs  = nullptr;
+                        P2.dense_items = 0;
                         P2.ticket     = reinterpret_cast<uint32_t *>(small + 4);
                         const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true);
                         if (perSM <= 0)
@@ -1107,8 +1116,9 @@ extern "C" int trn_debug_last_routes(trn_ctx *c, uint8_t *out, uint32_t cap, uin
         return TRN_OK;
 }
 
-extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
-                              const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap) {
+// plans a batch on the host as exec_device_impl would on a context that holds this index (trn_debug_plan, trn_debug_dense_runs)
+static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                            const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &plan, char *err, size_t errcap) {
         auto seterr = [&](const std::string &m, int rc) {
                 if (err && errcap) {
                         std::strncpy(err, m.c_str(), errcap - 1);
@@ -1116,7 +1126,7 @@ extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, 
                 }
                 return rc;
         };
-        if (!index || !terms || !queries || !nq || !routes || !nslots || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || mode < 0 || mode > 3)
+        if (!index || !terms || !queries || !nq || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || mode < 0 || mode > 3)
                 return seterr("bad arguments", TRN_ERR_ARG);
         BlockDirectory       dir;
         std::vector<DevTerm> ht;
@@ -1130,16 +1140,49 @@ extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, 
         pc.codec        = codec;
         pc.allow_phrase = codec == TRN_CODEC_GOOGLE;
         docid_span(ht, pc.min_docid, max_docid);
-        pc.max_docid = max_docid;
-        BatchPlan   plan;
-        std::string perr;
-        const int   rc = plan_batch(pc, ht, queries, nq, mode, k, plan, perr);
-        if (rc != TRN_OK)
-                return seterr(perr, rc);
+        pc.max_docid            = max_docid;
+        const DenseSelection ds = select_dense_terms(pc, ht, nbytes); // what trn_upload_index keeps
+        std::string          perr;
+        const int            rc = plan_batch(pc, ht, ds.order.empty() ? nullptr : ds.off.data(), queries, nq, mode, k, plan, perr);
+        return rc == TRN_OK ? TRN_OK : seterr(perr, rc);
+}
+
+extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                              const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint8_t *routes, uint32_t *nslots, char *err, size_t errcap) {
+        if (!routes || !nslots)
+                return TRN_ERR_ARG;
+        BatchPlan plan;
+        if (const int rc = debug_plan_batch(codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, plan, err, errcap); rc != TRN_OK)
+                return rc;
         for (uint32_t q = 0; q < nq; ++q)
                 routes[q] = uint8_t(plan.queries[q].route);
         nslots[0] = plan.nslots;
         nslots[1] = plan.tree_slots;
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                                    const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
+                                    char *err, size_t errcap) {
+        if (!qtiles || !n)
+                return TRN_ERR_ARG;
+        BatchPlan plan;
+        if (const int rc = debug_plan_batch(codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, plan, err, errcap); rc != TRN_OK)
+                return rc;
+        for (uint32_t q = 0; q < nq; ++q) {
+                qtiles[2 * q]     = plan.queries[q].tile_lo;
+                qtiles[2 * q + 1] = plan.queries[q].ntiles;
+        }
+        *n = plan.dense_runs.size();
+        if (cap < *n)
+                return TRN_ERR_CAPACITY;
+        for (uint64_t t = 0; t < *n; ++t) {
+                const uint2     e  = plan.dense_runs[t];
+                const DevQuery &dq = plan.queries[e.x];
+                tickets[3 * t]     = e.x;
+                tickets[3 * t + 1] = e.y;
+                tickets[3 * t + 2] = dense_run_end(e.y, dq.tile_lo, dq.ntiles, plan.exec_shift);
+        }
         return TRN_OK;
 }
 

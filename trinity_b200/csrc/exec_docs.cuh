@@ -560,6 +560,207 @@ __device__ __forceinline__ void lucene_leaf_warp(const DevIndex &ix, const DevTe
                 lucene_leaf_warp_t<0>(ix, T, bA, bB, lo, hi, bs, skipfilt, stage, lane, bar_s, seq);
 }
 
+// ---- emission of a tile's root docset (a bitmap in shared memory; lane l owns words [l * NW/32, (l + 1) * NW/32))
+struct TileCount {
+        uint32_t c, incl; // the lane's documents, and those of lanes 0 .. lane
+        uint32_t total;   // the tile's documents
+        uint32_t enc;     // compact results: the encoding (kEnc*)
+        uint32_t size;    // segment size: words (compact) or docIDs
+};
+// Compact results take whichever form needs the fewest words (a tile holds at most 2^16 documents):
+//   bitmap   the tile's words                                                          dense tiles (> 1 document in 8)
+//   U8B      per 256-docID bucket a count byte, then one offset byte per document      1 in 8 .. 1 in 256
+//   U16      16-bit offsets from the tile's first docID, two per word                  sparse tiles
+// live == false: the tile matches nothing (root is not read)
+__device__ __forceinline__ TileCount tile_count(const uint32_t *root, bool live, bool compact, uint32_t W, uint32_t NW, int lane) {
+        const uint32_t wpl = NW >> 5;
+        TileCount      t;
+        uint32_t       c = 0, full = 0;
+        if (live) {
+                uint32_t cb = 0; // documents of the current 256-docID bucket (8 words): 256 of them do not fit the bucketed form's count byte
+                for (uint32_t i = 0; i < wpl; ++i) {
+                        const uint32_t pc = __popc(root[lane * wpl + i]);
+                        c += pc;
+                        cb += pc;
+                        if ((i & 7u) == 7u) {
+                                full |= cb == 256u ? 1u : 0u;
+                                cb = 0;
+                        }
+                }
+        }
+        t.c     = c;
+        t.incl  = warp_incl_scan(c, lane);
+        t.total = __shfl_sync(0xffffffffu, t.incl, 31);
+        t.enc   = kEncBitmap;
+        t.size  = t.total;
+        if (compact) {
+                const uint32_t nbk  = W >> 8;
+                const bool     u8ok = wpl >= 8u && W <= 65536u && !__any_sync(0xffffffffu, full != 0u); // a lane owns whole buckets
+                uint32_t       words = NW;
+                if (W <= 65536u) {
+                        if (((t.total + 1u) >> 1) < words)
+                                t.enc = kEncU16, words = (t.total + 1u) >> 1;
+                        if (u8ok && ((nbk + t.total + 3u) >> 2) < words)
+                                t.enc = kEncU8B, words = (nbk + t.total + 3u) >> 2;
+                }
+                t.size = t.total ? words : 0u;
+        }
+        return t;
+}
+
+// the work item's segment record (one lane); base: the reserved segment, 0 for an empty tile, ~0 when the reservation overflowed
+__device__ __forceinline__ void tile_record(const ExecParams &P, uint32_t item, const TileCount &t, unsigned long long base) {
+        P.item_off[item] = base;
+        P.item_cnt[item] = base == ~0ull ? 0u : t.size;
+        if (P.item_desc)
+                P.item_desc[item] = base == ~0ull ? 0u : (t.total | t.enc << 30);
+}
+
+// the tile's matches into its segment at `base` (t.total > 0): the compact form t.enc, or plain docIDs
+__device__ __forceinline__ void tile_emit(const ExecParams &P, const uint32_t *root, const TileCount &t, unsigned long long base, uint32_t lo, uint32_t W,
+                                          uint32_t NW, int lane) {
+        const uint32_t wpl = NW >> 5;
+        if (!P.item_desc) {
+                unsigned long long pos = base + (t.incl - t.c);
+                for (uint32_t i = 0; i < wpl; ++i) {
+                        const uint32_t wi = lane * wpl + i;
+                        uint32_t       w  = root[wi];
+                        while (w) {
+                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
+                                w &= w - 1;
+                                P.seg_docids[pos++] = lo + wi * 32u + bit;
+                        }
+                }
+        } else if (t.enc == kEncBitmap) {
+                for (uint32_t i = lane; i < NW; i += 32)
+                        P.seg_docids[base + i] = root[i];
+        } else if (t.enc == kEncU8B) {
+                const uint32_t nbk = W >> 8;
+                uint8_t *      o8  = reinterpret_cast<uint8_t *>(P.seg_docids + base);
+                uint32_t       pos = nbk + (t.incl - t.c), cb = 0;
+                for (uint32_t i = 0; i < wpl; ++i) {
+                        const uint32_t wi = lane * wpl + i;
+                        uint32_t       w  = root[wi];
+                        cb += __popc(w);
+                        while (w) {
+                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
+                                w &= w - 1;
+                                o8[pos++] = uint8_t((wi & 7u) * 32u + bit);
+                        }
+                        if ((i & 7u) == 7u) {
+                                o8[wi >> 3] = uint8_t(cb);
+                                cb          = 0;
+                        }
+                }
+                if (lane == 31)
+                        for (uint32_t z = nbk + t.total; z < t.size * 4u; ++z)
+                                o8[z] = 0; // the pad bytes travel too
+        } else {
+                uint16_t *out = reinterpret_cast<uint16_t *>(P.seg_docids + base);
+                uint32_t  pos = t.incl - t.c;
+                for (uint32_t i = 0; i < wpl; ++i) {
+                        const uint32_t wi = lane * wpl + i;
+                        uint32_t       w  = root[wi];
+                        while (w) {
+                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
+                                w &= w - 1;
+                                out[pos++] = uint16_t(wi * 32u + bit);
+                        }
+                }
+                if (lane == 31 && (t.total & 1u))
+                        out[t.total] = 0; // the pad half-word travels too
+        }
+}
+
+// All-bitmap flat AND (BatchPlan::dense_runs): ticket e = {query, first tile} covers the query's tiles of one 2^kDenseAlignShift-docID run,
+// which lies wholly inside every operand's bitmap, so nothing is decoded and no block directory is searched.  The run-major order of the
+// tickets keeps every query that reads a run's bitmap words in flight together: each run of each bitmap comes from HBM about once per batch.
+// Pass 1 ANDs each tile's words (masked documents removed) into slot 0 and sizes its result; the run's segments take ONE reservation;
+// pass 2 rebuilds each non-empty tile (its words now come from L2) and writes it exactly as the per-tile path would.
+__device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, uint32_t *root, int lane) {
+        const uint32_t q = e.x, t0 = e.y;
+        const DevQuery &Q     = P.queries[q];
+        const uint32_t  nt    = dense_run_end(t0, Q.tile_lo, Q.ntiles, P.exec_shift) - t0; // 1 .. 16 tiles
+        const uint32_t  item0 = Q.item_base + (t0 - Q.tile_lo);
+        const uint32_t  lo0   = t0 << P.exec_shift;
+        // lane k: the word of operand k's bitmap at the run's first docID
+        uint32_t nleaf = 0, myTerm = kEmptyTerm, myw = 0;
+        for (uint32_t si = 0; si < Q.nsteps; ++si) {
+                const DevStep st = P.steps[Q.step_begin + si];
+                if (st.op == OP_LEAF) {
+                        if (uint32_t(lane) == nleaf)
+                                myTerm = st.term;
+                        ++nleaf;
+                }
+        }
+        if (myTerm != kEmptyTerm) {
+                const uint32_t f = P.ix.terms[myTerm].first_doc;
+                myw              = __ldg(P.ix.dense_off + myTerm) + ((lo0 - ((f >> kDenseAlignShift) << kDenseAlignShift)) >> 5);
+        }
+        const uint32_t NW4 = NW >> 2;
+        uint4 *        r4  = reinterpret_cast<uint4 *>(root);
+        auto           build = [&](uint32_t j) { // tile j of the run into root
+                __syncwarp(); // every lane is done reading the previous tile
+                const uint4 *mk = P.ix.masked ? reinterpret_cast<const uint4 *>(P.ix.masked + ((lo0 >> 5) + j * NW)) : nullptr;
+                for (uint32_t i = lane; i < NW4; i += 32) {
+                        uint4 w = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
+                        if (mk) {
+                                const uint4 m = mk[i];
+                                w             = make_uint4(~m.x, ~m.y, ~m.z, ~m.w);
+                        }
+                        for (uint32_t k = 0; k < nleaf; ++k) {
+                                const uint4 v = __ldg(reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, myw, int(k)) + j * NW) + i);
+                                w             = make_uint4(w.x & v.x, w.y & v.y, w.z & v.z, w.w & v.w);
+                        }
+                        r4[i] = w;
+                }
+                __syncwarp();
+        };
+        const bool compact = P.item_desc != nullptr;
+        uint32_t   mydesc = 0, mysize = 0; // lane j: tile j's documents | encoding << 30 (as item_desc), and its segment size
+        for (uint32_t j = 0; j < nt; ++j) {
+                build(j);
+                const TileCount tc = tile_count(root, true, compact, W, NW, lane);
+                if (uint32_t(lane) == j) {
+                        mydesc = tc.total | tc.enc << 30;
+                        mysize = tc.size;
+                }
+        }
+        const uint32_t mytot = mydesc & 0x3fffffffu;
+        const uint32_t incl = warp_incl_scan(mysize, lane), size = __shfl_sync(0xffffffffu, incl, 31);
+        const uint32_t total = __reduce_add_sync(0xffffffffu, mytot);
+        unsigned long long base = 0;
+        if (lane == 0 && size) {
+                base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(size));
+                atomicAdd(&P.match_counts[q], static_cast<unsigned long long>(total));
+                if (compact)
+                        atomicAdd(&P.word_counts[q], static_cast<unsigned long long>(size));
+                if (base + size > P.seg_capacity) {
+                        *P.overflow = 1;
+                        base        = ~0ull;
+                }
+        }
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (uint32_t(lane) < nt) {
+                TileCount t;
+                t.total = mytot;
+                t.size  = mysize;
+                t.enc   = mydesc >> 30;
+                tile_record(P, item0 + uint32_t(lane), t, !mytot ? 0ull : base == ~0ull ? ~0ull : base + (incl - mysize));
+        }
+        if (base == ~0ull)
+                return;
+        for (uint32_t j = 0; j < nt; ++j) {
+                const uint32_t off = __shfl_sync(0xffffffffu, incl - mysize, int(j));
+                if (!__shfl_sync(0xffffffffu, mytot, int(j)))
+                        continue;
+                build(j);
+                const TileCount tc = tile_count(root, true, compact, W, NW, lane);
+                tile_emit(P, root, tc, base + off, lo0 + j * W, W, NW, lane);
+        }
+        __syncwarp();
+}
+
 #include "exec_docs_flat.cuh"
 #include "exec_docs_cand.cuh"
 
@@ -600,8 +801,15 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 if (lane == 0)
                         gitem = atomicAdd(P.ticket, 1u);
                 gitem = __shfl_sync(0xffffffffu, gitem, 0);
-                if (gitem >= P.gen_items)
+                if (gitem >= P.dense_items + P.gen_items)
                         break;
+                if constexpr (!PH && !TREE && !LUC) {
+                        if (gitem < P.dense_items) { // all-bitmap flat AND: the query's tiles of one run
+                                dense_run_exec(P, P.dense_runs[gitem], W, NW, slots, lane);
+                                continue;
+                        }
+                }
+                gitem -= P.dense_items;
                 if (curq == 0xffffffffu || gitem < qgen || gitem - qgen >= Q.ntiles) {
                         uint32_t qlo = 0, qhi = P.nq;
                         while (qhi - qlo > 1) {
@@ -806,121 +1014,25 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                         __syncwarp();
                 }
                 // ---- emission: ordered compaction of the root docset
-                uint32_t c = 0, full = 0;
                 const uint32_t *root = slots + size_t(Q.root_slot) * NW;
-                if (!dead) {
-                        uint32_t cb = 0; // documents of the current 256-docID bucket (8 words): 256 of them do not fit the bucketed form's count byte
-                        for (uint32_t i = 0; i < wpl; ++i) {
-                                const uint32_t pc = __popc(root[lane * wpl + i]);
-                                c += pc;
-                                cb += pc;
-                                if ((i & 7u) == 7u) {
-                                        full |= cb == 256u ? 1u : 0u;
-                                        cb = 0;
-                                }
-                        }
-                }
-                const uint32_t incl  = warp_incl_scan(c, lane);
-                const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+                const TileCount tc   = tile_count(root, !dead, P.item_desc != nullptr, W, NW, lane);
                 unsigned long long base = 0;
-                if (P.item_desc) {
-                        // ---- compact results, whichever form takes the fewest words (a tile holds at most 2^16 documents):
-                        //   bitmap   the tile's words                                                          dense tiles (> 1 document in 8)
-                        //   U8B      per 256-docID bucket a count byte, then one offset byte per document      1 in 8 .. 1 in 256
-                        //   U16      16-bit offsets from the tile's first docID, two per word                  sparse tiles
-                        const uint32_t nbk  = W >> 8;
-                        const bool     u8ok = wpl >= 8u && W <= 65536u && !__any_sync(0xffffffffu, full != 0u); // a lane owns whole buckets
-                        uint32_t       enc = kEncBitmap, words = NW;
-                        if (W <= 65536u) {
-                                if (((total + 1u) >> 1) < words)
-                                        enc = kEncU16, words = (total + 1u) >> 1;
-                                if (u8ok && ((nbk + total + 3u) >> 2) < words)
-                                        enc = kEncU8B, words = (nbk + total + 3u) >> 2;
-                        }
-                        if (!total)
-                                words = 0;
-                        if (lane == 0) {
-                                if (total) {
-                                        base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(words));
-                                        atomicAdd(&P.match_counts[curq], static_cast<unsigned long long>(total));
-                                        atomicAdd(&P.word_counts[curq], static_cast<unsigned long long>(words));
-                                        if (base + words > P.seg_capacity) {
-                                                *P.overflow = 1;
-                                                base        = ~0ull;
-                                        }
-                                }
-                                P.item_off[item]  = base;
-                                P.item_cnt[item]  = base == ~0ull ? 0u : words;
-                                P.item_desc[item] = base == ~0ull ? 0u : (total | enc << 30);
-                        }
-                        base = __shfl_sync(0xffffffffu, base, 0);
-                        if (total && base != ~0ull) {
-                                if (enc == kEncBitmap) {
-                                        for (uint32_t i = lane; i < NW; i += 32)
-                                                P.seg_docids[base + i] = root[i];
-                                } else if (enc == kEncU8B) {
-                                        uint8_t *o8  = reinterpret_cast<uint8_t *>(P.seg_docids + base);
-                                        uint32_t pos = nbk + (incl - c), cb = 0;
-                                        for (uint32_t i = 0; i < wpl; ++i) {
-                                                const uint32_t wi = lane * wpl + i;
-                                                uint32_t       w  = root[wi];
-                                                cb += __popc(w);
-                                                while (w) {
-                                                        const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                                        w &= w - 1;
-                                                        o8[pos++] = uint8_t((wi & 7u) * 32u + bit);
-                                                }
-                                                if ((i & 7u) == 7u) {
-                                                        o8[wi >> 3] = uint8_t(cb);
-                                                        cb          = 0;
-                                                }
-                                        }
-                                        if (lane == 31)
-                                                for (uint32_t z = nbk + total; z < words * 4u; ++z)
-                                                        o8[z] = 0; // the pad bytes travel too
-                                } else {
-                                        uint16_t *out = reinterpret_cast<uint16_t *>(P.seg_docids + base);
-                                        uint32_t  pos = incl - c;
-                                        for (uint32_t i = 0; i < wpl; ++i) {
-                                                const uint32_t wi = lane * wpl + i;
-                                                uint32_t       w  = root[wi];
-                                                while (w) {
-                                                        const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                                        w &= w - 1;
-                                                        out[pos++] = uint16_t(wi * 32u + bit);
-                                                }
-                                        }
-                                        if (lane == 31 && (total & 1u))
-                                                out[total] = 0; // the pad half-word travels too
-                                }
-                        }
-                        continue;
-                }
                 if (lane == 0) {
-                        if (total) {
-                                base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(total));
-                                atomicAdd(&P.match_counts[curq], static_cast<unsigned long long>(total));
-                                if (base + total > P.seg_capacity) {
+                        if (tc.total) {
+                                base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(tc.size));
+                                atomicAdd(&P.match_counts[curq], static_cast<unsigned long long>(tc.total));
+                                if (P.item_desc)
+                                        atomicAdd(&P.word_counts[curq], static_cast<unsigned long long>(tc.size));
+                                if (base + tc.size > P.seg_capacity) {
                                         *P.overflow = 1;
                                         base        = ~0ull;
                                 }
                         }
-                        P.item_off[item] = base;
-                        P.item_cnt[item] = base == ~0ull ? 0u : total;
+                        tile_record(P, item, tc, base);
                 }
                 base = __shfl_sync(0xffffffffu, base, 0);
-                if (total && base != ~0ull) {
-                        unsigned long long pos = base + (incl - c);
-                        for (uint32_t i = 0; i < wpl; ++i) {
-                                const uint32_t wi = lane * wpl + i;
-                                uint32_t       w  = root[wi];
-                                while (w) {
-                                        const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                        w &= w - 1;
-                                        P.seg_docids[pos++] = lo + wi * 32u + bit;
-                                }
-                        }
-                }
+                if (tc.total && base != ~0ull)
+                        tile_emit(P, root, tc, base, lo, W, NW, lane);
         }
 }
 

@@ -1218,6 +1218,8 @@ PlanConfig trn::plan_config_from_env() {
                 if (v >= 0.0 && v <= 1.0)
                         pc.dense_budget = v;
         }
+        if (const char *e = getenv("TRN_DENSE_RUNS"))
+                pc.dense_runs = atoi(e) != 0;
         return pc;
 }
 
@@ -1295,8 +1297,8 @@ static int fail(std::string &err, int code, const std::string &m) {
         return code;
 }
 
-int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &out,
-                    std::string &err) {
+int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
+                    uint32_t k, BatchPlan &out, std::string &err) {
         out                = BatchPlan{};
         const bool scored  = mode == TRN_MODE_SCORED_ALL || mode == TRN_MODE_SCORED_TOPK;
         const bool google  = cfg.codec == TRN_CODEC_GOOGLE;
@@ -1543,14 +1545,62 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                         out.nslots = std::max(out.nslots, (need - stageB + slotBytes - 1u) / slotBytes);
         }
         // a flat conjunction keeps one bitmap per operand: with more operands than the launch has slots (final only here) it runs as a
-        // step program
-        for (auto &dq : out.queries)
+        // step program.  One whose operands all have a resident bitmap decodes nothing: it joins the run-major ticket space (dense_runs) —
+        // except beside a phrase plan, whose instantiation of k_exec_docs does not carry that path.
+        const bool runs = dense_off && cfg.dense_runs && google && !scored && !out.any_phrase;
+        std::vector<uint32_t> group; // the queries of dense_runs
+        for (uint32_t q = 0; q < nq; ++q) {
+                auto &dq = out.queries[q];
                 if (dq.route == TRN_ROUTE_FLAT_AND) {
                         uint32_t nleaf{0};
-                        for (uint32_t si = 0; si < dq.nsteps; ++si)
-                                nleaf += steps[dq.step_begin + si].op == OP_LEAF;
+                        bool     dense{runs && dq.ntiles};
+                        for (uint32_t si = 0; si < dq.nsteps; ++si) {
+                                const DevStep &st = steps[dq.step_begin + si];
+                                if (st.op == OP_LEAF) {
+                                        ++nleaf;
+                                        dense = dense && st.term != kEmptyTerm && dense_off[st.term] != kDenseNone;
+                                }
+                        }
                         if (nleaf > out.nslots)
                                 dq.route = TRN_ROUTE_STEPS;
+                        else if (dense)
+                                group.push_back(q);
                 }
+        }
+        if (!group.empty()) {
+                // (run, query) pairs, counting-sorted by run (queries ascending within a run).  Every tile of such a query lies inside every
+                // operand's bitmap span (the query's range is the intersection of the operands' ranges), and so does the run that holds it.
+                const uint32_t rs = kDenseAlignShift - execShift;
+                uint32_t       r0{0xffffffffu}, r1{0};
+                for (uint32_t q : group) {
+                        const auto &dq = out.queries[q];
+                        r0             = std::min(r0, dq.tile_lo >> rs);
+                        r1             = std::max(r1, (dq.tile_lo + dq.ntiles - 1u) >> rs);
+                }
+                std::vector<uint32_t> at(size_t(r1 - r0) + 2, 0);
+                for (uint32_t q : group) {
+                        const auto &dq = out.queries[q];
+                        for (uint32_t r = dq.tile_lo >> rs; r <= (dq.tile_lo + dq.ntiles - 1u) >> rs; ++r)
+                                ++at[r - r0 + 1];
+                }
+                for (size_t i = 1; i < at.size(); ++i)
+                        at[i] += at[i - 1];
+                out.dense_runs.resize(at.back());
+                for (uint32_t q : group) {
+                        const auto &dq = out.queries[q];
+                        for (uint32_t r = dq.tile_lo >> rs; r <= (dq.tile_lo + dq.ntiles - 1u) >> rs; ++r)
+                                out.dense_runs[at[r - r0]++] = uint2{q, std::max(dq.tile_lo, r << rs)};
+                }
+                // the step-program launch's own tickets without them (the items keep their item_base)
+                out.gen_items = 0;
+                for (uint32_t q = 0, g = 0; q < nq; ++q) {
+                        auto &dq    = out.queries[q];
+                        dq.gen_base = uint32_t(out.gen_items);
+                        if (g < group.size() && group[g] == q)
+                                ++g;
+                        else if (dq.route != TRN_ROUTE_FLAT_TREE)
+                                out.gen_items += dq.ntiles;
+                }
+        }
         return TRN_OK;
 }

@@ -33,6 +33,7 @@ struct PlanConfig {
         bool     allow_phrase{false}; // the kernels execute OP_PHRASE (GOOGLE: inline hits; LUCENE: once hits.data is uploaded)
         bool     dense_bitmaps{true}; // TRN_DENSE_BITMAPS=0: no resident docID bitmaps of dense terms (select_dense_terms)
         double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
+        bool     dense_runs{true};    // TRN_DENSE_RUNS=0: all-bitmap flat ANDs take (query, tile) tickets like the other flat ANDs (BatchPlan::dense_runs)
         // kernel limits (kernels.h)
         uint32_t score_flat_max_leaves{0};          // leaves of a k_score_flat query
         uint32_t docs_stage_bytes{0};               // per-warp staging bytes of k_exec_docs
@@ -53,16 +54,20 @@ struct BatchPlan {
         uint32_t               max_runs{0};    // most runs of one k_score_flat query
         uint64_t               items{0};       // (query, tile) work items of the batch
         uint64_t               gen_items{0}, gen_items2{0}, flat_items{0}; // tickets of the step-program, flat-tree and k_score_flat launches
+        // flat ANDs whose operands all have a resident bitmap (DocumentsOnly, no phrase plan in the batch): one ticket per (query, 2^17-docID
+        // run) pair, {query, first tile} (dense_run_end: device_types.h), ordered run-major, in front of the step-program launch's gen_items
+        std::vector<uint2>     dense_runs;
         uint64_t               seg_cap{0};     // upper bound of the batch's matches (result segments)
         uint64_t               cand_total{0};  // top-k candidate entries
         uint64_t               postings{0}, bytes{0};
         bool                   any_phrase{false};
 };
 
-// Plans a batch (mode: TRN_MODE_*; k: top-k).  Returns TRN_OK, or an error code with its message in err: TRN_ERR_ARG /
-// TRN_ERR_UNSUPPORTED for a plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.
-int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &out,
-               std::string &err);
+// Plans a batch (mode: TRN_MODE_*; k: top-k).  dense_off: per term, the first word of its resident bitmap (DenseSelection::off), or
+// null when the source has none.  Returns TRN_OK, or an error code with its message in err: TRN_ERR_ARG / TRN_ERR_UNSUPPORTED for a
+// plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.
+int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
+               uint32_t k, BatchPlan &out, std::string &err);
 
 // Resident docID bitmaps of dense terms (GOOGLE sources; LUCENE sources get none).  A selected term owns one bitmap over its own docID
 // span, both ends aligned to 2^kDenseAlignShift docIDs — the largest tile of any k_exec_docs launch — so every tile of every launch lies
