@@ -383,6 +383,21 @@ int trn_encode_google(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, co
                       uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
                       float *device_ms);
 
+/* GPU-side Encoder, LUCENE layout == one fresh Codecs::Lucene::IndexSession fed begin_term / begin_document / new_hit / end_document /
+ * end_term (lucene_codec.cpp:163-388; FastPFor<4> int-blocks of 128 values, one skiplist entry per full block) for hits without
+ * payloads: index and hits.data are BUILT on the device, byte for byte what trn_builder_add_term writes for CODEC_LUCENE (the PFor
+ * byte container's padding included: zeros).  term_begin / docids / freqs / positions (HOST pointers) mean what they mean for
+ * trn_encode_google; there are no geometry parameters (blocks of 128 documents and of 128 hits, SKIPLIST_STEP = 1 per term).
+ *   index_out[index_cap]    the chunks of the terms back to back; *index_bytes their total
+ *   hits_out[hits_cap]      hits.data of the terms back to back; *hits_bytes its total (chunk headers hold the offsets into it)
+ *   terms[nterms]           the term_index_ctx tuples
+ * TRN_ERR_ARG: docID 0 / not ascending, a position 0 / decreasing / >= Limits::MaxPosition (the inputs trn_encode_google refuses).
+ * TRN_ERR_CAPACITY: a buffer too small, or an output of 4 GiB or more (u32 offsets); *index_bytes and *hits_bytes are still set.
+ * *device_ms (may be NULL): the device time of the kernels and scans, without the host<->device copies. */
+int trn_encode_lucene(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                      uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
+                      trn_term *terms, float *device_ms);
+
 #ifdef __cplusplus
 }
 #endif

@@ -570,6 +570,29 @@ class GpuIndexSource:
                                            _ptr(out), cap, C.byref(nbytes), _ptr(terms), C.byref(ms)))
         return out[:nbytes.value].copy(), terms, int(cd.value), float(ms.value)
 
+    def encode_lucene(self, lists):
+        """GPU-side Encoder (== Codecs::Lucene::Encoder, lucene_codec.cpp:163-388): builds the LUCENE index and its hits.data on the device.
+        lists: one (docids, freqs[, positions]) per term, as for encode_google.  Returns (index bytes, hits bytes, terms array, device_ms)."""
+        lists = list(lists)
+        with_pos = len(lists) > 0 and len(lists[0]) > 2 and lists[0][2] is not None
+        tb = np.zeros(len(lists) + 1, np.uint64)
+        for i, l in enumerate(lists):
+            tb[i + 1] = tb[i] + len(l[0])
+        d = np.concatenate([_u32(l[0]) for l in lists]) if lists else np.zeros(0, np.uint32)
+        f = np.concatenate([_u32(l[1]) for l in lists]) if lists else np.zeros(0, np.uint32)
+        p = np.concatenate([_u32(l[2]) for l in lists]) if with_pos else None
+        terms = np.zeros(len(lists), dtype=TERM_DTYPE)
+        nhits = int(f.sum(dtype=np.uint64))
+        # upper bounds: an int-block is at most 1 + 4 * 166 bytes, so a full document block (two of them) < 11 bytes per document, a tail
+        # document <= 10; a full hit block (int-block + 3) < 6 bytes per hit, a tail hit <= 3 (deltas < 2^14)
+        icap = 16 + 14 * len(lists) + 11 * int(d.size) + 22 * (int(d.size) // 128)
+        hcap = 16 + 6 * nhits
+        index, hits = np.empty(icap, np.uint8), np.empty(hcap, np.uint8)
+        nb, hb, ms = C.c_uint64(), C.c_uint64(), C.c_float()
+        self._ck(self._L.trn_encode_lucene(self._h, _ptr(tb), len(lists), _ptr(d), _ptr(f), _ptr(p), _ptr(index), icap, C.byref(nb),
+                                           _ptr(hits), hcap, C.byref(hb), _ptr(terms), C.byref(ms)))
+        return index[:nb.value].copy(), hits[:hb.value].copy(), terms, float(ms.value)
+
     def close(self):
         if getattr(self, "_h", None):
             self._L.trn_destroy(self._h)

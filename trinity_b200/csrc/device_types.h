@@ -213,4 +213,26 @@ struct EncParams {
         uint32_t *                error;     // != 0: an input the reference encoder throws on (docIDs not ascending / 0, positions decreasing or 0)
 };
 
+// device-side LUCENE encoder (encode_lucene.cuh).  A term's doc units are its full 128-document blocks followed by its tail (the
+// documents % 128 varbyte pairs, possibly none); its hit units are its full 128-hit blocks followed by its hit tail.  Every term has
+// at least one unit of each kind, so a unit's term is the last term whose first unit is <= it.
+struct EncLuceneParams {
+        const unsigned long long *term_begin;  // nterms + 1: first posting of every term in docids[] / freqs[]
+        const unsigned long long *dunit_begin; // nterms + 1: first doc unit of every term
+        const unsigned long long *hunit_begin; // nterms + 1: first hit unit of every term
+        uint32_t                  nterms;
+        uint64_t                  ndunits, nhunits;
+        const uint32_t *          docids;
+        const uint32_t *          freqs;
+        const uint32_t *          positions; // every document's hits, concatenated in posting order; nullptr: positions 1..freq
+        const unsigned long long *hit_begin; // nposts + 1: exclusive scan of freqs
+        uint32_t *                dsz, *hsz;     // bytes of every doc / hit unit
+        uint32_t *                dterm, *hterm; // term of every doc / hit unit
+        const unsigned long long *doff, *hoff;   // exclusive scans of dsz / hsz (hoff is the unit's offset in hits_out)
+        const unsigned long long *term_off;      // nterms + 1: chunk offsets in index_out
+        uint8_t *                 index_out;
+        uint8_t *                 hits_out;
+        uint32_t *                error; // != 0: docIDs not ascending / 0, positions decreasing / 0 / >= Limits::MaxPosition
+};
+
 } // namespace trn

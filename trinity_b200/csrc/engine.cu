@@ -1393,6 +1393,161 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         return TRN_OK;
 }
 
+// =================================================================================================== device-side encoder (LUCENE)
+extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                                 uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
+                                 trn_term *terms, float *device_ms) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (!term_begin || !nterms || !index_bytes || !hits_bytes || !terms)
+                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        const uint64_t nposts = term_begin[nterms];
+        if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
+                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        constexpr uint32_t N = Codecs::Lucene::BLOCK_SIZE;
+        // doc units: every term's full blocks, then its tail; the chunk headers and skiplists around them are fixed by the block counts
+        std::vector<uint64_t> dunit(nterms + 1), fixed(nterms + 1), hunit(nterms + 1), th(nterms + 1);
+        uint64_t              ndunits{0}, fx{0};
+        for (uint32_t t = 0; t < nterms; ++t) {
+                if (term_begin[t + 1] < term_begin[t] || term_begin[t + 1] - term_begin[t] > 0xffffffffull)
+                        return fail(c, TRN_ERR_ARG, "trn_encode_lucene: term_begin must ascend (at most 2^32 - 1 documents per term)");
+                const uint64_t nfull = (term_begin[t + 1] - term_begin[t]) / N;
+                dunit[t]             = ndunits;
+                fixed[t]             = fx;
+                ndunits += nfull + 1u;
+                fx += 14u + 22u * std::min<uint64_t>(nfull, 65535u);
+        }
+        dunit[nterms] = ndunits;
+        fixed[nterms] = fx;
+        CK(cudaSetDevice(c->device));
+        DevBuf d_tb, d_du, d_hu, d_fx, d_doc, d_fr, d_pos, d_hb, d_th, d_dsz, d_hsz, d_dterm, d_hterm, d_doff, d_hoff, d_part, d_toff, d_hto, d_iout, d_hout, d_err;
+        struct Free {
+                std::vector<DevBuf *> v;
+                ~Free() {
+                        for (auto b : v)
+                                b->release();
+                }
+        } fr{{&d_tb, &d_du, &d_hu, &d_fx, &d_doc, &d_fr, &d_pos, &d_hb, &d_th, &d_dsz, &d_hsz, &d_dterm, &d_hterm, &d_doff, &d_hoff, &d_part, &d_toff, &d_hto,
+              &d_iout, &d_hout, &d_err}};
+        const size_t tw = (size_t(nterms) + 1) * 8;
+        CK(d_tb.ensure(tw));
+        CK(d_du.ensure(tw));
+        CK(d_hu.ensure(tw));
+        CK(d_fx.ensure(tw));
+        CK(d_th.ensure(tw));
+        CK(d_toff.ensure(tw));
+        CK(d_hto.ensure(tw));
+        CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(d_hb.ensure((nposts + 1) * 8));
+        CK(d_dsz.ensure(ndunits * 4));
+        CK(d_dterm.ensure(ndunits * 4));
+        CK(d_doff.ensure((ndunits + 1) * 8));
+        CK(d_err.ensure(4));
+        CK(cudaMemcpyAsync(d_tb.p, term_begin, tw, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_du.p, dunit.data(), tw, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_fx.p, fixed.data(), tw, cudaMemcpyHostToDevice, c->stream));
+        if (nposts) {
+                CK(cudaMemcpyAsync(d_doc.p, docids, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_fr.p, freqs, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        CK(cudaMemsetAsync(d_err.p, 0, 4, c->stream));
+        // (1) hits of every posting (scan of the freqs) and of every term; the host needs the per-term totals to number the hit units
+        CK(d_part.ensure(size_t(std::max(nposts, ndunits) / 4096 + 4) * 8));
+        float          ms{0}, a{0};
+        cudaEvent_t    e0 = c->ev0, e1 = c->ev1;
+        CK(cudaEventRecord(e0, c->stream));
+        CK(launch_enc_scan(d_fr.as<uint32_t>(), nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
+        CK(launch_enc_lucene_term_hits(d_tb.as<unsigned long long>(), d_hb.as<unsigned long long>(), nterms, d_th.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(e1, c->stream));
+        CK(cudaMemcpyAsync(th.data(), d_th.p, tw, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&a, e0, e1));
+        ms += a;
+        uint64_t nhunits{0};
+        for (uint32_t t = 0; t < nterms; ++t) {
+                hunit[t] = nhunits;
+                nhunits += (th[t + 1] - th[t]) / N + 1u;
+        }
+        hunit[nterms]       = nhunits;
+        const uint64_t nhits = th[nterms];
+        CK(d_hsz.ensure(nhunits * 4));
+        CK(d_hterm.ensure(nhunits * 4));
+        CK(d_hoff.ensure((nhunits + 1) * 8));
+        CK(d_part.ensure(size_t(nhunits / 4096 + 4) * 8));
+        CK(cudaMemcpyAsync(d_hu.p, hunit.data(), tw, cudaMemcpyHostToDevice, c->stream));
+        if (positions && nhits) {
+                CK(d_pos.ensure(nhits * 4));
+                CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        EncLuceneParams E{};
+        E.term_begin  = d_tb.as<unsigned long long>();
+        E.dunit_begin = d_du.as<unsigned long long>();
+        E.hunit_begin = d_hu.as<unsigned long long>();
+        E.nterms      = nterms;
+        E.ndunits     = ndunits;
+        E.nhunits     = nhunits;
+        E.docids      = d_doc.as<uint32_t>();
+        E.freqs       = d_fr.as<uint32_t>();
+        E.positions   = positions && nhits ? d_pos.as<uint32_t>() : nullptr;
+        E.hit_begin   = d_hb.as<unsigned long long>();
+        E.dsz         = d_dsz.as<uint32_t>();
+        E.hsz         = d_hsz.as<uint32_t>();
+        E.dterm       = d_dterm.as<uint32_t>();
+        E.hterm       = d_hterm.as<uint32_t>();
+        E.doff        = d_doff.as<unsigned long long>();
+        E.hoff        = d_hoff.as<unsigned long long>();
+        E.term_off    = d_toff.as<unsigned long long>();
+        E.error       = d_err.as<uint32_t>();
+        // (2) sizes of every unit, their scans, the chunk and hits.data offsets of every term
+        CK(cudaEventRecord(e0, c->stream));
+        CK(launch_enc_lucene_sizes(E, c->stream));
+        CK(launch_enc_scan(d_dsz.as<uint32_t>(), ndunits, d_part.as<unsigned long long>(), d_doff.as<unsigned long long>(), c->stream));
+        CK(launch_enc_scan(d_hsz.as<uint32_t>(), nhunits, d_part.as<unsigned long long>(), d_hoff.as<unsigned long long>(), c->stream));
+        CK(launch_enc_lucene_terms(E, d_fx.as<unsigned long long>(), d_toff.as<unsigned long long>(), d_hto.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(e1, c->stream));
+        std::vector<uint64_t> toff(nterms + 1), hto(nterms + 1);
+        uint32_t              herr{0};
+        CK(cudaMemcpyAsync(toff.data(), d_toff.p, tw, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(hto.data(), d_hto.p, tw, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(&herr, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&a, e0, e1));
+        ms += a;
+        if (herr)
+                return fail(c, TRN_ERR_ARG, "lucene encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 and non-decreasing");
+        const uint64_t total = toff[nterms], htotal = hto[nterms];
+        *index_bytes         = total;
+        *hits_bytes          = htotal;
+        if (total >= (1ull << 32) || htotal >= (1ull << 32))
+                return fail(c, TRN_ERR_CAPACITY, "lucene encoder: the index and hits.data of one source are limited to 4 GiB (u32 chunk and hits offsets)");
+        if (total > index_cap || htotal > hits_cap || !index_out || (htotal && !hits_out))
+                return fail(c, TRN_ERR_CAPACITY, "trn_encode_lucene: output buffer too small");
+        CK(d_iout.ensure(std::max<size_t>(4, total)));
+        CK(d_hout.ensure(std::max<size_t>(4, htotal)));
+        E.index_out = d_iout.as<uint8_t>();
+        E.hits_out  = d_hout.as<uint8_t>();
+        // (3) the bytes: every byte of both outputs is written by exactly one unit's warp
+        CK(cudaEventRecord(e0, c->stream));
+        CK(launch_enc_lucene_write(E, c->stream));
+        CK(cudaEventRecord(e1, c->stream));
+        CK(cudaMemcpyAsync(index_out, d_iout.p, total, cudaMemcpyDeviceToHost, c->stream));
+        if (htotal)
+                CK(cudaMemcpyAsync(hits_out, d_hout.p, htotal, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&a, e0, e1));
+        ms += a;
+        for (uint32_t t = 0; t < nterms; ++t) {
+                terms[t].documents = uint32_t(term_begin[t + 1] - term_begin[t]);
+                terms[t].chunk_off = uint32_t(toff[t]);
+                terms[t].chunk_len = uint32_t(toff[t + 1] - toff[t]);
+        }
+        if (device_ms)
+                *device_ms = ms;
+        c->have_kernel_events = false;
+        return TRN_OK;
+}
+
 // =================================================================================================== decode probe
 extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t nterms, int materialise, uint32_t *docids, uint32_t *freqs, uint64_t *sums,
                                 float *device_ms) {

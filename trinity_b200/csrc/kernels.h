@@ -35,6 +35,12 @@ cudaError_t launch_enc_scan(const uint32_t *in, uint64_t n, unsigned long long *
 cudaError_t launch_enc_google_sizes(const EncParams &E, cudaStream_t stream);
 cudaError_t launch_enc_term_sizes(const EncParams &E, unsigned long long *chunk_bytes, cudaStream_t stream);
 cudaError_t launch_enc_google_write(const EncParams &E, cudaStream_t stream);
+cudaError_t launch_enc_lucene_term_hits(const unsigned long long *term_begin, const unsigned long long *hit_begin, uint32_t nterms, unsigned long long *term_hits,
+                                        cudaStream_t stream);
+cudaError_t launch_enc_lucene_sizes(const EncLuceneParams &E, cudaStream_t stream);
+cudaError_t launch_enc_lucene_terms(const EncLuceneParams &E, const unsigned long long *fixed, unsigned long long *term_off, unsigned long long *hits_off,
+                                    cudaStream_t stream);
+cudaError_t launch_enc_lucene_write(const EncLuceneParams &E, cudaStream_t stream);
 uint32_t    kernel_max_k();
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
