@@ -349,6 +349,50 @@ int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, cons
  * bit b of word w = docID *base + 32 w + b; the words go to out[0..cap) (TRN_ERR_CAPACITY if cap is smaller). */
 int trn_debug_dense_bitmap(trn_ctx *, uint32_t term, uint32_t *out, uint64_t cap, uint64_t *base, uint64_t *nwords);
 
+/* ------------------------------------------------------------------------------------------------ default exec mode
+ * == exec_query() with no ExecFlags (exec.h:11-43): MatchedIndexDocumentsFilter::consider(const matched_document &) for every match, with
+ * the query terms the match holds and each term's hits (matches.h:34-130).  Which documents match is what DocumentsOnly computes, except
+ * that a root Filter over a disjunction really excludes (build_span makes a GenericDocsSetSpan in this mode, exec.cpp:452-505).  The terms
+ * of a match follow queryexec_ctx::collect_doc_matching_terms (queryexec_ctx.cpp:382-648): a TERM itself, every child of an AND, the
+ * children of an OR / SOME that hold the document, the required side of a NOT, an OPTIONAL's main and its opt where opt holds the document,
+ * every term of a PHRASE; duplicates removed; ascending term index.  A query has at most 32 distinct terms and 32 phrase nodes
+ * (TRN_ERR_UNSUPPORTED otherwise); a LUCENE source needs its hits.data (trn_upload_hits).  trn_exec_batch refuses this mode. */
+#define TRN_MODE_MATCHED_TERMS 4
+/* == term_hit (runtime.h:8-11), in its field order */
+typedef struct trn_hit {
+        uint64_t payload;
+        uint16_t pos;
+        uint8_t  payload_len;
+} trn_hit;
+/* Result of trn_exec_matches; pinned buffers owned by the ctx, valid until the next exec call.  Query q owns the matches
+ * [doc_offsets[q], doc_offsets[q+1]) of docids (ascending); match m owns the terms [term_offsets[m], term_offsets[m+1]) of terms (the term
+ * index, ascending) and freqs; term i owns the hits [hit_offsets[i], hit_offsets[i+1]) of hits. */
+typedef struct trn_matches {
+        uint32_t        nq;
+        uint64_t        total_matches, total_terms, total_hits;
+        const uint64_t *doc_offsets;
+        const uint32_t *docids;
+        const uint64_t *term_offsets;
+        const uint32_t *terms;
+        const uint32_t *freqs;
+        const uint64_t *hit_offsets;
+        const trn_hit * hits;
+        float           device_ms;  /* CUDA-event time of the whole call: host planning, both passes, the copies and the host synchronisations */
+        float           docs_ms;    /* CUDA-event time from the first kernel of the docs pass to the end of its result ordering (no host work) */
+        float           count_ms;   /* CUDA-event time of k_collect_count and the scans of terms and hits over the batch (no host work) */
+        float           write_ms;   /* CUDA-event time of the k_collect_write launches, summed over the chunks (no copies, no host work) */
+        uint32_t        chunks;     /* chunks of matches the write pass ran in (its output buffers are sized per chunk) */
+} trn_matches;
+/* Per match of the batch the collect pass keeps 28 bytes on the device; the terms and hits are written chunk by chunk of matches
+ * (TRN_MATCH_CHUNK, 2^22; halved while a chunk's outputs cannot be allocated) into the pinned result, which is sized once.  As for
+ * trn_exec_batch_device, TRN_ERR_CAPACITY means the batch's matches cannot be staged on the device: split the batch.  trn_fetch_results
+ * has nothing to fetch after this call (TRN_ERR_STATE). */
+int trn_exec_matches(trn_ctx *, const trn_query *queries, uint32_t nq, trn_matches *out);
+/* the kernels' hit walker (csrc/hitcursor.h HitWalker) run on the host over one term: for each listed document, whether the term holds it
+ * (found[i]) with its freq (counts[i]) and its hits into out[0..cap) (*total = their number) */
+int trn_debug_hits(int codec, const uint8_t *index, uint64_t nbytes, const uint8_t *hits, uint64_t hits_bytes, const trn_term *term, const uint32_t *docids, uint32_t n,
+                   uint8_t *found, uint32_t *counts, trn_hit *out, uint64_t cap, uint64_t *total, char *err, size_t errcap);
+
 /* Split form used by bench.py / multi-GPU: run on device only, results stay in HBM ... */
 int trn_exec_batch_device(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out_counts_only);
 /* ... device pointers of the last SCORED_TOPK run: nq*k u32 docids, nq*k f32 scores (unused slots: docid 0, score -1.0; real scores are >= 0), nq u32 counts */

@@ -12,10 +12,11 @@ from typing import Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from ._ffi import QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnQuery, TrnResult, TrnTerm, TrnTimings, lib
+from ._ffi import HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnMatches, TrnQuery, TrnResult, TrnTerm, TrnTimings, lib
 
 CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
+MODE_MATCHED_TERMS = 4  # no ExecFlags: every match with the query terms it holds and their hits (GpuIndexSource.exec_matches)
 MODE_DOCS_COMPACT = 3  # DocumentsOnly, compact result segments (bitmap / bucketed 8-bit offsets / 16-bit offsets / docIDs per tile): trn_result_decode replays them
 NODE_TERM, NODE_AND, NODE_OR, NODE_NOT, NODE_OPTIONAL, NODE_SOME, NODE_PHRASE = 0, 1, 2, 3, 4, 5, 6
 # the path a query ran (GpuIndexSource.last_routes, == TRN_ROUTE_* of include/trinity_b200.h)
@@ -393,6 +394,69 @@ class BatchResult:
         return d, s
 
 
+def debug_hits(codec: int, index: np.ndarray, hits: np.ndarray, term, docids) -> list:
+    """per listed document None when the term does not hold it, else (freq, positions, payload_lens, payloads) as the kernels' hit walker
+    (csrc/hitcursor.h HitWalker, run on the host) reads them for one term"""
+    index = np.ascontiguousarray(index, dtype=np.uint8)
+    hits = np.ascontiguousarray(hits if hits is not None else np.zeros(0, np.uint8), dtype=np.uint8)
+    t = TrnTerm(int(term[0]), int(term[1]), int(term[2]))
+    d = _u32(list(docids))
+    counts = np.zeros(max(len(d), 1), np.uint32)
+    found = np.zeros(max(len(d), 1), np.uint8)
+    cap = 1 << 16
+    while True:
+        out = np.zeros(cap, HIT_DTYPE)
+        total = C.c_uint64()
+        err = C.create_string_buffer(256)
+        rc = lib().trn_debug_hits(codec, _ptr(index), index.size, _ptr(hits) if hits.size else None, hits.size, C.byref(t), _ptr(d), len(d), _ptr(found),
+                                  _ptr(counts), out.ctypes.data, cap, C.byref(total), err, 256)
+        if rc == -6:
+            cap = int(total.value)
+            continue
+        if rc != 0:
+            raise TrinityError(err.value.decode("utf-8", "replace") or f"rc={rc}")
+        res, at = [], 0
+        for i in range(len(d)):
+            if not found[i]:
+                res.append(None)
+                continue
+            h = out[at: at + int(counts[i])]
+            res.append((int(counts[i]), h["pos"].copy(), h["payload_len"].copy(), h["payload"].copy()))
+            at += int(counts[i])
+        return res
+
+
+class MatchesResult:
+    """trn_exec_matches: per query its matches (ascending docID), per match its terms (ascending term index) and freqs, per term its
+    hits (HIT_DTYPE: payload, pos, payload_len)"""
+
+    def __init__(self, r: TrnMatches):
+        nq, nm, nt, nh = int(r.nq), int(r.total_matches), int(r.total_terms), int(r.total_hits)
+        self.nq = nq
+        self.doc_offsets = np.ctypeslib.as_array(r.doc_offsets, shape=(nq + 1,)).copy()
+        self.docids = np.ctypeslib.as_array(r.docids, shape=(max(nm, 1),))[:nm].copy()
+        self.term_offsets = np.ctypeslib.as_array(r.term_offsets, shape=(nm + 1,)).copy()
+        self.terms = np.ctypeslib.as_array(r.terms, shape=(max(nt, 1),))[:nt].copy()
+        self.freqs = np.ctypeslib.as_array(r.freqs, shape=(max(nt, 1),))[:nt].copy()
+        self.hit_offsets = np.ctypeslib.as_array(r.hit_offsets, shape=(nt + 1,)).copy()
+        raw = (C.c_uint8 * (max(nh, 1) * HIT_DTYPE.itemsize)).from_address(r.hits)
+        self.hits = np.frombuffer(raw, dtype=HIT_DTYPE, count=max(nh, 1))[:nh].copy()
+        self.device_ms, self.docs_ms, self.chunks = float(r.device_ms), float(r.docs_ms), int(r.chunks)
+        self.count_ms, self.write_ms = float(r.count_ms), float(r.write_ms)
+
+    def query(self, q: int) -> np.ndarray:
+        return self.docids[int(self.doc_offsets[q]): int(self.doc_offsets[q + 1])]
+
+    def matches(self, q: int):
+        """== the consider(const matched_document &) stream of query q: (docid, [(term, freq, positions, payload_lens, payloads)])"""
+        for m in range(int(self.doc_offsets[q]), int(self.doc_offsets[q + 1])):
+            terms = []
+            for t in range(int(self.term_offsets[m]), int(self.term_offsets[m + 1])):
+                h = self.hits[int(self.hit_offsets[t]): int(self.hit_offsets[t + 1])]
+                terms.append((int(self.terms[t]), int(self.freqs[t]), h["pos"], h["payload_len"], h["payload"]))
+            yield int(self.docids[m]), terms
+
+
 class GpuIndexSource:
     """== one device-resident IndexSource + AccessProxy (index_source.h:18-155, codecs.h:290-317) and the batch form of
     exec_query() (exec.h:50-52) over it."""
@@ -503,6 +567,14 @@ class GpuIndexSource:
         self._ck(self._L.trn_exec_batch(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, C.byref(r)))
         self._last = (mode, k, len(queries))
         return self._wrap(r, mode, k, copy)
+
+    def exec_matches(self, queries: Sequence[np.ndarray], packed=None) -> MatchesResult:
+        """== exec_query() with no ExecFlags for a batch: every match with the query terms it holds and their hits (TRN_MODE_MATCHED_TERMS)"""
+        arr, keep = packed if packed is not None else self._pack(queries)
+        r = TrnMatches()
+        self._ck(self._L.trn_exec_matches(self._h, C.cast(arr, C.c_void_p), len(queries), C.byref(r)))
+        self._last = (MODE_MATCHED_TERMS, 0, len(queries))
+        return MatchesResult(r)
 
     def last_timings(self) -> dict:
         """host-side breakdown (ms) of the last exec_batch / exec_batch_device call"""

@@ -22,6 +22,7 @@ EXPORTS = [
     "trn_exec_batch", "trn_exec_batch_device", "trn_last_topk_device", "trn_merge_topk", "trn_fetch_results", "trn_last_timings",
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_encode_lucene", "trn_debug_chunk_plan",
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
+    "trn_exec_matches", "trn_debug_hits",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -50,6 +51,16 @@ class TrnResult(C.Structure):
                 ("match_counts", C.POINTER(C.c_uint64)), ("postings_scanned", C.c_uint64),
                 ("index_bytes_touched", C.c_uint64), ("kernel_launches", C.c_uint32), ("device_ms", C.c_float), ("exec_kernel_ms", C.c_float),
                 ("words", C.POINTER(C.c_uint32)), ("total_words", C.c_uint64), ("item_desc", C.POINTER(C.c_uint32)), ("qitems", C.c_void_p)]
+
+
+HIT_DTYPE = np.dtype({"names": ["payload", "pos", "payload_len"], "formats": ["<u8", "<u2", "u1"], "offsets": [0, 8, 10], "itemsize": 16})  # trn_hit
+
+
+class TrnMatches(C.Structure):
+    _fields_ = [("nq", C.c_uint32), ("total_matches", C.c_uint64), ("total_terms", C.c_uint64), ("total_hits", C.c_uint64),
+                ("doc_offsets", C.POINTER(C.c_uint64)), ("docids", C.POINTER(C.c_uint32)), ("term_offsets", C.POINTER(C.c_uint64)),
+                ("terms", C.POINTER(C.c_uint32)), ("freqs", C.POINTER(C.c_uint32)), ("hit_offsets", C.POINTER(C.c_uint64)), ("hits", C.c_void_p),
+                ("device_ms", C.c_float), ("docs_ms", C.c_float), ("count_ms", C.c_float), ("write_ms", C.c_float), ("chunks", C.c_uint32)]
 
 
 CONSIDER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
@@ -142,6 +153,8 @@ def lib() -> C.CDLL:
     sig("trn_encode_google", i32, vp, vp, u32, vp, vp, vp, u32, u32, P(u32), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_encode_lucene", i32, vp, vp, u32, vp, vp, vp, vp, C.c_uint64, P(C.c_uint64), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_debug_last_routes", i32, vp, vp, u32, P(u32))
+    sig("trn_exec_matches", i32, vp, vp, u32, P(TrnMatches))
+    sig("trn_debug_hits", i32, i32, vp, C.c_uint64, vp, C.c_uint64, vp, vp, u32, vp, vp, vp, C.c_uint64, P(C.c_uint64), C.c_char_p, C.c_size_t)
     sig("trn_debug_plan", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, P(u32), C.c_char_p, C.c_size_t)
     sig("trn_debug_dense_runs", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     sig("trn_debug_dense_bitmap", i32, vp, u32, vp, u64, P(u64), P(u64))

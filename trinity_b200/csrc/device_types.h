@@ -235,4 +235,50 @@ struct EncLuceneParams {
         uint32_t *                error; // != 0: docIDs not ascending / 0, positions decreasing / 0 / >= Limits::MaxPosition
 };
 
+// ---- the default exec mode (TRN_MODE_MATCHED_TERMS): which query terms a match holds (collect.cuh; planner.cpp plan_collect)
+static constexpr uint32_t kCollectMaxTerms   = 32; // distinct terms of a query: one u32 mask per match
+static constexpr uint32_t kCollectMaxPhrases = 32; // phrase nodes of a query: one ballot
+static constexpr uint32_t kCollectMaxStack   = 32; // operands pending while the post-order program runs
+enum CollectOpKind : uint8_t { CO_TERM = 0, CO_AND = 1, CO_OR = 2, CO_NOT = 3, CO_OPTIONAL = 4, CO_SOME = 5, CO_PHRASE = 6 };
+struct CollectOp { // one node of the post-order collect program
+        uint8_t  kind, nchildren;
+        uint16_t min; // CO_SOME: min-should-match
+        uint32_t arg; // CO_TERM: bit of the term in the query's table (kEmptyTerm: a term the source does not hold); CO_PHRASE: phrase index
+};
+struct CollectPhrase {
+        uint32_t arg_begin; // first OP_ARG step of its term ids (phrase.cuh phrase_arg), in CollectPlan::args
+        uint32_t k;         // terms of the phrase
+        uint32_t mask;      // its terms' bits in the query's table
+        uint32_t pad;
+};
+struct CollectQuery {
+        uint32_t term_begin, nterms;     // the query's distinct terms, ascending term index (bit j = terms[term_begin + j])
+        uint32_t phrase_begin, nphrases; // its phrase nodes
+        uint32_t prog_begin, nprog;      // its post-order program
+};
+static_assert(sizeof(trn_hit) == 16, "trn_hit: payload, pos, payload_len, 5 padding bytes");
+struct CollectParams {
+        DevIndex             ix;
+        const CollectQuery * queries;
+        const uint32_t *     terms;
+        const CollectPhrase *phrases;
+        const DevStep *      args;
+        const CollectOp *    prog;
+        const uint64_t *     q_offsets; // nq + 1: the matches of query q are [q_offsets[q], q_offsets[q + 1]) of docids
+        const uint32_t *     docids;
+        uint32_t             nq;
+        uint64_t             m0, m1;   // the launch's matches (the count kernel: the whole batch; the write kernel: one chunk)
+        uint32_t *           mask;     // per match of the batch: the matched terms
+        uint32_t *           nterms;   // ... their number
+        uint32_t *           nhits;    // ... and the sum of their freqs
+        const unsigned long long *term_scan, *hit_scan; // exclusive scans of nterms / nhits over the batch
+        uint64_t             term_base, hit_base;        // the chunk's first term / hit: where out_terms ... / out_hits start
+        uint64_t *           term_offsets; // per match of the chunk: its first term (global)
+        uint32_t *           out_terms;    // per term of the chunk
+        uint32_t *           out_freqs;
+        uint64_t *           hit_offsets;  // per term of the chunk: its first hit (global)
+        trn_hit *            out_hits;     // per hit of the chunk
+        uint32_t *           error;        // != 0: a match the collect program does not accept (a docs-pass / program disagreement)
+};
+
 } // namespace trn

@@ -137,6 +137,24 @@ struct trn_ctx {
         uint64_t last_postings{0}, last_bytes{0};
         float    last_ms{0};
         std::vector<uint8_t> last_routes; // TRN_ROUTE_* of every query of the last batch (trn_debug_last_routes)
+        // the default exec mode (trn_exec_matches): collect programs, per-chunk intermediates and outputs, the pinned result
+        struct MatchBufs {
+                DevBuf d_cq, d_cterms, d_cphrases, d_cargs, d_cprog, d_mask, d_nterms, d_nhits, d_tscan, d_hscan, d_part, d_term_off, d_terms, d_freqs,
+                    d_hit_off, d_hits, d_error;
+                PinBuf      h_doc_off, h_docids, h_term_off, h_terms, h_freqs, h_hit_off, h_hits, h_small;
+                cudaEvent_t ev_docs{nullptr}, ev_c0{nullptr}, ev_c1{nullptr}, ev_w0{nullptr}, ev_w1{nullptr}, ev_end{nullptr};
+                void release() {
+                        for (DevBuf *b : {&d_cq, &d_cterms, &d_cphrases, &d_cargs, &d_cprog, &d_mask, &d_nterms, &d_nhits, &d_tscan, &d_hscan, &d_part, &d_term_off,
+                                          &d_terms, &d_freqs, &d_hit_off, &d_hits, &d_error})
+                                b->release();
+                        for (PinBuf *b : {&h_doc_off, &h_docids, &h_term_off, &h_terms, &h_freqs, &h_hit_off, &h_hits, &h_small})
+                                b->release();
+                        for (cudaEvent_t e : {ev_docs, ev_c0, ev_c1, ev_w0, ev_w1, ev_end})
+                                if (e)
+                                        cudaEventDestroy(e);
+                }
+        } mt;
+        uint64_t match_chunk{1ull << 22}; // TRN_MATCH_CHUNK: matches per chunk of the write pass (halved while its outputs do not fit)
 };
 
 #define CK(call)                                                                                                                                               \
@@ -208,6 +226,11 @@ extern "C" int trn_create(int device, trn_ctx **out) {
                 if (v >= 1)
                         c->chunk_postings = uint64_t(v);
         }
+        if (const char *e = getenv("TRN_MATCH_CHUNK")) {
+                const long long v = atoll(e);
+                if (v >= 1)
+                        c->match_chunk = uint64_t(v);
+        }
         CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
                 CK(cudaEventCreateWithFlags(&c->ev_done[i], cudaEventDisableTiming));
@@ -244,6 +267,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
                 if (c->ev_ck1[i])
                         cudaEventDestroy(c->ev_ck1[i]);
         }
+        c->mt.release();
         if (c->copy_stream)
                 cudaStreamDestroy(c->copy_stream);
         delete c;
@@ -526,8 +550,10 @@ static DevIndex dev_index(trn_ctx *c) {
 // =================================================================================================== exec
 // small device scratch layout (d_small): [0] ticket u32, [2..3] seg_cursor u64, [4] overflow u32, then per-query arrays.
 // routes[0 .. nq): the TRN_ROUTE_* of every query (written on success)
+// collect: non-null = the docs pass of the default exec mode (mode DOCS_ONLY; the plan is made in TRN_MODE_MATCHED_TERMS, and its collect
+// programs are moved to *collect)
 static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out, int set, cudaEvent_t k0, cudaEvent_t k1,
-                            uint8_t *routes) {
+                            uint8_t *routes, CollectPlan *collect = nullptr) {
         if (!c)
                 return TRN_ERR_ARG;
         if (!c->have_index)
@@ -548,9 +574,12 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         c->pc.allow_phrase     = c->pc.codec == TRN_CODEC_GOOGLE || c->have_hits; // GOOGLE: inline hits; LUCENE: hits.data uploaded (trn_upload_hits)
         BatchPlan   plan;
         std::string perr;
-        const int   prc = plan_batch(c->pc, c->h_terms, c->dense_terms ? c->h_dense_off.data() : nullptr, queries, nq, mode, k, plan, perr);
+        const int   prc = plan_batch(c->pc, c->h_terms, c->dense_terms ? c->h_dense_off.data() : nullptr, queries, nq, collect ? TRN_MODE_MATCHED_TERMS : mode, k, plan,
+                                     perr);
         if (prc != TRN_OK)
                 return fail(c, prc, perr);
+        if (collect)
+                *collect = std::move(plan.collect);
         c->tm.host_compile_ms += float(now_ms() - tCompile0);
         const double   tEnqueue0  = now_ms();
         const uint32_t totalItems = uint32_t(plan.items);
@@ -1117,6 +1146,186 @@ extern "C" int trn_debug_last_routes(trn_ctx *c, uint8_t *out, uint32_t cap, uin
 }
 
 // plans a batch on the host as exec_device_impl would on a context that holds this index (trn_debug_plan, trn_debug_dense_runs)
+// ============================================================================================ default exec mode
+extern "C" int trn_exec_matches(trn_ctx *c, const trn_query *queries, uint32_t nq, trn_matches *out) {
+        if (!c || !out)
+                return TRN_ERR_ARG;
+        CK(cudaSetDevice(c->device));
+        std::memset(out, 0, sizeof(*out));
+        c->have_kernel_events = false;
+        c->tm                 = trn_timings{};
+        c->last_routes.clear();
+        c->last_mode = -1;
+        auto &M      = c->mt;
+        if (!M.ev_docs) {
+                for (cudaEvent_t *e : {&M.ev_docs, &M.ev_c0, &M.ev_c1, &M.ev_w0, &M.ev_w1, &M.ev_end})
+                        CK(cudaEventCreate(e));
+        }
+        const double t0 = now_ms();
+        // ---- docs pass: the DocumentsOnly routes (root-filter quirk off) into d_out_docids[0] / d_q_offsets[0]
+        CK(cudaEventRecord(c->ev0, c->stream));
+        std::vector<uint8_t> routes(nq);
+        CollectPlan          cp;
+        const int            r = exec_device_impl(c, queries, nq, TRN_MODE_DOCS_ONLY, 0, nullptr, 0, c->evk0, c->evk1, routes.data(), &cp);
+        c->last_mode         = -1; // trn_fetch_results has nothing to fetch after this call (the docs pass leaves no trn_result)
+        if (r != TRN_OK)
+                return r;
+        CK(cudaEventRecord(M.ev_docs, c->stream));
+        CK(M.h_doc_off.ensure((size_t(nq) + 1) * 8));
+        CK(cudaMemcpyAsync(M.h_doc_off.p, c->d_q_offsets[0].p, (size_t(nq) + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(M.h_small.ensure(64));
+        CK(cudaMemcpyAsync(M.h_small.p, c->d_small[0].p, 64, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        if (M.h_small.as<uint32_t>()[4])
+                return fail(c, TRN_ERR_CAPACITY, "segment buffer overflow (internal bound violated)");
+        const uint64_t nm = M.h_doc_off.as<uint64_t>()[nq];
+        CK(M.h_docids.ensure(std::max<size_t>(4, nm * 4)));
+        if (nm)
+                CK(cudaMemcpyAsync(M.h_docids.p, c->d_out_docids[0].p, nm * 4, cudaMemcpyDeviceToHost, c->stream));
+
+        // ---- collect programs; per match of the batch: mask, term and hit counts and their scans (28 bytes)
+        auto upload = [&](DevBuf &b, const void *src, size_t bytes) -> cudaError_t {
+                if (const cudaError_t e = b.ensure(std::max<size_t>(16, bytes)); e != cudaSuccess)
+                        return e;
+                return bytes ? cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
+        };
+        CK(upload(M.d_cq, cp.queries.data(), cp.queries.size() * sizeof(CollectQuery)));
+        CK(upload(M.d_cterms, cp.terms.data(), cp.terms.size() * 4));
+        CK(upload(M.d_cphrases, cp.phrases.data(), cp.phrases.size() * sizeof(CollectPhrase)));
+        CK(upload(M.d_cargs, cp.args.data(), cp.args.size() * sizeof(DevStep)));
+        CK(upload(M.d_cprog, cp.prog.data(), cp.prog.size() * sizeof(CollectOp)));
+        CK(M.d_error.ensure(4));
+        CK(cudaMemsetAsync(M.d_error.p, 0, 4, c->stream));
+        for (DevBuf *b : {&M.d_mask, &M.d_nterms, &M.d_nhits})
+                CK(b->ensure(std::max<size_t>(4, nm * 4)));
+        for (DevBuf *b : {&M.d_tscan, &M.d_hscan})
+                CK(b->ensure((nm + 1) * 8));
+        CK(M.d_part.ensure((nm / 4096 + 2) * 8));
+
+        CollectParams P;
+        std::memset(&P, 0, sizeof(P));
+        P.ix        = dev_index(c);
+        P.queries   = M.d_cq.as<CollectQuery>();
+        P.terms     = M.d_cterms.as<uint32_t>();
+        P.phrases   = M.d_cphrases.as<CollectPhrase>();
+        P.args      = M.d_cargs.as<DevStep>();
+        P.prog      = M.d_cprog.as<CollectOp>();
+        P.q_offsets = c->d_q_offsets[0].as<uint64_t>();
+        P.docids    = c->d_out_docids[0].as<uint32_t>();
+        P.nq        = nq;
+        P.error     = M.d_error.as<uint32_t>();
+        P.mask      = M.d_mask.as<uint32_t>();
+        P.nterms    = M.d_nterms.as<uint32_t>();
+        P.nhits     = M.d_nhits.as<uint32_t>();
+        P.term_scan = M.d_tscan.as<unsigned long long>();
+        P.hit_scan  = M.d_hscan.as<unsigned long long>();
+        P.m0        = 0;
+        P.m1        = nm;
+        CK(cudaEventRecord(M.ev_c0, c->stream));
+        CK(launch_collect_count(P, c->stream));
+        CK(launch_enc_scan(P.nterms, nm, M.d_part.as<unsigned long long>(), M.d_tscan.as<unsigned long long>(), c->stream));
+        CK(launch_enc_scan(P.nhits, nm, M.d_part.as<unsigned long long>(), M.d_hscan.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(M.ev_c1, c->stream));
+        uint64_t *tot = M.h_small.as<uint64_t>();
+        CK(cudaMemcpyAsync(tot, M.d_tscan.as<uint64_t>() + nm, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(tot + 1, M.d_hscan.as<uint64_t>() + nm, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(tot + 2, M.d_error.p, 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        if (uint32_t(tot[2]))
+                return fail(c, TRN_ERR_STATE, "a match of the docs pass is not accepted by its query's collect program (internal error)");
+        float countMs{0};
+        (void)cudaEventElapsedTime(&countMs, M.ev_c0, M.ev_c1);
+        const uint64_t nt = tot[0], nh = tot[1];
+
+        // ---- the result's pinned host buffers, sized once
+        CK(M.h_term_off.ensure((nm + 1) * 8));
+        CK(M.h_terms.ensure(std::max<size_t>(4, nt * 4)));
+        CK(M.h_freqs.ensure(std::max<size_t>(4, nt * 4)));
+        CK(M.h_hit_off.ensure((nt + 1) * 8));
+        CK(M.h_hits.ensure(std::max<size_t>(sizeof(trn_hit), nh * sizeof(trn_hit))));
+        CK(cudaMemcpyAsync(M.h_term_off.as<uint64_t>() + nm, M.d_tscan.as<uint64_t>() + nm, 8, cudaMemcpyDeviceToHost, c->stream));
+        M.h_hit_off.as<uint64_t>()[nt] = nh;
+
+        // ---- write pass, chunk by chunk of matches: a chunk's terms and hits go through device buffers sized for it
+        uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(1, c->match_chunk), std::max<uint64_t>(1, nm));
+        float    writeMs{0};
+        uint32_t chunks{0};
+        for (uint64_t m0 = 0; m0 < nm;) {
+                const uint64_t m1 = std::min(nm, m0 + chunk), n = m1 - m0;
+                uint64_t *     sc = tot + 4; // the scans at the chunk's bounds
+                CK(cudaMemcpyAsync(sc, M.d_tscan.as<uint64_t>() + m0, 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaMemcpyAsync(sc + 1, M.d_tscan.as<uint64_t>() + m1, 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaMemcpyAsync(sc + 2, M.d_hscan.as<uint64_t>() + m0, 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaMemcpyAsync(sc + 3, M.d_hscan.as<uint64_t>() + m1, 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaStreamSynchronize(c->stream));
+                const uint64_t t0c = sc[0], ntc = sc[1] - sc[0], h0c = sc[2], nhc = sc[3] - sc[2];
+                cudaError_t    e = M.d_term_off.ensure(n * 8);
+                for (DevBuf *b : {&M.d_terms, &M.d_freqs})
+                        if (e == cudaSuccess)
+                                e = b->ensure(std::max<uint64_t>(4, ntc * 4));
+                if (e == cudaSuccess)
+                        e = M.d_hit_off.ensure(std::max<uint64_t>(8, ntc * 8));
+                if (e == cudaSuccess)
+                        e = M.d_hits.ensure(std::max<uint64_t>(16, nhc * sizeof(trn_hit)));
+                if (e == cudaErrorMemoryAllocation && chunk > 1) { // the chunk's outputs do not fit: halve it
+                        (void)cudaGetLastError();
+                        chunk = (chunk + 1) / 2;
+                        continue;
+                }
+                CK(e);
+                P.m0           = m0;
+                P.m1           = m1;
+                P.term_base    = t0c;
+                P.hit_base     = h0c;
+                P.term_offsets = M.d_term_off.as<uint64_t>();
+                P.out_terms    = M.d_terms.as<uint32_t>();
+                P.out_freqs    = M.d_freqs.as<uint32_t>();
+                P.hit_offsets  = M.d_hit_off.as<uint64_t>();
+                P.out_hits     = M.d_hits.as<trn_hit>();
+                CK(cudaEventRecord(M.ev_w0, c->stream));
+                CK(launch_collect_write(P, c->stream));
+                CK(cudaEventRecord(M.ev_w1, c->stream));
+                CK(cudaMemcpyAsync(M.h_term_off.as<uint64_t>() + m0, P.term_offsets, n * 8, cudaMemcpyDeviceToHost, c->stream));
+                if (ntc) {
+                        CK(cudaMemcpyAsync(M.h_terms.as<uint32_t>() + t0c, P.out_terms, ntc * 4, cudaMemcpyDeviceToHost, c->stream));
+                        CK(cudaMemcpyAsync(M.h_freqs.as<uint32_t>() + t0c, P.out_freqs, ntc * 4, cudaMemcpyDeviceToHost, c->stream));
+                        CK(cudaMemcpyAsync(M.h_hit_off.as<uint64_t>() + t0c, P.hit_offsets, ntc * 8, cudaMemcpyDeviceToHost, c->stream));
+                }
+                if (nhc)
+                        CK(cudaMemcpyAsync(M.h_hits.as<trn_hit>() + h0c, P.out_hits, nhc * sizeof(trn_hit), cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaStreamSynchronize(c->stream)); // the chunk's device buffers are reused by the next chunk
+                float ms{0};
+                if (cudaEventElapsedTime(&ms, M.ev_w0, M.ev_w1) == cudaSuccess)
+                        writeMs += ms;
+                m0 = m1;
+                ++chunks;
+        }
+        CK(cudaEventRecord(M.ev_end, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        c->last_routes     = std::move(routes);
+        c->tm.total_ms     = float(now_ms() - t0);
+        out->nq            = nq;
+        out->total_matches = nm;
+        out->total_terms   = nt;
+        out->total_hits    = nh;
+        out->doc_offsets   = M.h_doc_off.as<uint64_t>();
+        out->docids        = M.h_docids.as<uint32_t>();
+        out->term_offsets  = M.h_term_off.as<uint64_t>();
+        out->terms         = M.h_terms.as<uint32_t>();
+        out->freqs         = M.h_freqs.as<uint32_t>();
+        out->hit_offsets   = M.h_hit_off.as<uint64_t>();
+        out->hits          = M.h_hits.as<trn_hit>();
+        out->chunks        = chunks;
+        out->count_ms      = countMs;
+        out->write_ms      = writeMs;
+        float ms{0};
+        if (cudaEventElapsedTime(&ms, c->ev0, M.ev_end) == cudaSuccess)
+                out->device_ms = ms;
+        if (cudaEventElapsedTime(&ms, c->evk0, M.ev_docs) == cudaSuccess)
+                out->docs_ms = ms;
+        return TRN_OK;
+}
+
 static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
                             const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &plan, char *err, size_t errcap) {
         auto seterr = [&](const std::string &m, int rc) {
@@ -1126,7 +1335,7 @@ static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, co
                 }
                 return rc;
         };
-        if (!index || !terms || !queries || !nq || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || mode < 0 || mode > 3)
+        if (!index || !terms || !queries || !nq || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || mode < 0 || mode > TRN_MODE_MATCHED_TERMS)
                 return seterr("bad arguments", TRN_ERR_ARG);
         BlockDirectory       dir;
         std::vector<DevTerm> ht;

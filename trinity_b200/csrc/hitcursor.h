@@ -279,5 +279,177 @@ TRN_HD HitCursor hit_cursor(const HitsView &ix, const PhraseTerm &t, uint32_t d)
         return ix.codec == 0 ? hit_cursor_google(ix, t, d) : hit_cursor_lucene(ix, t, d);
 }
 
+// ---- hits with their payloads (the default exec mode's term_hit{payload, pos, payloadLen}, runtime.h:8-11; collect.cuh, trn_debug_hits)
+// Whether the term holds d at all: a LUCENE document may have freq 0 and so no hits, but the term still holds it.
+TRN_HD bool term_holds(const HitsView &ix, const PhraseTerm &t, uint32_t d, uint32_t &freq) {
+        freq = 0;
+        if (!t.nb || d < t.first || d > t.last)
+                return false;
+        const uint32_t b = dir_first_block_ge(ix.blk_last + t.dir, ix.tile_first + t.tfb, t.nb, t.first, t.last, t.tfbase, t.tfs, d);
+        if (b >= t.nb)
+                return false;
+        const uint32_t prev = b ? TRN_LDG(ix.blk_last + t.dir + b - 1u) : 0u;
+        const uint8_t *p    = ix.index + TRN_LDG(ix.blk_off + t.dir + b);
+        if (ix.codec == 0) { // doc deltas, then one freq per document (google_codec.cpp:497-531)
+                const uint32_t last = TRN_LDG(ix.blk_last + t.dir + b);
+                const uint32_t n    = (b + 1u == t.nb) ? (t.docs - 32u * (t.nb - 1u)) : 32u;
+                uint32_t       idx = 0xffffffffu, doc = prev;
+                for (uint32_t i = 0; i + 1u < n; ++i) {
+                        doc += varbyte_get(p);
+                        if (doc == d)
+                                idx = i;
+                }
+                if (last == d)
+                        idx = n - 1u;
+                if (idx == 0xffffffffu)
+                        return false;
+                for (uint32_t i = 0; i <= idx; ++i)
+                        freq = varbyte_get(p);
+                freq &= 0xffffu;
+                return true;
+        }
+        if (b < (t.docs >> 7)) {
+                PforRef D;
+                D.init(p);
+                uint32_t doc = prev, idx = 0, e = 0;
+                for (; idx < 128u; ++idx) {
+                        doc += D.get(idx, e);
+                        if (doc >= d)
+                                break;
+                }
+                if (idx == 128u || doc != d)
+                        return false;
+                PforRef F;
+                F.init(D.end());
+                e = F.exceptions_before(idx);
+                freq = F.get(idx, e) & 0xffffu;
+                return true;
+        }
+        const uint32_t n   = t.docs & 127u;
+        uint32_t       doc = prev;
+        for (uint32_t i = 0; i < n; ++i) {
+                doc += varbyte_get(p);
+                const uint32_t f = varbyte_get(p);
+                if (doc == d) {
+                        freq = f & 0xffffu;
+                        return true;
+                }
+                if (doc > d)
+                        break;
+        }
+        return false;
+}
+
+// low `len` bytes of v replaced by p[0 .. len) (memcpy into the little-endian u64)
+TRN_HD uint64_t payload_overwrite(uint64_t v, const uint8_t *p, uint32_t len) {
+        uint64_t x = 0;
+        for (uint32_t i = 0; i < len; ++i)
+                x |= uint64_t(TRN_LDG(p + i)) << (8u * i);
+        const uint64_t keep = len >= 8u ? 0ull : (~0ull << (8u * len));
+        return (v & keep) | x;
+}
+
+// The hits of one document of one term with their payloads, in order:
+//   GOOGLE (materialize_hits, google_codec.cpp:533-594): the payload u64 starts at 0 for each document and is zeroed only while the
+//          current size is 0; a non-zero size overwrites its low bytes, so a hit keeps the high bytes of an earlier, longer payload.
+//   LUCENE (refill_hits / materialize_hits, lucene_codec.cpp:401-462, 767-856): a full 128-hit block is [deltas int-block][payload
+//          lengths int-block][varbyte chunk length][payload bytes]; the varbyte tail carries a payload length that persists from hit to
+//          hit across documents, starting at 0 at the tail's start, and its payload bytes follow all its varbytes.  Each payload is zeroed
+//          before its bytes are copied.
+struct HitWalker {
+        HitCursor      c;     // positions (its LUCENE block / tail state is followed below)
+        uint64_t       payload;
+        uint32_t       plen;  // GOOGLE: current size; LUCENE tail: the persisting length
+        const uint8_t *pp;    // next payload byte
+        PforRef        lens;  // LUCENE full block: payload lengths
+        uint32_t       le, tail_n;
+
+        // LUCENE: enter hit block hb at value `within` (lengths of the values before it skipped)
+        TRN_HD void lucene_block(uint32_t within) {
+                lens.init(c.blk.end());
+                const uint8_t *q = lens.end();
+                (void)varbyte_get(q); // the chunk length
+                pp = q;
+                le = 0;
+                for (uint32_t i = 0; i < within; ++i)
+                        pp += lens.get(i, le);
+        }
+        // LUCENE: the tail starting at p; position the payload pointer and the persisting length at hit `within`
+        TRN_HD void lucene_tail(const uint8_t *p, uint32_t within) {
+                uint32_t len = 0, off = 0, at = 0;
+                for (uint32_t i = 0; i < tail_n; ++i) {
+                        if (i == within)
+                                at = len;
+                        const uint32_t step = varbyte_get(p);
+                        if (step & 1u)
+                                len = TRN_LDG(p++);
+                        if (i < within)
+                                off += len;
+                }
+                pp   = p + off;
+                plen = at;
+        }
+
+        TRN_HD void init(const HitsView &ix, const PhraseTerm &t, uint32_t d) {
+                c       = hit_cursor(ix, t, d);
+                payload = 0;
+                plen = le = tail_n = 0;
+                pp               = nullptr;
+                if (ix.codec == 0 || !c.left)
+                        return;
+                tail_n = ix.hit_term[t.id].sum_hits & 127u;
+                if (c.mode == 1u)
+                        lucene_block(c.within);
+                else
+                        lucene_tail(c.hits + TRN_LDG(c.hoff + c.nfh), c.within);
+        }
+
+        // the next hit: returns its position, sets payload / len
+        TRN_HD uint32_t next(uint32_t &len) {
+                --c.left;
+                if (c.mode == 0u) {
+                        const uint32_t step = varbyte_get(c.p);
+                        if (step & 1u)
+                                c.psize = TRN_LDG(c.p++);
+                        c.pos += step >> 1;
+                        len = c.psize;
+                        if (len) {
+                                payload = payload_overwrite(payload, c.p, len > 8u ? 8u : len);
+                                c.p += len;
+                        } else
+                                payload = 0;
+                        return c.pos;
+                }
+                if (c.mode == 1u) {
+                        c.pos += c.blk.get(c.within, c.e);
+                        len     = lens.get(c.within, le);
+                        payload = payload_overwrite(0, pp, len > 8u ? 8u : len);
+                        pp += len;
+                        if (++c.within == 128u && c.left) { // on to the next block / the tail
+                                ++c.hb;
+                                c.within = 0;
+                                c.e      = 0;
+                                if (c.hb < c.nfh) {
+                                        c.blk.init(c.hits + TRN_LDG(c.hoff + c.hb));
+                                        lucene_block(0);
+                                } else {
+                                        c.mode = 2u;
+                                        c.p    = c.hits + TRN_LDG(c.hoff + c.nfh);
+                                        lucene_tail(c.p, 0);
+                                }
+                        }
+                        return c.pos;
+                }
+                const uint32_t step = varbyte_get(c.p);
+                if (step & 1u)
+                        plen = TRN_LDG(c.p++);
+                c.pos += step >> 1;
+                len     = plen;
+                payload = payload_overwrite(0, pp, len > 8u ? 8u : len);
+                pp += len;
+                return c.pos;
+        }
+};
+
 
 } // namespace trn

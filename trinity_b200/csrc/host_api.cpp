@@ -255,6 +255,72 @@ extern "C" int trn_debug_positions(int codec, const uint8_t *index, uint64_t nby
         }
 }
 
+extern "C" int trn_debug_hits(int codec, const uint8_t *index, uint64_t nbytes, const uint8_t *hits, uint64_t hbytes, const trn_term *term, const uint32_t *docids,
+                              uint32_t n, uint8_t *found, uint32_t *counts, trn_hit *out, uint64_t cap, uint64_t *total, char *err, size_t errcap) {
+        if (!index || !term || !total || (n && (!docids || !counts || !found)) || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))
+                return TRN_ERR_ARG;
+        try {
+                term_index_ctx t;
+                t.documents = term->documents;
+                t.offset    = term->chunk_off;
+                t.size      = term->chunk_len;
+                BlockDirectory d;
+                build_block_directory(codec == TRN_CODEC_GOOGLE ? Codec::Google : Codec::Lucene, index, nbytes, &t, 1, 1, d);
+                HitsDirectory hd;
+                HitTerm       ht{0, 0};
+                if (codec == TRN_CODEC_LUCENE) {
+                        build_hits_directory(index, nbytes, hits, hbytes, &t, 1, d, 1, hd);
+                        ht = HitTerm{hd.hb_begin[0], hd.sum_hits[0]};
+                }
+                HitsView v;
+                v.index      = index;
+                v.blk_last   = d.blk_last.data();
+                v.blk_off    = d.blk_off.data();
+                v.tile_first = d.tile_first.data();
+                v.hits       = hits;
+                v.hit_base   = hd.hit_base.data();
+                v.hblk_off   = hd.hblk_off.data();
+                v.hit_term   = &ht;
+                v.codec      = codec == TRN_CODEC_GOOGLE ? 0 : 1;
+                const auto &T = d.terms[0];
+                PhraseTerm  pt;
+                pt.dir    = T.dir_begin;
+                pt.nb     = T.nblocks;
+                pt.docs   = T.documents;
+                pt.first  = T.first_doc;
+                pt.last   = T.last_doc;
+                pt.tfb    = T.tf_begin;
+                pt.tfbase = T.tf_base;
+                pt.tfs    = T.tf_shift;
+                pt.id     = 0;
+                uint64_t k{0};
+                for (uint32_t i = 0; i < n; ++i) {
+                        uint32_t freq{0};
+                        found[i]  = term_holds(v, pt, docids[i], freq) ? 1 : 0;
+                        counts[i] = freq;
+                        if (!found[i] || !freq)
+                                continue;
+                        HitWalker w;
+                        w.init(v, pt, docids[i]);
+                        while (w.c.left) {
+                                uint32_t       len{0};
+                                const uint32_t pos = w.next(len);
+                                if (k < cap && out)
+                                        out[k] = trn_hit{w.payload, uint16_t(pos), uint8_t(len)};
+                                ++k;
+                        }
+                }
+                *total = k;
+                return k > cap ? TRN_ERR_CAPACITY : TRN_OK;
+        } catch (const std::exception &e) {
+                if (err && errcap) {
+                        std::strncpy(err, e.what(), errcap - 1);
+                        err[errcap - 1] = 0;
+                }
+                return TRN_ERR_FORMAT;
+        }
+}
+
 extern "C" int trn_directory_stats(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, int threads, uint64_t *directory_bytes,
                                    uint64_t *total_blocks, uint64_t *table_entries, char *err, size_t errcap) {
         if (!index || !terms || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))

@@ -41,6 +41,8 @@ cudaError_t launch_enc_lucene_sizes(const EncLuceneParams &E, cudaStream_t strea
 cudaError_t launch_enc_lucene_terms(const EncLuceneParams &E, const unsigned long long *fixed, unsigned long long *term_off, unsigned long long *hits_off,
                                     cudaStream_t stream);
 cudaError_t launch_enc_lucene_write(const EncLuceneParams &E, cudaStream_t stream);
+cudaError_t launch_collect_count(const CollectParams &P, cudaStream_t stream); // the default exec mode's collect pass (collect.cuh)
+cudaError_t launch_collect_write(const CollectParams &P, cudaStream_t stream);
 uint32_t    kernel_max_k();
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);

@@ -1301,6 +1301,12 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                     uint32_t k, BatchPlan &out, std::string &err) {
         out                = BatchPlan{};
         const bool scored  = mode == TRN_MODE_SCORED_ALL || mode == TRN_MODE_SCORED_TOPK;
+        if (mode == TRN_MODE_MATCHED_TERMS) { // the DocumentsOnly program, plus what the collect pass runs per match
+                if (!cfg.allow_phrase)
+                        return fail(err, TRN_ERR_UNSUPPORTED, "the default exec mode needs the hits: a LUCENE source runs it once its hits.data has been uploaded (trn_upload_hits)");
+                if (const int rc = plan_collect(terms, queries, nq, out.collect, err); rc != TRN_OK)
+                        return rc;
+        }
         const bool google  = cfg.codec == TRN_CODEC_GOOGLE;
         const double width = double(cfg.max_docid) - double(std::min(cfg.min_docid, cfg.max_docid)) + 1.0; // docID span of THIS source
         // docID tile of the step-program launch: set queries run one warp per tile (k_exec_docs) on larger tiles; scored queries keep a
@@ -1316,6 +1322,8 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                         return fail(err, TRN_ERR_ARG, "empty query");
                 Compiler cc(Q.nodes, Q.nnodes, terms, scored, Q.root, steps);
                 cc.allow_phrase = cfg.allow_phrase;
+                // the default exec mode makes a GenericDocsSetSpan for every root (exec.cpp:452-505), which honours a root Filter
+                cc.reference_quirks = mode != TRN_MODE_MATCHED_TERMS;
                 auto &dq        = out.queries[q];
                 dq.step_begin   = uint32_t(steps.size());
                 const int rs    = cc.run();
@@ -1601,6 +1609,124 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                         else if (dq.route != TRN_ROUTE_FLAT_TREE)
                                 out.gen_items += dq.ntiles;
                 }
+        }
+        return TRN_OK;
+}
+
+// The collect program of a query (the default exec mode, collect.cuh): its distinct terms, ascending, and its nodes in post order with
+// queryexec_ctx::collect_doc_matching_terms' rules (queryexec_ctx.cpp:382-648) — a TERM reports itself, an AND all its children, an OR /
+// SOME the children that hold the document, a NOT its required side, an OPTIONAL its main and its opt where opt holds the document, a
+// PHRASE all its terms.  A term the source does not hold never holds a document; so does a phrase with such a term.
+int trn::plan_collect(const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, CollectPlan &out, std::string &err) {
+        out = CollectPlan{};
+        out.queries.resize(nq);
+        for (uint32_t q = 0; q < nq; ++q) {
+                const auto &Q = queries[q];
+                const auto *n = Q.nodes;
+                if (!n || !Q.nnodes || Q.root >= Q.nnodes || !plan_depth_ok(n, Q.nnodes))
+                        return fail(err, TRN_ERR_ARG, "query " + std::to_string(q) + ": bad plan");
+                auto held = [&](uint32_t t) { return t != kEmptyTerm && t < terms.size() && terms[t].documents != 0; };
+                // the distinct terms below the root
+                std::vector<uint32_t> tv, todo{Q.root};
+                while (!todo.empty()) {
+                        const uint32_t i = todo.back();
+                        todo.pop_back();
+                        if (n[i].kind == TRN_NODE_TERM) {
+                                if (held(n[i].term))
+                                        tv.push_back(n[i].term);
+                        } else
+                                for (uint32_t c = 0; c < n[i].nchildren; ++c)
+                                        if (uint32_t(n[i].first_child) + c < Q.nnodes && n[i].first_child > i)
+                                                todo.push_back(n[i].first_child + c);
+                }
+                std::sort(tv.begin(), tv.end());
+                tv.erase(std::unique(tv.begin(), tv.end()), tv.end());
+                if (tv.size() > kCollectMaxTerms)
+                        return fail(err, TRN_ERR_UNSUPPORTED,
+                                    "query " + std::to_string(q) + ": the default exec mode takes at most 32 distinct terms per query (" + std::to_string(tv.size()) + ")");
+                auto bit = [&](uint32_t t) { return held(t) ? uint32_t(std::lower_bound(tv.begin(), tv.end(), t) - tv.begin()) : kEmptyTerm; };
+                auto &cq        = out.queries[q];
+                cq.term_begin   = uint32_t(out.terms.size());
+                cq.nterms       = uint32_t(tv.size());
+                cq.phrase_begin = uint32_t(out.phrases.size());
+                cq.prog_begin   = uint32_t(out.prog.size());
+                out.terms.insert(out.terms.end(), tv.begin(), tv.end());
+                uint32_t    sp{0}, nph{0};
+                std::string perr;
+                // post order, iteratively (trees are up to 64 levels deep): a node is emitted once all its children have been
+                std::vector<std::pair<uint32_t, uint32_t>> st{{Q.root, 0}};
+                while (!st.empty() && perr.empty()) {
+                        auto [i, c]   = st.back();
+                        const auto &X = n[i];
+                        CollectOp   o{};
+                        if (X.kind == TRN_NODE_TERM || X.kind == TRN_NODE_PHRASE) {
+                                st.pop_back();
+                                o.kind = CO_TERM;
+                                o.arg  = X.kind == TRN_NODE_TERM ? bit(X.term) : kEmptyTerm;
+                                if (X.kind == TRN_NODE_PHRASE) {
+                                        bool     all{X.nchildren >= 2 && X.nchildren <= 16 && X.first_child > i && uint32_t(X.first_child) + X.nchildren <= Q.nnodes};
+                                        uint32_t mask{0};
+                                        for (uint32_t k = 0; all && k < X.nchildren; ++k) {
+                                                const auto &C = n[X.first_child + k];
+                                                all           = C.kind == TRN_NODE_TERM && held(C.term);
+                                                if (all)
+                                                        mask |= 1u << bit(C.term);
+                                        }
+                                        if (all) { // (a phrase with a term the source does not hold matches nothing: it stays a TERM that never holds)
+                                                if (nph == kCollectMaxPhrases) {
+                                                        perr = "the default exec mode takes at most 32 phrase nodes per query";
+                                                        break;
+                                                }
+                                                CollectPhrase F{};
+                                                F.arg_begin = uint32_t(out.args.size());
+                                                F.k         = X.nchildren;
+                                                F.mask      = mask;
+                                                for (uint32_t j = 0; j < X.nchildren; j += 4) { // four term ids per OP_ARG step (phrase.cuh phrase_arg)
+                                                        auto   t = [&](uint32_t k) { return k < X.nchildren ? n[X.first_child + k].term : 0u; };
+                                                        DevStep a;
+                                                        std::memset(&a, 0, sizeof(a));
+                                                        a.op                = OP_ARG;
+                                                        a.term              = t(j);
+                                                        a.pad2              = t(j + 1);
+                                                        const uint64_t hi   = uint64_t(t(j + 2)) | (uint64_t(t(j + 3)) << 32);
+                                                        std::memcpy(&a.idf, &hi, 8);
+                                                        out.args.push_back(a);
+                                                }
+                                                out.phrases.push_back(F);
+                                                o.kind = CO_PHRASE;
+                                                o.arg  = nph++;
+                                        }
+                                }
+                        } else if (c < X.nchildren) {
+                                if (X.first_child <= i || uint32_t(X.first_child) + X.nchildren > Q.nnodes) {
+                                        perr = "children must follow their parent in the node array";
+                                        break;
+                                }
+                                st.back().second = c + 1;
+                                st.push_back({uint32_t(X.first_child) + c, 0});
+                                continue;
+                        } else {
+                                st.pop_back();
+                                if ((X.kind == TRN_NODE_NOT || X.kind == TRN_NODE_OPTIONAL) && X.nchildren != 2) {
+                                        perr = "NOT and OPTIONAL nodes have two children";
+                                        break;
+                                }
+                                o.kind      = X.kind == TRN_NODE_AND ? CO_AND : X.kind == TRN_NODE_OR ? CO_OR : X.kind == TRN_NODE_NOT ? CO_NOT : X.kind == TRN_NODE_OPTIONAL ? CO_OPTIONAL : CO_SOME;
+                                o.nchildren = X.nchildren;
+                                o.min       = uint16_t(X.kind == TRN_NODE_SOME ? std::min<uint32_t>(X.term, 0xffffu) : 0u);
+                                o.arg       = 0;
+                                sp -= X.nchildren;
+                        }
+                        out.prog.push_back(o);
+                        if (++sp > kCollectMaxStack) {
+                                perr = "the query's collect program needs more than 32 pending operands";
+                                break;
+                        }
+                }
+                if (!perr.empty())
+                        return fail(err, TRN_ERR_UNSUPPORTED, "query " + std::to_string(q) + ": " + perr);
+                cq.nphrases = nph;
+                cq.nprog    = uint32_t(out.prog.size()) - cq.prog_begin;
         }
         return TRN_OK;
 }

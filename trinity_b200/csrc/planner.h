@@ -61,9 +61,22 @@ struct BatchPlan {
         uint64_t               cand_total{0};  // top-k candidate entries
         uint64_t               postings{0}, bytes{0};
         bool                   any_phrase{false};
+        struct CollectPlan {   // TRN_MODE_MATCHED_TERMS: what the collect pass runs per match (plan_collect)
+                std::vector<CollectQuery>  queries;
+                std::vector<uint32_t>      terms;
+                std::vector<CollectPhrase> phrases;
+                std::vector<DevStep>       args;
+                std::vector<CollectOp>     prog;
+        } collect;
 };
+using CollectPlan = BatchPlan::CollectPlan;
 
-// Plans a batch (mode: TRN_MODE_*; k: top-k).  dense_off: per term, the first word of its resident bitmap (DenseSelection::off), or
+// The collect programs of a batch in the default exec mode (TRN_MODE_MATCHED_TERMS): per query its distinct terms (at most 32, ascending
+// term index), its phrase nodes (at most 32) and its nodes in post order.  TRN_ERR_UNSUPPORTED beyond those limits.
+int plan_collect(const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, CollectPlan &out, std::string &err);
+
+// Plans a batch (mode: TRN_MODE_*; k: top-k; TRN_MODE_MATCHED_TERMS: the DocumentsOnly program without the root-filter quirk, plus
+// BatchPlan::collect).  dense_off: per term, the first word of its resident bitmap (DenseSelection::off), or
 // null when the source has none.  Returns TRN_OK, or an error code with its message in err: TRN_ERR_ARG / TRN_ERR_UNSUPPORTED for a
 // plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.
 int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
