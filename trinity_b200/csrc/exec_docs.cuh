@@ -560,42 +560,38 @@ __device__ __forceinline__ void lucene_leaf_warp(const DevIndex &ix, const DevTe
                 lucene_leaf_warp_t<0>(ix, T, bA, bB, lo, hi, bs, skipfilt, stage, lane, bar_s, seq);
 }
 
-// ---- emission of a tile's root docset (a bitmap in shared memory; lane l owns words [l * NW/32, (l + 1) * NW/32))
+// ---- emission of a tile's root docset, row by row: row r is the tile's words [128 r, 128 r + 128), and lane l holds its uint4 r * 32 + l
+// (words 128 r + 4 l .. + 3).  Reading a shared-memory bitmap that way is one conflict-free 128-bit load per lane and row, and the
+// lanes of a row write their documents to neighbouring places of the segment.  A tile below 2^12 documents is part of one row
+// (lanes past its end hold zero words).
 struct TileCount {
-        uint32_t c, incl; // the lane's documents, and those of lanes 0 .. lane
-        uint32_t total;   // the tile's documents
-        uint32_t enc;     // compact results: the encoding (kEnc*)
-        uint32_t size;    // segment size: words (compact) or docIDs
+        uint32_t total; // the tile's documents
+        uint32_t enc;   // compact results: the encoding (kEnc*)
+        uint32_t size;  // segment size: words (compact) or docIDs
 };
+__device__ __forceinline__ uint32_t popc4(uint4 v) {
+        return __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w);
+}
+// one row into the lane's document count `c`; `full` (warp-uniform) becomes non-zero when a 256-docID bucket (8 words: a lane pair)
+// holds 256 documents, which do not fit the bucketed form's count byte
+__device__ __forceinline__ void count_row(uint4 v, uint32_t &c, uint32_t &full) {
+        const uint32_t pc = popc4(v);
+        c += pc;
+        const uint32_t m = __ballot_sync(0xffffffffu, pc == 128u);
+        full |= m & (m >> 1) & 0x55555555u;
+}
 // Compact results take whichever form needs the fewest words (a tile holds at most 2^16 documents):
 //   bitmap   the tile's words                                                          dense tiles (> 1 document in 8)
-//   U8B      per 256-docID bucket a count byte, then one offset byte per document      1 in 8 .. 1 in 256
+//   U8B      per 256-docID bucket a count byte, then one offset byte per document      1 in 8 .. 1 in 256 (tiles of 2^13 documents or more)
 //   U16      16-bit offsets from the tile's first docID, two per word                  sparse tiles
-// live == false: the tile matches nothing (root is not read)
-__device__ __forceinline__ TileCount tile_count(const uint32_t *root, bool live, bool compact, uint32_t W, uint32_t NW, int lane) {
-        const uint32_t wpl = NW >> 5;
-        TileCount      t;
-        uint32_t       c = 0, full = 0;
-        if (live) {
-                uint32_t cb = 0; // documents of the current 256-docID bucket (8 words): 256 of them do not fit the bucketed form's count byte
-                for (uint32_t i = 0; i < wpl; ++i) {
-                        const uint32_t pc = __popc(root[lane * wpl + i]);
-                        c += pc;
-                        cb += pc;
-                        if ((i & 7u) == 7u) {
-                                full |= cb == 256u ? 1u : 0u;
-                                cb = 0;
-                        }
-                }
-        }
-        t.c     = c;
-        t.incl  = warp_incl_scan(c, lane);
-        t.total = __shfl_sync(0xffffffffu, t.incl, 31);
+__device__ __forceinline__ TileCount tile_encoding(uint32_t c, uint32_t full, bool compact, uint32_t W, uint32_t NW) {
+        TileCount t;
+        t.total = __reduce_add_sync(0xffffffffu, c);
         t.enc   = kEncBitmap;
         t.size  = t.total;
         if (compact) {
                 const uint32_t nbk  = W >> 8;
-                const bool     u8ok = wpl >= 8u && W <= 65536u && !__any_sync(0xffffffffu, full != 0u); // a lane owns whole buckets
+                const bool     u8ok = NW >= 256u && W <= 65536u && full == 0u;
                 uint32_t       words = NW;
                 if (W <= 65536u) {
                         if (((t.total + 1u) >> 1) < words)
@@ -607,6 +603,19 @@ __device__ __forceinline__ TileCount tile_count(const uint32_t *root, bool live,
         }
         return t;
 }
+// the lane's uint4 of row r of a shared-memory bitmap (zero past the tile's end)
+__device__ __forceinline__ uint4 smem_row(const uint32_t *root, uint32_t r, uint32_t NW, int lane) {
+        const uint32_t i = r * 32u + uint32_t(lane);
+        return i < (NW >> 2) ? reinterpret_cast<const uint4 *>(root)[i] : make_uint4(0u, 0u, 0u, 0u);
+}
+// live == false: the tile matches nothing (root is not read)
+__device__ __forceinline__ TileCount tile_count(const uint32_t *root, bool live, bool compact, uint32_t W, uint32_t NW, int lane) {
+        uint32_t c = 0, full = 0;
+        if (live)
+                for (uint32_t r = 0; r * 128u < NW; ++r)
+                        count_row(smem_row(root, r, NW, lane), c, full);
+        return tile_encoding(c, full, compact, W, NW);
+}
 
 // the work item's segment record (one lane); base: the reserved segment, 0 for an empty tile, ~0 when the reservation overflowed
 __device__ __forceinline__ void tile_record(const ExecParams &P, uint32_t item, const TileCount &t, unsigned long long base) {
@@ -616,68 +625,81 @@ __device__ __forceinline__ void tile_record(const ExecParams &P, uint32_t item, 
                 P.item_desc[item] = base == ~0ull ? 0u : (t.total | t.enc << 30);
 }
 
-// the tile's matches into its segment at `base` (t.total > 0): the compact form t.enc, or plain docIDs
+// Row r of a tile into its segment `seg` (t.total > 0): the compact form t.enc, or plain docIDs.  `done`: the documents of the
+// rows before r (the same in every lane).  A lane writes its documents in docID order from the place the warp's scan gives it.
+__device__ __forceinline__ void emit_row(const ExecParams &P, const TileCount &t, uint32_t *seg, uint32_t lo, uint32_t W, uint32_t NW, uint4 v,
+                                         uint32_t r, uint32_t &done, int lane) {
+        if (P.item_desc && t.enc == kEncBitmap) {
+                // one store per 32-word quarter m of the row, all lanes in it: lane l = 8 g + q takes component i of lane 8 ((i + g) & 3) + q,
+                // so it holds word 4 q + i of quarter (i + g) & 3 for every i, and one word of every quarter
+                const uint32_t g = uint32_t(lane) >> 3, q = uint32_t(lane) & 7u;
+                const uint32_t s0 = __shfl_sync(0xffffffffu, v.x, int(8u * (g & 3u) + q)), s1 = __shfl_sync(0xffffffffu, v.y, int(8u * ((g + 1u) & 3u) + q));
+                const uint32_t s2 = __shfl_sync(0xffffffffu, v.z, int(8u * ((g + 2u) & 3u) + q)), s3 = __shfl_sync(0xffffffffu, v.w, int(8u * ((g + 3u) & 3u) + q));
+#pragma unroll
+                for (uint32_t m = 0; m < 4u; ++m) {
+                        const uint32_t i = (m - g) & 3u, wi = r * 128u + 32u * m + 4u * q + i;
+                        if (wi < NW)
+                                seg[wi] = i == 0u ? s0 : i == 1u ? s1 : i == 2u ? s2 : s3;
+                }
+                return;
+        }
+        const uint32_t c = popc4(v), incl = warp_incl_scan(c, lane);
+        uint32_t       pos = done + incl - c;
+        done += __shfl_sync(0xffffffffu, incl, 31);
+        const uint32_t wi0 = r * 128u + 4u * uint32_t(lane); // the lane's first word
+        auto           word = [&](uint32_t k) { return k == 0u ? v.x : k == 1u ? v.y : k == 2u ? v.z : v.w; };
+        if (!P.item_desc) {
+#pragma unroll 1
+                for (uint32_t k = 0; k < 4u; ++k)
+                        for (uint32_t w = word(k); w; w &= w - 1)
+                                seg[pos++] = lo + (wi0 + k) * 32u + uint32_t(__ffs(int(w)) - 1);
+        } else if (t.enc == kEncU8B) { // the lane pair (2i, 2i + 1) holds bucket 16 r + i; the even lane writes its count byte
+                uint8_t *      o8 = reinterpret_cast<uint8_t *>(seg);
+                const uint32_t cb = c + __shfl_xor_sync(0xffffffffu, c, 1);
+                if (!(lane & 1))
+                        o8[r * 16u + (uint32_t(lane) >> 1)] = uint8_t(cb);
+                pos += W >> 8;
+#pragma unroll 1
+                for (uint32_t k = 0; k < 4u; ++k)
+                        for (uint32_t w = word(k); w; w &= w - 1)
+                                o8[pos++] = uint8_t((wi0 + k) * 32u + uint32_t(__ffs(int(w)) - 1)); // (256-docID bucket offset)
+        } else {
+                uint16_t *out = reinterpret_cast<uint16_t *>(seg);
+#pragma unroll 1
+                for (uint32_t k = 0; k < 4u; ++k)
+                        for (uint32_t w = word(k); w; w &= w - 1)
+                                out[pos++] = uint16_t((wi0 + k) * 32u + uint32_t(__ffs(int(w)) - 1));
+        }
+}
+// after the last row: the pad bytes of U8B and the pad half-word of U16 travel too (t.size is not read)
+__device__ __forceinline__ void emit_pad(const ExecParams &P, const TileCount &t, uint32_t *seg, uint32_t W, int lane) {
+        if (!P.item_desc || lane != 31)
+                return;
+        if (t.enc == kEncU8B) {
+                uint8_t *o8 = reinterpret_cast<uint8_t *>(seg);
+                for (uint32_t z = (W >> 8) + t.total; z & 3u; ++z)
+                        o8[z] = 0;
+        } else if (t.enc == kEncU16 && (t.total & 1u))
+                reinterpret_cast<uint16_t *>(seg)[t.total] = 0;
+}
+
+// the tile's matches (a shared-memory bitmap) into its segment at `base` (t.total > 0)
 __device__ __forceinline__ void tile_emit(const ExecParams &P, const uint32_t *root, const TileCount &t, unsigned long long base, uint32_t lo, uint32_t W,
                                           uint32_t NW, int lane) {
-        const uint32_t wpl = NW >> 5;
-        if (!P.item_desc) {
-                unsigned long long pos = base + (t.incl - t.c);
-                for (uint32_t i = 0; i < wpl; ++i) {
-                        const uint32_t wi = lane * wpl + i;
-                        uint32_t       w  = root[wi];
-                        while (w) {
-                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                w &= w - 1;
-                                P.seg_docids[pos++] = lo + wi * 32u + bit;
-                        }
-                }
-        } else if (t.enc == kEncBitmap) {
-                for (uint32_t i = lane; i < NW; i += 32)
-                        P.seg_docids[base + i] = root[i];
-        } else if (t.enc == kEncU8B) {
-                const uint32_t nbk = W >> 8;
-                uint8_t *      o8  = reinterpret_cast<uint8_t *>(P.seg_docids + base);
-                uint32_t       pos = nbk + (t.incl - t.c), cb = 0;
-                for (uint32_t i = 0; i < wpl; ++i) {
-                        const uint32_t wi = lane * wpl + i;
-                        uint32_t       w  = root[wi];
-                        cb += __popc(w);
-                        while (w) {
-                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                w &= w - 1;
-                                o8[pos++] = uint8_t((wi & 7u) * 32u + bit);
-                        }
-                        if ((i & 7u) == 7u) {
-                                o8[wi >> 3] = uint8_t(cb);
-                                cb          = 0;
-                        }
-                }
-                if (lane == 31)
-                        for (uint32_t z = nbk + t.total; z < t.size * 4u; ++z)
-                                o8[z] = 0; // the pad bytes travel too
-        } else {
-                uint16_t *out = reinterpret_cast<uint16_t *>(P.seg_docids + base);
-                uint32_t  pos = t.incl - t.c;
-                for (uint32_t i = 0; i < wpl; ++i) {
-                        const uint32_t wi = lane * wpl + i;
-                        uint32_t       w  = root[wi];
-                        while (w) {
-                                const uint32_t bit = uint32_t(__ffs(int(w)) - 1);
-                                w &= w - 1;
-                                out[pos++] = uint16_t(wi * 32u + bit);
-                        }
-                }
-                if (lane == 31 && (t.total & 1u))
-                        out[t.total] = 0; // the pad half-word travels too
-        }
+        uint32_t *seg  = P.seg_docids + base;
+        uint32_t  done = 0;
+        for (uint32_t r = 0; r * 128u < NW; ++r)
+                emit_row(P, t, seg, lo, W, NW, smem_row(root, r, NW, lane), r, done, lane);
+        emit_pad(P, t, seg, W, lane);
 }
 
 // All-bitmap flat AND (BatchPlan::dense_runs): ticket e = {query, first tile} covers the query's tiles of one 2^kDenseAlignShift-docID run,
 // which lies wholly inside every operand's bitmap, so nothing is decoded and no block directory is searched.  The run-major order of the
 // tickets keeps every query that reads a run's bitmap words in flight together: each run of each bitmap comes from HBM about once per batch.
-// Pass 1 ANDs each tile's words (masked documents removed) into slot 0 and sizes its result; the run's segments take ONE reservation;
-// pass 2 rebuilds each non-empty tile (its words now come from L2) and writes it exactly as the per-tile path would.
-__device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, uint32_t *root, int lane) {
+// Pass 1 ANDs each tile's words (masked documents removed) row by row in registers and sizes its result; the run's segments take ONE
+// reservation; pass 2 rebuilds each non-empty tile row by row (its words now come from L2) and writes it exactly as the per-tile path
+// would.  No tile passes through shared memory.
+__device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, int lane) {
         const uint32_t q = e.x, t0 = e.y;
         const DevQuery &Q     = P.queries[q];
         const uint32_t  nt    = dense_run_end(t0, Q.tile_lo, Q.ntiles, P.exec_shift) - t0; // 1 .. 16 tiles
@@ -697,30 +719,36 @@ __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
                 const uint32_t f = P.ix.terms[myTerm].first_doc;
                 myw              = __ldg(P.ix.dense_off + myTerm) + ((lo0 - ((f >> kDenseAlignShift) << kDenseAlignShift)) >> 5);
         }
-        const uint32_t NW4 = NW >> 2;
-        uint4 *        r4  = reinterpret_cast<uint4 *>(root);
-        auto           build = [&](uint32_t j) { // tile j of the run into root
-                __syncwarp(); // every lane is done reading the previous tile
-                const uint4 *mk = P.ix.masked ? reinterpret_cast<const uint4 *>(P.ix.masked + ((lo0 >> 5) + j * NW)) : nullptr;
-                for (uint32_t i = lane; i < NW4; i += 32) {
-                        uint4 w = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
-                        if (mk) {
-                                const uint4 m = mk[i];
-                                w             = make_uint4(~m.x, ~m.y, ~m.z, ~m.w);
-                        }
-                        for (uint32_t k = 0; k < nleaf; ++k) {
-                                const uint4 v = __ldg(reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, myw, int(k)) + j * NW) + i);
-                                w             = make_uint4(w.x & v.x, w.y & v.y, w.z & v.z, w.w & v.w);
-                        }
-                        r4[i] = w;
+        // the lane's uint4 of row r of tile j of the run (a tile of a run is >= 2^13 documents: whole rows).  PASS 2 reads the words from L2 and
+        // emits: there the operands are loaded one after the other, which keeps the emitter within the register bound
+        auto row = [&](uint32_t j, uint32_t r, auto pass2) {
+                const uint32_t i = r * 32u + uint32_t(lane);
+                uint4          w = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
+                if (P.ix.masked) {
+                        const uint4 m = reinterpret_cast<const uint4 *>(P.ix.masked + ((lo0 >> 5) + j * NW))[i];
+                        w             = make_uint4(~m.x, ~m.y, ~m.z, ~m.w);
                 }
-                __syncwarp();
+                auto leaf = [&](uint32_t k) {
+                        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, myw, int(k)) + j * NW) + i);
+                        w             = make_uint4(w.x & v.x, w.y & v.y, w.z & v.z, w.w & v.w);
+                };
+                if constexpr (decltype(pass2)::value) {
+#pragma unroll 1
+                        for (uint32_t k = 0; k < nleaf; ++k)
+                                leaf(k);
+                } else {
+                        for (uint32_t k = 0; k < nleaf; ++k)
+                                leaf(k);
+                }
+                return w;
         };
         const bool compact = P.item_desc != nullptr;
         uint32_t   mydesc = 0, mysize = 0; // lane j: tile j's documents | encoding << 30 (as item_desc), and its segment size
         for (uint32_t j = 0; j < nt; ++j) {
-                build(j);
-                const TileCount tc = tile_count(root, true, compact, W, NW, lane);
+                uint32_t c = 0, full = 0;
+                for (uint32_t r = 0; r * 128u < NW; ++r)
+                        count_row(row(j, r, std::false_type()), c, full);
+                const TileCount tc = tile_encoding(c, full, compact, W, NW);
                 if (uint32_t(lane) == j) {
                         mydesc = tc.total | tc.enc << 30;
                         mysize = tc.size;
@@ -750,15 +778,20 @@ __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
         }
         if (base == ~0ull)
                 return;
+        const uint32_t myoff = incl - mysize;
         for (uint32_t j = 0; j < nt; ++j) {
-                const uint32_t off = __shfl_sync(0xffffffffu, incl - mysize, int(j));
-                if (!__shfl_sync(0xffffffffu, mytot, int(j)))
+                const uint32_t d = __shfl_sync(0xffffffffu, mydesc, int(j)), off = __shfl_sync(0xffffffffu, myoff, int(j));
+                TileCount      t;
+                t.total = d & 0x3fffffffu;
+                if (!t.total)
                         continue;
-                build(j);
-                const TileCount tc = tile_count(root, true, compact, W, NW, lane);
-                tile_emit(P, root, tc, base + off, lo0 + j * W, W, NW, lane);
+                t.enc = d >> 30;
+                uint32_t *seg  = P.seg_docids + (base + off);
+                uint32_t  done = 0;
+                for (uint32_t r = 0; r * 128u < NW; ++r)
+                        emit_row(P, t, seg, lo0 + j * W, W, NW, row(j, r, std::true_type()), r, done, lane);
+                emit_pad(P, t, seg, W, lane);
         }
-        __syncwarp();
 }
 
 #include "exec_docs_flat.cuh"
@@ -786,7 +819,6 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
         const size_t   perWarp = size_t(P.nslots) * NW * 4 + P.docs_stage_bytes;
         uint32_t *     slots = reinterpret_cast<uint32_t *>(dyn_smem + perWarp * warp);
         uint8_t *      stage = reinterpret_cast<uint8_t *>(slots + size_t(P.nslots) * NW);
-        const uint32_t wpl   = NW >> 5; // bitmap words per lane (contiguous ownership: lane l owns words [l*wpl, (l+1)*wpl))
 
         uint32_t curq = 0xffffffffu, qgen = 0; // qgen: the current query's first ticket
         DevQuery Q;
@@ -805,7 +837,7 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                         break;
                 if constexpr (!PH && !TREE && !LUC) {
                         if (gitem < P.dense_items) { // all-bitmap flat AND: the query's tiles of one run
-                                dense_run_exec(P, P.dense_runs[gitem], W, NW, slots, lane);
+                                dense_run_exec(P, P.dense_runs[gitem], W, NW, lane);
                                 continue;
                         }
                 }
@@ -941,13 +973,13 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                                 } else { // M_AND
                                         // candidates alive in dst: count + span (the GPU form of "where would advance() land")
                                         uint32_t cnt = 0, mn = 0xffffffffu, mx = 0;
-                                        for (uint32_t i = 0; i < wpl; ++i) {
-                                                const uint32_t wi = lane * wpl + i, w = dst[wi];
-                                                tmp[wi]           = 0;
+                                        for (uint32_t i = lane; i < NW; i += 32) {
+                                                const uint32_t w = dst[i];
+                                                tmp[i]           = 0;
                                                 if (w) {
                                                         cnt += __popc(w);
-                                                        mn = min(mn, wi * 32u + uint32_t(__ffs(int(w)) - 1));
-                                                        mx = wi * 32u + uint32_t(31 - __clz(int(w)));
+                                                        mn = min(mn, i * 32u + uint32_t(__ffs(int(w)) - 1));
+                                                        mx = max(mx, i * 32u + uint32_t(31 - __clz(int(w))));
                                                 }
                                         }
                                         for (int d = 16; d > 0; d >>= 1) {
