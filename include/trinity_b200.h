@@ -442,6 +442,47 @@ int trn_encode_lucene(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, co
                       uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
                       trn_term *terms, float *device_ms);
 
+/* ------------------------------------------------------------------------------------------------ query-token intersections
+ * == Trinity::intersect_impl(stopwordsMask, tokens, src, maskedDocumentsRegistry, out) (intersect.h:25-37, intersect.cpp:5-170), one call
+ * for a batch of requests over this source, with the context's masked documents as the registry.  Request i has `ngroups` <= 64 groups of
+ * synonymous tokens; group g is terms[group_offsets[g] .. group_offsets[g + 1]) (term ids of the uploaded terms table; a term listed twice
+ * in one group counts once, as in the reference's unordered_set).  A term that is TRN_EMPTY_TERM or has no documents is unknown: then the
+ * query's own mask is not excluded (origMask = 0); with no known token the result is empty.  The result of request i is every
+ * {mask, count} of the reference, ordered by popcount descending, count descending, mask ascending (the reference leaves ties in no
+ * defined order).  Refusals, never a wrong answer: more than 64 groups or more than 512 known tokens over all groups (a term in two groups
+ * counts twice) TRN_ERR_ARG; stopwords_mask != 0 TRN_ERR_UNSUPPORTED (the reference tests it against iterator slots, whose order is
+ * not reproducible); more than 65536 distinct masks in a request (TRN_ISECT_MAX_MASKS may lower the limit), or epoch arrays of more
+ * than 2^24 entries, TRN_ERR_CAPACITY, naming the request. */
+#define TRN_EMPTY_TERM 0xffffffffu
+typedef struct trn_isect_req {
+        const uint32_t *group_offsets; /* ngroups + 1 */
+        const uint32_t *terms;
+        uint32_t        ngroups;
+        uint64_t        stopwords_mask;
+} trn_isect_req;
+/* owned by the ctx, valid until the next trn_intersect call: request i owns [offsets[i], offsets[i + 1]) of masks / counts */
+typedef struct trn_intersections {
+        uint32_t        n;
+        uint64_t        total;
+        const uint64_t *offsets;
+        const uint64_t *masks;
+        const uint32_t *counts;
+        uint64_t        postings;     /* documents of the known tokens of every request (each token once per group it is in) */
+        uint64_t        distinct;     /* distinct masks over the requests (pass A's output) */
+        float           masks_ms;     /* CUDA-event time of pass A (k_isect<.., false>), kernel only */
+        float           plan_ms;      /* host time of the epoch planner over every request */
+        float           count_ms;     /* CUDA-event time of the carries and pass B (k_isect<.., true>), kernels only */
+        float           total_ms;     /* host time of the whole call */
+} trn_intersections;
+int trn_intersect(trn_ctx *, const trn_isect_req *reqs, uint32_t n, trn_intersections *out);
+/* Host-only view of the host step between the passes (tests, tooling; no GPU needed): the epochs of one request from its distinct masks and
+ * their first docIDs (csrc/isectplan.h).  max_masks = 0: the default limit.  epoch_start[0..*nepochs), epoch_off[0..*nepochs] (entries of
+ * epoch e: [epoch_off[e], epoch_off[e + 1]) of snap_mask / snap_slot, cap entries at most), final_mask[0..*nfinal) (n entries suffice for
+ * epoch_start and final_mask, n + 1 for epoch_off).  snap_slot: the entry's index in final_mask, -1 when its count is lost. */
+int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *firsts, uint32_t n, uint32_t max_masks, uint32_t *epoch_start, uint32_t *epoch_off,
+                             uint64_t *snap_mask, int32_t *snap_slot, uint64_t cap, uint32_t *nepochs, uint64_t *nentries, uint64_t *final_mask, uint32_t *nfinal,
+                             char *err, size_t errcap);
+
 #ifdef __cplusplus
 }
 #endif

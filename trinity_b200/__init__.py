@@ -12,7 +12,8 @@ from typing import Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from ._ffi import HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnMatches, TrnQuery, TrnResult, TrnTerm, TrnTimings, lib
+from ._ffi import (HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnIntersections, TrnIsectReq, TrnMatches, TrnQuery, TrnResult, TrnTerm, TrnTimings,
+                   lib)
 
 CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
@@ -181,6 +182,12 @@ class TermDictionary:
 
     def __len__(self):
         return len(self.names)
+
+    def term_id(self, name: str) -> int:
+        """the term's id, EMPTY_TERM when the dictionary does not hold it"""
+        if not hasattr(self, "_ids"):
+            self._ids = {n: i for i, n in enumerate(self.names)}
+        return self._ids.get(name, EMPTY_TERM)
 
     def __del__(self):
         try:
@@ -457,6 +464,50 @@ class MatchesResult:
             yield int(self.docids[m]), terms
 
 
+def debug_intersect_plan(masks, firsts, max_masks: int = 0):
+    """the host step of GpuIndexSource.intersect (csrc/isectplan.h) on one request's distinct masks and their first docIDs ->
+    (epoch_start, [epoch arrays as [(mask, final index or -1)]], final antichain)"""
+    m = np.ascontiguousarray(masks, np.uint64)
+    f = _u32(firsts)
+    n = len(m)
+    es, eo, fm = np.zeros(max(n, 1), np.uint32), np.zeros(n + 1, np.uint32), np.zeros(max(n, 1), np.uint64)
+    ne, nent, nf = C.c_uint32(), C.c_uint64(), C.c_uint32()
+    err = C.create_string_buffer(256)
+    cap = 1 << 12
+    while True:
+        sm, ss = np.zeros(cap, np.uint64), np.zeros(cap, np.int32)
+        rc = lib().trn_debug_intersect_plan(_ptr(m), _ptr(f), n, max_masks, _ptr(es), _ptr(eo), _ptr(sm), _ptr(ss), cap, C.byref(ne), C.byref(nent),
+                                            _ptr(fm), C.byref(nf), err, 256)
+        if rc == -6 and nent.value > cap:
+            cap = nent.value
+            continue
+        if rc != 0:
+            raise TrinityError(f"rc={rc}: {err.value.decode()}")
+        break
+    arrays = [[(int(sm[i]), int(ss[i])) for i in range(int(eo[e]), int(eo[e + 1]))] for e in range(ne.value)]
+    return [int(x) for x in es[: ne.value]], arrays, [int(x) for x in fm[: nf.value]]
+
+
+class IntersectResult:
+    """GpuIndexSource.intersect_batch: per request its [(mask, count)] in finalize()'s order (popcount, then count, descending; ties by mask),
+    and the device times of the two passes and the host time of the planner between them"""
+
+    def __init__(self, r: TrnIntersections):
+        n, tot = int(r.n), int(r.total)
+        offs = np.ctypeslib.as_array(r.offsets, shape=(n + 1,)).copy() if n else np.zeros(1, np.uint64)
+        masks = np.ctypeslib.as_array(r.masks, shape=(max(tot, 1),))[:tot].copy() if tot else np.zeros(0, np.uint64)
+        counts = np.ctypeslib.as_array(r.counts, shape=(max(tot, 1),))[:tot].copy() if tot else np.zeros(0, np.uint32)
+        self.results = [[(int(masks[j]), int(counts[j])) for j in range(int(offs[i]), int(offs[i + 1]))] for i in range(n)]
+        self.postings, self.distinct = int(r.postings), int(r.distinct)
+        self.masks_ms, self.plan_ms, self.count_ms, self.total_ms = float(r.masks_ms), float(r.plan_ms), float(r.count_ms), float(r.total_ms)
+
+    def __getitem__(self, i: int):
+        return self.results[i]
+
+    def __len__(self):
+        return len(self.results)
+
+
 class GpuIndexSource:
     """== one device-resident IndexSource + AccessProxy (index_source.h:18-155, codecs.h:290-317) and the batch form of
     exec_query() (exec.h:50-52) over it."""
@@ -575,6 +626,28 @@ class GpuIndexSource:
         self._ck(self._L.trn_exec_matches(self._h, C.cast(arr, C.c_void_p), len(queries), C.byref(r)))
         self._last = (MODE_MATCHED_TERMS, 0, len(queries))
         return MatchesResult(r)
+
+    def intersect_batch(self, requests: Sequence[Sequence[Sequence[int]]], stopwords_mask: int = 0) -> IntersectResult:
+        """== Trinity::intersect_impl(stopwordsMask, tokens, src, maskedDocumentsRegistry) (intersect.cpp:5-170) for every request in one
+        call: a request is a list of up to 64 groups of synonymous term ids (EMPTY_TERM: a token the source does not know); bit g of a
+        result mask stands for group g.  The masked documents set on this source are the registry."""
+        keep, arr = [], (TrnIsectReq * max(len(requests), 1))()
+        for i, groups in enumerate(requests):
+            offs = _u32(np.concatenate([[0], np.cumsum([len(g) for g in groups])]) if len(groups) else [0])
+            terms = _u32([t for g in groups for t in g] or [0])
+            keep += [offs, terms]
+            arr[i] = TrnIsectReq(offs.ctypes.data, terms.ctypes.data, len(groups), stopwords_mask)
+        r = TrnIntersections()
+        self._ck(self._L.trn_intersect(self._h, C.cast(arr, C.c_void_p), len(requests), C.byref(r)))
+        return IntersectResult(r)
+
+    def intersect(self, groups: Sequence[Sequence[int]], stopwords_mask: int = 0):
+        """one request of intersect_batch -> [(mask, count)]"""
+        return self.intersect_batch([groups], stopwords_mask)[0]
+
+    def intersect_tokens(self, token_groups: Sequence[Sequence[str]], tdict: "TermDictionary", stopwords_mask: int = 0):
+        """intersect() with the tokens named: each resolved through the source's dictionary (unknown names are unknown tokens)"""
+        return self.intersect([[tdict.term_id(t) for t in g] for g in token_groups], stopwords_mask)
 
     def last_timings(self) -> dict:
         """host-side breakdown (ms) of the last exec_batch / exec_batch_device call"""

@@ -22,7 +22,7 @@ EXPORTS = [
     "trn_exec_batch", "trn_exec_batch_device", "trn_last_topk_device", "trn_merge_topk", "trn_fetch_results", "trn_last_timings",
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_encode_lucene", "trn_debug_chunk_plan",
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
-    "trn_exec_matches", "trn_debug_hits",
+    "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -61,6 +61,16 @@ class TrnMatches(C.Structure):
                 ("doc_offsets", C.POINTER(C.c_uint64)), ("docids", C.POINTER(C.c_uint32)), ("term_offsets", C.POINTER(C.c_uint64)),
                 ("terms", C.POINTER(C.c_uint32)), ("freqs", C.POINTER(C.c_uint32)), ("hit_offsets", C.POINTER(C.c_uint64)), ("hits", C.c_void_p),
                 ("device_ms", C.c_float), ("docs_ms", C.c_float), ("count_ms", C.c_float), ("write_ms", C.c_float), ("chunks", C.c_uint32)]
+
+
+class TrnIsectReq(C.Structure):
+    _fields_ = [("group_offsets", C.c_void_p), ("terms", C.c_void_p), ("ngroups", C.c_uint32), ("stopwords_mask", C.c_uint64)]
+
+
+class TrnIntersections(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("total", C.c_uint64), ("offsets", C.POINTER(C.c_uint64)), ("masks", C.POINTER(C.c_uint64)),
+                ("counts", C.POINTER(C.c_uint32)), ("postings", C.c_uint64), ("distinct", C.c_uint64), ("masks_ms", C.c_float),
+                ("plan_ms", C.c_float), ("count_ms", C.c_float), ("total_ms", C.c_float)]
 
 
 CONSIDER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
@@ -159,5 +169,7 @@ def lib() -> C.CDLL:
     sig("trn_debug_dense_runs", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     sig("trn_debug_dense_bitmap", i32, vp, u32, vp, u64, P(u64), P(u64))
     sig("trn_debug_dense_terms", i32, i32, vp, u64, vp, u32, vp, P(u32), P(u64), C.c_char_p, C.c_size_t)
+    sig("trn_intersect", i32, vp, vp, u32, P(TrnIntersections))
+    sig("trn_debug_intersect_plan", i32, vp, vp, u32, u32, vp, vp, vp, vp, u64, P(u32), P(u64), vp, P(u32), C.c_char_p, C.c_size_t)
     _lib = L
     return L

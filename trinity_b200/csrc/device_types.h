@@ -281,4 +281,46 @@ struct CollectParams {
         uint32_t *           error;        // != 0: a match the collect program does not accept (a docs-pass / program disagreement)
 };
 
+// ---- query-token intersections (trn_intersect; intersect.cuh, isectplan.h)
+// a warp's group bitmaps hold 2^16 bits (intersect.cuh): a request with G groups cuts the docID space into tiles of 2^16 / max(8, G rounded up
+// to a power of two) documents, 2^13 .. 2^10
+inline uint32_t isect_tile_shift(uint32_t ngroups) {
+        uint32_t lg = 3;
+        while ((1u << lg) < ngroups)
+                ++lg;
+        return 16u - lg;
+}
+struct IsectReq {
+        uint32_t tok_begin, ntok;     // its known tokens: IsectParams::tok[tok_begin .. + ntok), {term, group}
+        uint32_t ngroups, shift;      // groups; log2 of its docID tile (isect_tile_shift: the more groups, the smaller the tile)
+        uint32_t tile_lo, ntiles;     // tiles [tile_lo, tile_lo + ntiles) of 2^shift docIDs
+        uint32_t item_base;           // its first work item
+        uint32_t epoch_begin;         // pass B: its first epoch (global numbering of IsectParams::epoch_start / epoch_off)
+        uint32_t nepochs;             // ...
+        uint32_t pad;
+        uint64_t orig_mask;           // documents holding exactly this mask are not considered (0: some token is unknown)
+        uint64_t slots, table_base;   // pass A: its open-addressing table of distinct masks (slots: a power of two)
+};
+struct IsectParams {
+        DevIndex        ix;
+        const IsectReq *reqs;
+        const uint2 *   tok;
+        uint32_t        nreq, total_items;
+        uint32_t        max_masks; // distinct masks a request may have
+        uint32_t *      ticket;
+        uint32_t *      error; // pass A: a table overflowed; pass B: a document found no target (internal bound violated)
+        // pass A
+        unsigned long long *keys;      // per table slot: the mask (0: empty)
+        uint32_t *          first;     // per table slot: its first docID (atomicMin)
+        uint32_t *          ndist;     // per request: distinct masks inserted
+        unsigned long long *tile_last; // per work item: the mask of its last considered document (0: none)
+        // pass B
+        const unsigned long long *carry;      // per work item: the mask of the last considered document before its tile (0: none)
+        const uint32_t *          epoch_start; // per epoch: the docID of the push that starts it
+        const uint32_t *          epoch_off;   // per epoch + 1: its array is entries [epoch_off[e], epoch_off[e + 1])
+        const unsigned long long *snap_mask;   // per entry: the mask
+        const int32_t *           snap_slot;   // per entry: its slot in counts (-1: removed later, its count is lost)
+        uint32_t *                counts;      // per final antichain entry of every request
+};
+
 } // namespace trn

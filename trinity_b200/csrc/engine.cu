@@ -8,12 +8,14 @@
 #include "device_types.h"
 #include "hitcursor.h"
 #include "chunkplan.h"
+#include "isectplan.h"
 #include "kernels.h"
 #include "planner.h"
 #include <algorithm>
 #include <array>
 #include <chrono>
 #include <cmath>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <limits>
@@ -155,6 +157,22 @@ struct trn_ctx {
                 }
         } mt;
         uint64_t match_chunk{1ull << 22}; // TRN_MATCH_CHUNK: matches per chunk of the write pass (halved while its outputs do not fit)
+        // query-token intersections (trn_intersect): device scratch of both passes, the result
+        struct IsectBufs {
+                DevBuf d_reqs, d_tok, d_small, d_keys, d_first, d_tile_last, d_carry, d_base, d_cmask, d_cfirst, d_estart, d_eoff, d_smask, d_sslot, d_counts;
+                std::vector<uint64_t> offsets, masks;
+                std::vector<uint32_t> counts;
+                cudaEvent_t ev[4]{nullptr, nullptr, nullptr, nullptr};
+                void release() {
+                        for (DevBuf *b : {&d_reqs, &d_tok, &d_small, &d_keys, &d_first, &d_tile_last, &d_carry, &d_base, &d_cmask, &d_cfirst, &d_estart, &d_eoff, &d_smask,
+                                          &d_sslot, &d_counts})
+                                b->release();
+                        for (cudaEvent_t e : ev)
+                                if (e)
+                                        cudaEventDestroy(e);
+                }
+        } it;
+        uint32_t isect_max_masks{kIsectMaxMasks}; // TRN_ISECT_MAX_MASKS: distinct masks a request may have (lowers the limit only)
 };
 
 #define CK(call)                                                                                                                                               \
@@ -231,6 +249,11 @@ extern "C" int trn_create(int device, trn_ctx **out) {
                 if (v >= 1)
                         c->match_chunk = uint64_t(v);
         }
+        if (const char *e = getenv("TRN_ISECT_MAX_MASKS")) {
+                const long long v = atoll(e);
+                if (v >= 1 && v < (long long)kIsectMaxMasks)
+                        c->isect_max_masks = uint32_t(v);
+        }
         CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
                 CK(cudaEventCreateWithFlags(&c->ev_done[i], cudaEventDisableTiming));
@@ -268,6 +291,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
                         cudaEventDestroy(c->ev_ck1[i]);
         }
         c->mt.release();
+        c->it.release();
         if (c->copy_stream)
                 cudaStreamDestroy(c->copy_stream);
         delete c;
@@ -1863,5 +1887,276 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                 CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
                 *device_ms = ms;
         }
+        return TRN_OK;
+}
+
+// =================================================================================================== query-token intersections
+// Two device passes with the epoch planner between them (intersect.cuh, isectplan.h; DESIGN.md §4).  Three host synchronisations: the
+// distinct-mask counts after pass A (to refuse a request over the limit and to lay out the dense copy), that copy, and the counts.
+extern "C" int trn_intersect(trn_ctx *c, const trn_isect_req *reqs, uint32_t n, trn_intersections *out) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (!out || (n && !reqs))
+                return fail(c, TRN_ERR_ARG, "trn_intersect: bad arguments");
+        if (!c->have_index)
+                return fail(c, TRN_ERR_STATE, "no index uploaded");
+        if (c->pc.codec == TRN_CODEC_GOOGLE && c->block_docs != 32)
+                return fail(c, TRN_ERR_UNSUPPORTED, "the uploaded index was built with a block size other than the reference format's (decode sweep only)");
+        CK(cudaSetDevice(c->device));
+        std::memset(out, 0, sizeof(*out));
+        const double t0 = now_ms();
+        auto &       B  = c->it;
+        if (!B.ev[0])
+                for (cudaEvent_t &e : B.ev)
+                        CK(cudaEventCreate(&e));
+
+        // ---- the requests: known tokens (deduplicated per group), tile geometry, mask tables
+        std::vector<IsectReq> rq(n);
+        std::vector<uint2>    tok;
+        uint64_t              items = 0, slots = 0, postings = 0;
+        for (uint32_t i = 0; i < n; ++i) {
+                const trn_isect_req &q   = reqs[i];
+                const std::string    who = "trn_intersect: request " + std::to_string(i) + ": ";
+                if (q.ngroups > 64)
+                        return fail(c, TRN_ERR_ARG, who + std::to_string(q.ngroups) + " token groups (at most 64: one bit of a 64-bit mask each)");
+                if (q.stopwords_mask)
+                        return fail(c, TRN_ERR_UNSUPPORTED, who + "a non-zero stopwords mask (the reference tests it against iterator slots, whose order is not reproducible)");
+                if (q.ngroups && !q.group_offsets)
+                        return fail(c, TRN_ERR_ARG, who + "null group_offsets");
+                IsectReq &R = rq[i];
+                std::memset(&R, 0, sizeof(R));
+                R.tok_begin = uint32_t(tok.size());
+                R.ngroups   = q.ngroups;
+                R.shift     = isect_tile_shift(q.ngroups);
+                bool     unknown{false};
+                uint64_t orig{0}, docs{0};
+                uint32_t lo{0xffffffffu}, hi{0};
+                for (uint32_t g = 0; g < q.ngroups; ++g) {
+                        const uint32_t a = q.group_offsets[g], b = q.group_offsets[g + 1];
+                        if (b < a || (b > a && !q.terms))
+                                return fail(c, TRN_ERR_ARG, who + "group_offsets must not decrease, and terms must be given");
+                        std::vector<uint32_t> ts(q.terms + a, q.terms + b);
+                        std::sort(ts.begin(), ts.end());
+                        ts.erase(std::unique(ts.begin(), ts.end()), ts.end());
+                        for (const uint32_t t : ts) {
+                                if (t != TRN_EMPTY_TERM && t >= c->nterms)
+                                        return fail(c, TRN_ERR_ARG, who + "term id " + std::to_string(t) + " out of range");
+                                if (t == TRN_EMPTY_TERM || !c->h_terms[t].documents) {
+                                        unknown = true;
+                                        continue;
+                                }
+                                const DevTerm &T = c->h_terms[t];
+                                tok.push_back(make_uint2(t, g));
+                                orig |= 1ull << g;
+                                lo = std::min(lo, T.first_doc);
+                                hi = std::max(hi, T.last_doc);
+                                docs += T.documents;
+                        }
+                }
+                R.ntok = uint32_t(tok.size()) - R.tok_begin;
+                if (R.ntok > 512)
+                        return fail(c, TRN_ERR_ARG, who + std::to_string(R.ntok) + " known tokens (at most 512, the reference's iterator slots; a token in two groups takes two)");
+                postings += docs;
+                R.orig_mask  = unknown ? 0ull : orig;
+                R.item_base  = uint32_t(items);
+                R.table_base = slots;
+                if (!R.ntok)
+                        continue; // nothing to intersect: an empty result
+                R.tile_lo = lo >> R.shift;
+                R.ntiles  = (hi >> R.shift) - R.tile_lo + 1u;
+                items += R.ntiles;
+                uint64_t bound = std::min<uint64_t>(c->isect_max_masks, docs); // distinct masks can be no more than the documents ...
+                if (q.ngroups < 64)
+                        bound = std::min<uint64_t>(bound, (1ull << q.ngroups) - 1u); // ... or the non-empty masks
+                uint64_t s = 64;
+                while (s < 2u * (bound + 1u)) // one more than the limit must fit, to be seen
+                        s <<= 1;
+                R.slots = s;
+                slots += s;
+        }
+        if (items >= (1ull << 31))
+                return fail(c, TRN_ERR_CAPACITY, "trn_intersect: the batch covers " + std::to_string(items) + " docID tiles; split it");
+
+        auto upload = [&](DevBuf &b, const void *src, size_t bytes) -> cudaError_t {
+                if (const cudaError_t e = b.ensure(std::max<size_t>(16, bytes)); e != cudaSuccess)
+                        return e;
+                return bytes ? cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
+        };
+        const bool  luc = c->pc.codec == TRN_CODEC_LUCENE;
+        IsectParams P;
+        std::memset(&P, 0, sizeof(P));
+        P.ix          = dev_index(c);
+        P.nreq        = n;
+        P.total_items = uint32_t(items);
+        P.max_masks   = c->isect_max_masks;
+        // small: ticket, error, ndist[n], compact cursors[n]
+        CK(B.d_small.ensure((2 + 2 * size_t(n)) * 4));
+        CK(cudaMemsetAsync(B.d_small.p, 0, (2 + 2 * size_t(n)) * 4, c->stream));
+        P.ticket = B.d_small.as<uint32_t>();
+        P.error  = P.ticket + 1;
+        P.ndist  = P.ticket + 2;
+        CK(upload(B.d_tok, tok.data(), tok.size() * sizeof(uint2)));
+        P.tok = B.d_tok.as<uint2>();
+        CK(B.d_keys.ensure(std::max<size_t>(16, slots * 8)));
+        CK(B.d_first.ensure(std::max<size_t>(16, slots * 4)));
+        CK(B.d_tile_last.ensure(std::max<size_t>(16, items * 8)));
+        CK(cudaMemsetAsync(B.d_keys.p, 0, slots * 8, c->stream));
+        CK(cudaMemsetAsync(B.d_first.p, 0xff, slots * 4, c->stream));
+        P.keys      = B.d_keys.as<unsigned long long>();
+        P.first     = B.d_first.as<uint32_t>();
+        P.tile_last = B.d_tile_last.as<unsigned long long>();
+
+        // ---- pass A: the distinct masks of every request with their first docIDs, and every tile's last considered mask
+        CK(upload(B.d_reqs, rq.data(), rq.size() * sizeof(IsectReq)));
+        P.reqs = B.d_reqs.as<IsectReq>();
+        CK(cudaEventRecord(B.ev[0], c->stream));
+        if (items)
+                CK(launch_isect(P, luc, false, c->num_sms, c->stream));
+        CK(cudaEventRecord(B.ev[1], c->stream));
+        std::vector<uint32_t> small(2 + size_t(n));
+        CK(cudaMemcpyAsync(small.data(), B.d_small.p, small.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        for (uint32_t i = 0; i < n; ++i)
+                if (small[2 + i] > c->isect_max_masks)
+                        return fail(c, TRN_ERR_CAPACITY, "trn_intersect: request " + std::to_string(i) + " has more than " + std::to_string(c->isect_max_masks) +
+                                                              " distinct token masks; TRN_ISECT_MAX_MASKS may only lower that limit");
+        if (small[1])
+                return fail(c, TRN_ERR_CAPACITY, "trn_intersect: a mask table overflowed (internal bound violated)");
+        float masksMs{0};
+        (void)cudaEventElapsedTime(&masksMs, B.ev[0], B.ev[1]);
+
+        // ---- the distinct masks, densely, to the host
+        std::vector<uint64_t> base(size_t(n) + 1, 0);
+        for (uint32_t i = 0; i < n; ++i)
+                base[i + 1] = base[i] + small[2 + i];
+        const uint64_t        D = base[n];
+        std::vector<uint64_t> hmask(D);
+        std::vector<uint32_t> hfirst(D);
+        if (D) {
+                CK(upload(B.d_base, base.data(), base.size() * 8));
+                CK(B.d_cmask.ensure(D * 8));
+                CK(B.d_cfirst.ensure(D * 4));
+                CK(launch_isect_compact(P, slots, B.d_base.as<uint64_t>(), P.ndist + n, B.d_cmask.as<unsigned long long>(), B.d_cfirst.as<uint32_t>(), c->num_sms,
+                                        c->stream));
+                CK(cudaMemcpyAsync(hmask.data(), B.d_cmask.p, D * 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaMemcpyAsync(hfirst.data(), B.d_cfirst.p, D * 4, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaStreamSynchronize(c->stream));
+        }
+
+        // ---- host step: every request's epochs and their arrays
+        const double          th = now_ms();
+        std::vector<uint32_t> estart, eoff;
+        std::vector<uint64_t> smask, fmask;
+        std::vector<int32_t>  sslot;
+        std::vector<uint64_t> fbase(size_t(n) + 1, 0);
+        for (uint32_t i = 0; i < n; ++i) {
+                IsectPlan   pl;
+                std::string err;
+                if (isect_plan(hmask.data() + base[i], hfirst.data() + base[i], small[2 + i], c->isect_max_masks, pl, err))
+                        return fail(c, TRN_ERR_CAPACITY, "trn_intersect: request " + std::to_string(i) + ": " + err);
+                IsectReq &R   = rq[i];
+                R.epoch_begin = uint32_t(estart.size());
+                R.nepochs     = uint32_t(pl.epoch_start.size());
+                const uint32_t sb = uint32_t(smask.size()), fb = uint32_t(fmask.size());
+                estart.insert(estart.end(), pl.epoch_start.begin(), pl.epoch_start.end());
+                for (size_t e = 0; e < pl.epoch_start.size(); ++e)
+                        eoff.push_back(sb + pl.epoch_off[e]);
+                smask.insert(smask.end(), pl.snap_mask.begin(), pl.snap_mask.end());
+                for (const int32_t s : pl.snap_slot)
+                        sslot.push_back(s < 0 ? -1 : int32_t(fb) + s);
+                fmask.insert(fmask.end(), pl.final_mask.begin(), pl.final_mask.end());
+                fbase[i + 1] = fmask.size();
+        }
+        eoff.push_back(uint32_t(smask.size()));
+        const float planMs = float(now_ms() - th);
+
+        // ---- pass B: every considered document's contribution to its target's final count
+        std::vector<uint32_t> counts(fmask.size());
+        float                 countMs{0};
+        if (D) {
+                CK(upload(B.d_reqs, rq.data(), rq.size() * sizeof(IsectReq)));
+                CK(upload(B.d_estart, estart.data(), estart.size() * 4));
+                CK(upload(B.d_eoff, eoff.data(), eoff.size() * 4));
+                CK(upload(B.d_smask, smask.data(), smask.size() * 8));
+                CK(upload(B.d_sslot, sslot.data(), sslot.size() * 4));
+                CK(B.d_counts.ensure(std::max<size_t>(16, counts.size() * 4)));
+                CK(cudaMemsetAsync(B.d_counts.p, 0, counts.size() * 4, c->stream));
+                CK(B.d_carry.ensure(std::max<size_t>(16, items * 8)));
+                CK(cudaMemsetAsync(P.ticket, 0, 4, c->stream));
+                P.carry       = B.d_carry.as<unsigned long long>();
+                P.epoch_start = B.d_estart.as<uint32_t>();
+                P.epoch_off   = B.d_eoff.as<uint32_t>();
+                P.snap_mask   = B.d_smask.as<unsigned long long>();
+                P.snap_slot   = B.d_sslot.as<int32_t>();
+                P.counts      = B.d_counts.as<uint32_t>();
+                CK(cudaEventRecord(B.ev[2], c->stream));
+                CK(launch_isect_carry(P, B.d_carry.as<unsigned long long>(), c->stream));
+                CK(launch_isect(P, luc, true, c->num_sms, c->stream));
+                CK(cudaEventRecord(B.ev[3], c->stream));
+                CK(cudaMemcpyAsync(counts.data(), B.d_counts.p, counts.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaMemcpyAsync(small.data(), B.d_small.p, 8, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaStreamSynchronize(c->stream));
+                if (small[1])
+                        return fail(c, TRN_ERR_STATE, "trn_intersect: a considered document found no entry in its epoch's array (internal error)");
+                (void)cudaEventElapsedTime(&countMs, B.ev[2], B.ev[3]);
+        }
+
+        // ---- the result, in finalize()'s order with ties broken by mask
+        B.offsets.assign(size_t(n) + 1, 0);
+        B.masks.clear();
+        B.counts.clear();
+        for (uint32_t i = 0; i < n; ++i) {
+                std::vector<uint32_t> ord(fbase[i + 1] - fbase[i]);
+                std::iota(ord.begin(), ord.end(), uint32_t(fbase[i]));
+                std::sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return isect_result_less(fmask[a], counts[a], fmask[b], counts[b]); });
+                for (const uint32_t j : ord) {
+                        B.masks.push_back(fmask[j]);
+                        B.counts.push_back(counts[j]);
+                }
+                B.offsets[i + 1] = B.masks.size();
+        }
+        out->n        = n;
+        out->total    = B.masks.size();
+        out->offsets  = B.offsets.data();
+        out->masks    = B.masks.data();
+        out->counts   = B.counts.data();
+        out->postings = postings;
+        out->distinct = D;
+        out->masks_ms = masksMs;
+        out->plan_ms  = planMs;
+        out->count_ms = countMs;
+        out->total_ms = float(now_ms() - t0);
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *firsts, uint32_t n, uint32_t max_masks, uint32_t *epoch_start, uint32_t *epoch_off,
+                                        uint64_t *snap_mask, int32_t *snap_slot, uint64_t cap, uint32_t *nepochs, uint64_t *nentries, uint64_t *final_mask,
+                                        uint32_t *nfinal, char *err, size_t errcap) {
+        auto say = [&](const std::string &m) {
+                if (err && errcap)
+                        snprintf(err, errcap, "%s", m.c_str());
+        };
+        if ((n && (!masks || !firsts)) || !epoch_start || !epoch_off || !nepochs || !nentries || !final_mask || !nfinal || (cap && (!snap_mask || !snap_slot))) {
+                say("trn_debug_intersect_plan: bad arguments");
+                return TRN_ERR_ARG;
+        }
+        IsectPlan   pl;
+        std::string e;
+        if (isect_plan(masks, firsts, n, max_masks ? max_masks : kIsectMaxMasks, pl, e)) {
+                say(e);
+                return TRN_ERR_CAPACITY;
+        }
+        *nepochs  = uint32_t(pl.epoch_start.size());
+        *nentries = pl.snap_mask.size();
+        *nfinal   = uint32_t(pl.final_mask.size());
+        if (pl.snap_mask.size() > cap) {
+                say("trn_debug_intersect_plan: " + std::to_string(pl.snap_mask.size()) + " entries do not fit");
+                return TRN_ERR_CAPACITY;
+        }
+        std::copy(pl.epoch_start.begin(), pl.epoch_start.end(), epoch_start);
+        std::copy(pl.epoch_off.begin(), pl.epoch_off.end(), epoch_off);
+        std::copy(pl.snap_mask.begin(), pl.snap_mask.end(), snap_mask);
+        std::copy(pl.snap_slot.begin(), pl.snap_slot.end(), snap_slot);
+        std::copy(pl.final_mask.begin(), pl.final_mask.end(), final_mask);
         return TRN_OK;
 }

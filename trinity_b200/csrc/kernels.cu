@@ -1073,6 +1073,7 @@ __global__ void __launch_bounds__(kThreads) k_decode_terms(DevIndex ix, const ui
 #include "encode_google.cuh"
 #include "encode_lucene.cuh"
 #include "collect.cuh"
+#include "intersect.cuh"
 
 // ------------------------------------------------------------------------------------------------ launch wrappers
 uint32_t exec_stage_bytes(int codec) {

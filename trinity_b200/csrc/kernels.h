@@ -44,6 +44,12 @@ cudaError_t launch_enc_lucene_write(const EncLuceneParams &E, cudaStream_t strea
 cudaError_t launch_collect_count(const CollectParams &P, cudaStream_t stream); // the default exec mode's collect pass (collect.cuh)
 cudaError_t launch_collect_write(const CollectParams &P, cudaStream_t stream);
 uint32_t    kernel_max_k();
+// query-token intersections (intersect.cuh): pass A (passb false) / pass B of trn_intersect, the dense copy of the distinct masks, the tiles' carries
+size_t      isect_smem_bytes();
+cudaError_t launch_isect(const IsectParams &P, bool lucene, bool passb, int num_sms, cudaStream_t stream);
+cudaError_t launch_isect_compact(const IsectParams &P, uint64_t total_slots, const uint64_t *base, uint32_t *cursor, unsigned long long *out_mask, uint32_t *out_first,
+                                 int num_sms, cudaStream_t stream);
+cudaError_t launch_isect_carry(const IsectParams &P, unsigned long long *carry, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
 } // namespace trn

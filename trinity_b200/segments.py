@@ -60,6 +60,15 @@ class SegmentCollection:
             out.append(nodes)
         return out
 
+    def intersect(self, token_groups: Sequence[Sequence[str]]):
+        """== Trinity::intersect(0, tokens, collection) (intersect.cpp:172-201): every source's intersections with the updated documents of
+        the newer sources masked, the tokens resolved per segment dictionary; concatenated, ordered by mask, equal masks summed"""
+        acc = {}
+        for g, d in zip(self.sources, self.dicts):
+            for m, c in g.intersect_tokens(token_groups, d):
+                acc[m] = acc.get(m, 0) + c
+        return sorted(acc.items())
+
     def exec_batch(self, queries: Sequence[str], mode: int, k: int = 100):
         """-> [BatchResult per segment], collection order (newest first)"""
         from . import MODE_DOCS_ONLY
