@@ -483,6 +483,56 @@ int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *firsts, uint
                              uint64_t *snap_mask, int32_t *snap_slot, uint64_t cap, uint32_t *nepochs, uint64_t *nentries, uint64_t *final_mask, uint32_t *nfinal,
                              char *err, size_t errcap);
 
+/* ------------------------------------------------------------------------------------------------ percolator
+ * == Trinity's percolator_query(q).match(proxy) (percolator.h, percolator.cpp) for every registered query and every document of a batch:
+ * which stored queries match an incoming document.  A ctx holds at most one registered query set; it needs no uploaded index, and a ctx
+ * may hold an index and a registry at once.
+ *   Registry   trn_percolator_register: the same trn_qnode trees trn_exec_batch takes; query ids are indices into `queries`; registering
+ *              again replaces the set.  Term ids index a percolator vocabulary of `nterms` terms; TRN_EMPTY_TERM is a query term outside it.
+ *              term_cost (optional, nterms entries; NULL: all equal), e.g. each term's document frequency, only chooses the anchors.
+ *   Documents  trn_percolate: document d is tokens[doc_offsets[d] .. doc_offsets[d + 1]) and token i sits at position i + 1; a token
+ *              outside the vocabulary is TRN_EMPTY_TERM: it takes up a position and equals no query term, not even TRN_EMPTY_TERM.
+ *   Meaning    query q matches document d exactly when percolator_query(q).match(proxy) returns true for the proxy whose match_term(t) says
+ *              whether the document holds the token t, and whose match_phrase(t0..tk) whether, at some position p, the tokens at p .. p + k
+ *              are t0 .. tk.  TERM / AND / OR / NOT (the first operand and none of the others) / OPTIONAL (its main side) / SOME (at least
+ *              `min` >= 1 operands) / PHRASE mean what matchterm / logicaland / logicalor / logicalnot / consttrueexpr beside a conjunction /
+ *              matchsome / matchphrase evaluate to.  A const-true expression that does not stand beside a conjunction operand (`<a>`,
+ *              `<a> OR <b>`) has no tree form: the front-end drops its wrapper, and the tree means the exec_query meaning.
+ *   Refusals   never a wrong answer.  TRN_ERR_ARG, naming the query or document: a malformed tree (the plan compiler's structural checks), a
+ *              phrase of more than 16 terms (Limits::MaxPhraseSize), a term id >= nterms other than TRN_EMPTY_TERM, a document token >= nterms
+ *              other than TRN_EMPTY_TERM, a document of more than 16383 tokens (positions below Limits::MaxPosition).  TRN_ERR_UNSUPPORTED:
+ *              a query whose post-order program needs more than 64 pending operands (an operator with more than 64 operands).
+ *              TRN_ERR_STATE: trn_percolate without a registry.  TRN_ERR_CAPACITY: the batch's matches cannot be staged (split the batch). */
+typedef struct trn_percolator_info {
+        uint32_t nqueries;
+        uint32_t unanchored;     /* queries a match may hold none of the terms of (evaluated for every document) */
+        uint32_t never;          /* queries no document can match (never evaluated) */
+        uint32_t pad;
+        uint64_t anchor_entries; /* (term, query) entries of the term -> anchored-queries index */
+        uint64_t device_bytes;   /* the registry in HBM */
+} trn_percolator_info;
+int trn_percolator_register(trn_ctx *, const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, trn_percolator_info *out);
+/* owned by the ctx, valid until the next trn_percolate: document d owns [offsets[d], offsets[d + 1]) of queries (ascending, no duplicates) */
+typedef struct trn_percolation {
+        uint32_t        ndocs;
+        uint32_t        long_docs;  /* documents of more than 512 tokens (the long launch: larger shared tables) */
+        uint32_t        dense_docs; /* documents of more than 4096 matches (ids emitted from a bitmap over the query ids, not sorted in shared memory) */
+        uint32_t        pad;
+        uint64_t        total;
+        const uint64_t *offsets;
+        const uint32_t *queries;
+        uint64_t        candidates; /* (document, query) pairs evaluated */
+        float           count_ms;   /* CUDA-event time of the count pass and the scan of the counts (kernels only) */
+        float           write_ms;   /* CUDA-event time of the write pass (kernels only) */
+        float           total_ms;   /* host time of the whole call */
+} trn_percolation;
+int trn_percolate(trn_ctx *, const uint64_t *doc_offsets, const uint32_t *tokens, uint32_t ndocs, trn_percolation *out);
+/* Host-only view of the registration planner (csrc/percplan.h; tests, tooling; no GPU needed): status[q] = 0 anchored, 1 unanchored, 2 no
+ * document can match; query q's anchor cover (ascending term id) = cover_terms[cover_off[q] .. cover_off[q + 1]) (nq + 1 offsets, at most cap
+ * terms: TRN_ERR_CAPACITY beyond, *ncover = the number needed).  The refusals of trn_percolator_register. */
+int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, uint8_t *status, uint32_t *cover_off,
+                              uint32_t *cover_terms, uint64_t cap, uint64_t *ncover, char *err, size_t errcap);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,8 +12,8 @@ from typing import Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from ._ffi import (HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnIntersections, TrnIsectReq, TrnMatches, TrnQuery, TrnResult, TrnTerm, TrnTimings,
-                   lib)
+from ._ffi import (HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnIntersections, TrnIsectReq, TrnMatches, TrnPercolation, TrnPercolatorInfo, TrnQuery,
+                   TrnResult, TrnTerm, TrnTimings, lib)
 
 CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
@@ -738,6 +738,27 @@ class GpuIndexSource:
                                            _ptr(hits), hcap, C.byref(hb), _ptr(terms), C.byref(ms)))
         return index[:nb.value].copy(), hits[:hb.value].copy(), terms, float(ms.value)
 
+    def percolator_register(self, queries: Sequence[np.ndarray], nterms: int, term_cost=None) -> dict:
+        """registers the query set of this context's percolator (replacing any earlier one): query ids are indices into `queries`; term ids
+        index a vocabulary of nterms terms; term_cost (e.g. document frequencies) only chooses the anchors"""
+        arr, keep = _pack_queries(queries)
+        cost = None if term_cost is None else _u32(term_cost)
+        if cost is not None and len(cost) != nterms:
+            raise TrinityError("term_cost needs one entry per vocabulary term")
+        i = TrnPercolatorInfo()
+        self._ck(self._L.trn_percolator_register(self._h, C.cast(arr, C.c_void_p), len(queries), nterms, _ptr(cost) if cost is not None else None,
+                                                 C.byref(i)))
+        return {f: int(getattr(i, f)) for f, _ in TrnPercolatorInfo._fields_ if f != "pad"}
+
+    def percolate(self, docs: Sequence[np.ndarray]) -> "PercolationResult":
+        """every registered query each document matches: docs are uint32 token arrays (EMPTY_TERM: a token outside the vocabulary)"""
+        offs = np.zeros(len(docs) + 1, np.uint64)
+        offs[1:] = np.cumsum([len(d) for d in docs])
+        tok = _u32(np.concatenate([np.asarray(d, np.uint32) for d in docs]) if len(docs) else [])
+        r = TrnPercolation()
+        self._ck(self._L.trn_percolate(self._h, _ptr(offs), _ptr(tok) if len(tok) else None, len(docs), C.byref(r)))
+        return PercolationResult(r)
+
     def close(self):
         if getattr(self, "_h", None):
             self._L.trn_destroy(self._h)
@@ -748,6 +769,75 @@ class GpuIndexSource:
             self.close()
         except Exception:
             pass
+
+
+class PercolationResult:
+    """Percolator.percolate: per document the ascending ids of the registered queries it matches, the (document, query) pairs evaluated,
+    the documents of the long launch and of the bitmap output, and the device times of both passes and the host time of the call"""
+
+    def __init__(self, r: TrnPercolation):
+        n, tot = int(r.ndocs), int(r.total)
+        self.offsets = np.ctypeslib.as_array(r.offsets, shape=(n + 1,)).copy() if r.offsets else np.zeros(1, np.uint64)
+        self.queries = np.ctypeslib.as_array(r.queries, shape=(tot,)).copy() if tot else np.zeros(0, np.uint32)
+        self.ndocs, self.total, self.candidates = n, tot, int(r.candidates)
+        self.long_docs, self.dense_docs = int(r.long_docs), int(r.dense_docs)
+        self.count_ms, self.write_ms, self.total_ms = float(r.count_ms), float(r.write_ms), float(r.total_ms)
+
+    def document(self, d: int) -> np.ndarray:
+        return self.queries[int(self.offsets[d]): int(self.offsets[d + 1])]
+
+    def __len__(self):
+        return self.ndocs
+
+
+class Percolator:
+    """== Trinity's percolator_query::match (percolator.h) for a whole registered query set at once: which stored queries each incoming
+    document matches.  queries: trn_qnode trees (parse_query); nterms: the size of the vocabulary their term ids index; term_cost: optional
+    per-term cost (e.g. document frequency) that picks each query's anchors; source: a GpuIndexSource whose context to share (its index and
+    exec_batch stay as they are), else a context of its own on `device`."""
+
+    def __init__(self, queries: Sequence[np.ndarray], device: int = 0, nterms: int = 0, term_cost=None, source: Optional["GpuIndexSource"] = None):
+        self.source = source if source is not None else GpuIndexSource(device)
+        self._info = self.source.percolator_register(queries, nterms, term_cost)
+        self._last = None
+
+    def percolate(self, docs: Sequence[np.ndarray]) -> PercolationResult:
+        self._last = self.source.percolate(docs)
+        return self._last
+
+    def percolate_tokens(self, token_lists: Sequence[Sequence[str]], tdict: "TermDictionary") -> PercolationResult:
+        """percolate() with the tokens named: each resolved through the dictionary (an unknown name becomes EMPTY_TERM)"""
+        return self.percolate([np.array([tdict.term_id(t) for t in toks], np.uint32) for toks in token_lists])
+
+    def info(self) -> dict:
+        return dict(self._info)
+
+    def last_timings(self) -> dict:
+        """device times (ms) of the count and write passes of the last percolate() call and its host time"""
+        r = self._last
+        return {} if r is None else {"count_ms": r.count_ms, "write_ms": r.write_ms, "total_ms": r.total_ms}
+
+
+def debug_percolator_plan(queries: Sequence[np.ndarray], nterms: int, term_cost=None):
+    """the registration planner (csrc/percplan.h) on the host: per query (status, cover) with status 0 anchored, 1 unanchored, 2 cannot match
+    and the anchor cover as ascending term ids"""
+    arr, keep = _pack_queries(queries)
+    cost = None if term_cost is None else _u32(term_cost)
+    nq = len(queries)
+    status, off = np.zeros(max(nq, 1), np.uint8), np.zeros(nq + 1, np.uint32)
+    n = C.c_uint64()
+    err = C.create_string_buffer(512)
+    cap = 1 << 12
+    while True:
+        terms = np.zeros(cap, np.uint32)
+        rc = lib().trn_debug_percolator_plan(C.cast(arr, C.c_void_p), nq, nterms, _ptr(cost) if cost is not None else None, _ptr(status), _ptr(off),
+                                             _ptr(terms), cap, C.byref(n), err, 512)
+        if rc == -6 and n.value > cap:
+            cap = int(n.value)
+            continue
+        if rc != 0:
+            raise TrinityError(f"rc={rc}: {err.value.decode()}")
+        return [(int(status[q]), [int(t) for t in terms[int(off[q]): int(off[q + 1])]]) for q in range(nq)]
 
 
 def directory_probe(codec: int, index: np.ndarray, term: tuple):

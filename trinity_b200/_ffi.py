@@ -23,6 +23,7 @@ EXPORTS = [
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_encode_lucene", "trn_debug_chunk_plan",
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
+    "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -71,6 +72,17 @@ class TrnIntersections(C.Structure):
     _fields_ = [("n", C.c_uint32), ("total", C.c_uint64), ("offsets", C.POINTER(C.c_uint64)), ("masks", C.POINTER(C.c_uint64)),
                 ("counts", C.POINTER(C.c_uint32)), ("postings", C.c_uint64), ("distinct", C.c_uint64), ("masks_ms", C.c_float),
                 ("plan_ms", C.c_float), ("count_ms", C.c_float), ("total_ms", C.c_float)]
+
+
+class TrnPercolatorInfo(C.Structure):
+    _fields_ = [("nqueries", C.c_uint32), ("unanchored", C.c_uint32), ("never", C.c_uint32), ("pad", C.c_uint32), ("anchor_entries", C.c_uint64),
+                ("device_bytes", C.c_uint64)]
+
+
+class TrnPercolation(C.Structure):
+    _fields_ = [("ndocs", C.c_uint32), ("long_docs", C.c_uint32), ("dense_docs", C.c_uint32), ("pad", C.c_uint32), ("total", C.c_uint64),
+                ("offsets", C.POINTER(C.c_uint64)), ("queries", C.POINTER(C.c_uint32)), ("candidates", C.c_uint64), ("count_ms", C.c_float),
+                ("write_ms", C.c_float), ("total_ms", C.c_float)]
 
 
 CONSIDER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
@@ -171,5 +183,8 @@ def lib() -> C.CDLL:
     sig("trn_debug_dense_terms", i32, i32, vp, u64, vp, u32, vp, P(u32), P(u64), C.c_char_p, C.c_size_t)
     sig("trn_intersect", i32, vp, vp, u32, P(TrnIntersections))
     sig("trn_debug_intersect_plan", i32, vp, vp, u32, u32, vp, vp, vp, vp, u64, P(u32), P(u64), vp, P(u32), C.c_char_p, C.c_size_t)
+    sig("trn_percolator_register", i32, vp, vp, u32, u32, vp, P(TrnPercolatorInfo))
+    sig("trn_percolate", i32, vp, vp, vp, u32, P(TrnPercolation))
+    sig("trn_debug_percolator_plan", i32, vp, u32, u32, vp, vp, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     _lib = L
     return L

@@ -323,4 +323,60 @@ struct IsectParams {
         uint32_t *                counts;      // per final antichain entry of every request
 };
 
+// ---- percolator (trn_percolator_register / trn_percolate; percplan.h, percolate.cuh)
+static constexpr uint32_t kPercMaxDocLen  = 16383; // tokens of a document: positions 1 .. 16383, below Limits::MaxPosition
+static constexpr uint32_t kPercShortLen   = 512;   // documents up to this many tokens run in the short launch (small shared tables, many CTAs per SM)
+static constexpr uint32_t kPercMaxHash    = 16384; // slots of a document's distinct-term table (a power of two >= 2 x its length, at most this)
+static constexpr uint32_t kPercSortCap    = 4096;  // a document with at most this many matches sorts its ids in shared memory; more: a bitmap
+static constexpr uint32_t kPercStack      = 64;    // evaluation stack of a query program: one bit per pending operand, in one 64-bit register
+// slots of the distinct-term table of a document of L tokens (at least one more than its distinct terms)
+__host__ __device__ inline uint32_t perc_hash_slots(uint32_t L) {
+        uint32_t H = 32;
+        while (H < 2u * L && H < kPercMaxHash)
+                H <<= 1;
+        return H;
+}
+enum : uint8_t { PERC_TERM, PERC_PHRASE, PERC_CONST, PERC_AND, PERC_OR, PERC_NOT, PERC_OPT, PERC_SOME };
+// one post-order operation of a query program.  TERM: the term is on the document.  PHRASE: the n terms phrase_terms[term .. + n) stand at
+// consecutive positions; arg = the index of its cheapest term (the one whose positions are tried).  CONST: the value `term`.  AND / OR /
+// NOT (the first operand and none of the others) / OPT (the first operand) / SOME (at least arg >= 1 operands): of the n topmost values.
+struct PercOp {
+        uint8_t  op, n;
+        uint16_t arg;
+        uint32_t term;
+};
+struct PercQuery {
+        uint32_t op_begin, nops;       // its program: ops[op_begin .. + nops)
+        uint32_t cover_begin, ncover;  // its anchor cover, ascending term id: covers[cover_begin .. + ncover)
+};
+struct PercEntry {
+        uint32_t query, ordinal; // an anchored query and the index of this anchor in its sorted cover
+};
+struct PercParams {
+        // the registry
+        const PercQuery *queries;
+        const PercOp *   ops;
+        const uint32_t * phrase_terms;
+        const uint32_t * covers;
+        const uint32_t * csr_off; // per term + 1: its anchored queries are csr[csr_off[t] .. csr_off[t + 1])
+        const PercEntry *csr;
+        const uint32_t * unanchored; // queries every document evaluates
+        uint32_t         nunanchored, nterms;
+        // the documents of this launch: docs[0 .. ndocs), document d = tokens[doc_off[d] .. doc_off[d + 1])
+        const unsigned long long *doc_off;
+        const uint32_t *          tokens;
+        const uint32_t *          docs;
+        uint32_t                  ndocs, max_len; // max_len: the longest document of the launch (shared token array)
+        uint32_t                  max_hash;       // slots of the launch's shared distinct-term table
+        // count pass
+        uint32_t *          counts;     // per document: its matches
+        unsigned long long *candidates; // (document, query) pairs evaluated
+        // write pass
+        const unsigned long long *out_off;    // per document + 1: its ids go to out[out_off[d] ..)
+        uint32_t *                out;
+        uint32_t *                bitmaps;    // documents with more than kPercSortCap matches: one zeroed bitmap of bitmap_words words each
+        const uint32_t *          dense_slot; // ... the index of a document's bitmap
+        uint32_t                  bitmap_words;
+};
+
 } // namespace trn

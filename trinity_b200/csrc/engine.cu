@@ -9,6 +9,7 @@
 #include "hitcursor.h"
 #include "chunkplan.h"
 #include "isectplan.h"
+#include "percplan.h"
 #include "kernels.h"
 #include "planner.h"
 #include <algorithm>
@@ -173,6 +174,26 @@ struct trn_ctx {
                 }
         } it;
         uint32_t isect_max_masks{kIsectMaxMasks}; // TRN_ISECT_MAX_MASKS: distinct masks a request may have (lowers the limit only)
+        // percolator (trn_percolator_register / trn_percolate): the registry, the batch scratch, the pinned result
+        struct PercBufs {
+                bool                have{false};
+                uint32_t            nq{0}, nterms{0}, nunanchored{0};
+                trn_percolator_info info{};
+                DevBuf d_queries, d_ops, d_pterms, d_covers, d_csr_off, d_csr, d_unanch; // the registry
+                DevBuf d_doc_off, d_tokens, d_docs, d_counts, d_small, d_part, d_out_off, d_out, d_bitmaps, d_dense_slot;
+                PinBuf h_offsets, h_ids;
+                cudaEvent_t ev[4]{nullptr, nullptr, nullptr, nullptr};
+                void release() {
+                        for (DevBuf *b : {&d_queries, &d_ops, &d_pterms, &d_covers, &d_csr_off, &d_csr, &d_unanch, &d_doc_off, &d_tokens, &d_docs, &d_counts, &d_small, &d_part,
+                                          &d_out_off, &d_out, &d_bitmaps, &d_dense_slot})
+                                b->release();
+                        for (PinBuf *b : {&h_offsets, &h_ids})
+                                b->release();
+                        for (cudaEvent_t e : ev)
+                                if (e)
+                                        cudaEventDestroy(e);
+                }
+        } pq;
 };
 
 #define CK(call)                                                                                                                                               \
@@ -292,6 +313,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         }
         c->mt.release();
         c->it.release();
+        c->pq.release();
         if (c->copy_stream)
                 cudaStreamDestroy(c->copy_stream);
         delete c;
@@ -2158,5 +2180,220 @@ extern "C" int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *f
         std::copy(pl.snap_mask.begin(), pl.snap_mask.end(), snap_mask);
         std::copy(pl.snap_slot.begin(), pl.snap_slot.end(), snap_slot);
         std::copy(pl.final_mask.begin(), pl.final_mask.end(), final_mask);
+        return TRN_OK;
+}
+
+// =================================================================================================== percolator
+// Registration plans on the host (percplan.h) and uploads the registry; trn_percolate runs the count pass, scans the counts, sizes the
+// result once from them and runs the write pass (percolate.cuh; DESIGN.md §4).  Two host synchronisations: the offsets after the scan, the
+// result.
+extern "C" int trn_percolator_register(trn_ctx *c, const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, trn_percolator_info *out) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (nq && !queries)
+                return fail(c, TRN_ERR_ARG, "trn_percolator_register: bad arguments");
+        CK(cudaSetDevice(c->device));
+        PercPlan    P;
+        std::string err;
+        if (const int rc = perc_plan(queries, nq, nterms, term_cost, P, err))
+                return fail(c, rc, "trn_percolator_register: " + err);
+        auto &B = c->pq;
+        B.have  = false;
+        uint64_t bytes{0};
+        auto     upload = [&](DevBuf &b, const void *src, size_t n) -> cudaError_t {
+                bytes += n;
+                if (const cudaError_t e = b.ensure(std::max<size_t>(16, n)); e != cudaSuccess)
+                        return e;
+                return n ? cudaMemcpyAsync(b.p, src, n, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
+        };
+        CK(upload(B.d_queries, P.queries.data(), P.queries.size() * sizeof(PercQuery)));
+        CK(upload(B.d_ops, P.ops.data(), P.ops.size() * sizeof(PercOp)));
+        CK(upload(B.d_pterms, P.phrase_terms.data(), P.phrase_terms.size() * 4));
+        CK(upload(B.d_covers, P.covers.data(), P.covers.size() * 4));
+        CK(upload(B.d_csr_off, P.csr_off.data(), P.csr_off.size() * 4));
+        CK(upload(B.d_csr, P.csr.data(), P.csr.size() * sizeof(PercEntry)));
+        CK(upload(B.d_unanch, P.unanchored.data(), P.unanchored.size() * 4));
+        CK(cudaStreamSynchronize(c->stream));
+        B.nq          = nq;
+        B.nterms      = nterms;
+        B.nunanchored = uint32_t(P.unanchored.size());
+        B.info        = trn_percolator_info{nq, B.nunanchored, P.never, 0, P.csr.size(), bytes};
+        B.have        = true;
+        if (out)
+                *out = B.info;
+        return TRN_OK;
+}
+
+extern "C" int trn_percolate(trn_ctx *c, const uint64_t *doc_offsets, const uint32_t *tokens, uint32_t ndocs, trn_percolation *out) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (!out || (ndocs && !doc_offsets))
+                return fail(c, TRN_ERR_ARG, "trn_percolate: bad arguments");
+        auto &B = c->pq;
+        if (!B.have)
+                return fail(c, TRN_ERR_STATE, "trn_percolate: no query set registered (trn_percolator_register)");
+        CK(cudaSetDevice(c->device));
+        std::memset(out, 0, sizeof(*out));
+        const double t0 = now_ms();
+        if (!B.ev[0])
+                for (cudaEvent_t &e : B.ev)
+                        CK(cudaEventCreate(&e));
+
+        // ---- the documents: lengths, tokens, the short and the long launch
+        const uint64_t base = ndocs ? doc_offsets[0] : 0, ntok = ndocs ? doc_offsets[ndocs] - base : 0;
+        if (ntok && !tokens)
+                return fail(c, TRN_ERR_ARG, "trn_percolate: bad arguments");
+        std::vector<uint32_t> docs[2];
+        uint32_t              max_len[2]{0, 0};
+        std::vector<uint64_t> off(size_t(ndocs) + 1, 0);
+        for (uint32_t d = 0; d < ndocs; ++d) {
+                const std::string who = "trn_percolate: document " + std::to_string(d) + ": ";
+                if (doc_offsets[d + 1] < doc_offsets[d] || doc_offsets[d + 1] - base > ntok)
+                        return fail(c, TRN_ERR_ARG, who + "doc_offsets must not decrease");
+                const uint64_t L = doc_offsets[d + 1] - doc_offsets[d];
+                if (L > kPercMaxDocLen)
+                        return fail(c, TRN_ERR_ARG, who + std::to_string(L) + " tokens (at most 16383: positions below Limits::MaxPosition)");
+                for (uint64_t i = doc_offsets[d]; i < doc_offsets[d + 1]; ++i)
+                        if (tokens[i] != kEmptyTerm && tokens[i] >= B.nterms)
+                                return fail(c, TRN_ERR_ARG, who + "token id " + std::to_string(tokens[i]) + " outside the vocabulary (use TRN_EMPTY_TERM)");
+                const int lg = L > kPercShortLen;
+                docs[lg].push_back(d);
+                max_len[lg] = std::max(max_len[lg], uint32_t(L));
+                off[d + 1]  = doc_offsets[d + 1] - base;
+        }
+        auto upload = [&](DevBuf &b, const void *src, size_t n) -> cudaError_t {
+                if (const cudaError_t e = b.ensure(std::max<size_t>(16, n)); e != cudaSuccess)
+                        return e;
+                return n ? cudaMemcpyAsync(b.p, src, n, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
+        };
+        CK(upload(B.d_doc_off, off.data(), off.size() * 8));
+        CK(upload(B.d_tokens, tokens + base, ntok * 4));
+        CK(B.d_docs.ensure(std::max<size_t>(16, size_t(ndocs) * 4)));
+        CK(cudaMemcpyAsync(B.d_docs.p, docs[0].data(), docs[0].size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(B.d_docs.as<uint32_t>() + docs[0].size(), docs[1].data(), docs[1].size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(B.d_counts.ensure(std::max<size_t>(16, size_t(ndocs) * 4)));
+        CK(B.d_small.ensure(16));
+        CK(cudaMemsetAsync(B.d_small.p, 0, 8, c->stream));
+        CK(B.d_part.ensure((size_t(ndocs) / 4096 + 2) * 8));
+        CK(B.d_out_off.ensure((size_t(ndocs) + 1) * 8));
+
+        PercParams P;
+        std::memset(&P, 0, sizeof(P));
+        P.queries      = B.d_queries.as<PercQuery>();
+        P.ops          = B.d_ops.as<PercOp>();
+        P.phrase_terms = B.d_pterms.as<uint32_t>();
+        P.covers       = B.d_covers.as<uint32_t>();
+        P.csr_off      = B.d_csr_off.as<uint32_t>();
+        P.csr          = B.d_csr.as<PercEntry>();
+        P.unanchored   = B.d_unanch.as<uint32_t>();
+        P.nunanchored  = B.nunanchored;
+        P.nterms       = B.nterms;
+        P.doc_off      = B.d_doc_off.as<unsigned long long>();
+        P.tokens       = B.d_tokens.as<uint32_t>();
+        P.counts       = B.d_counts.as<uint32_t>();
+        P.candidates   = B.d_small.as<unsigned long long>();
+        auto launches  = [&](bool write) -> cudaError_t {
+                for (int lg = 0; lg < 2; ++lg) {
+                        PercParams L = P;
+                        L.docs       = B.d_docs.as<uint32_t>() + (lg ? docs[0].size() : 0);
+                        L.ndocs      = uint32_t(docs[lg].size());
+                        L.max_len    = max_len[lg];
+                        L.max_hash   = perc_hash_slots(max_len[lg]);
+                        if (const cudaError_t e = launch_perc(L, write, c->num_sms, c->stream); e != cudaSuccess)
+                                return e;
+                }
+                return cudaSuccess;
+        };
+
+        // ---- count pass and the scan of the counts
+        CK(cudaEventRecord(B.ev[0], c->stream));
+        CK(launches(false));
+        CK(launch_enc_scan(P.counts, ndocs, B.d_part.as<unsigned long long>(), B.d_out_off.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(B.ev[1], c->stream));
+        CK(B.h_offsets.ensure((size_t(ndocs) + 1) * 8));
+        uint64_t cand{0};
+        CK(cudaMemcpyAsync(B.h_offsets.p, B.d_out_off.p, (size_t(ndocs) + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(&cand, B.d_small.p, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        const uint64_t *hoff  = B.h_offsets.as<uint64_t>();
+        const uint64_t  total = hoff[ndocs];
+
+        // ---- the result, sized once; a bitmap per document with more matches than shared memory sorts
+        std::vector<uint32_t> slot(ndocs, 0);
+        uint32_t              ndense{0};
+        for (uint32_t d = 0; d < ndocs; ++d)
+                if (hoff[d + 1] - hoff[d] > kPercSortCap)
+                        slot[d] = ndense++;
+        const uint32_t words = (B.nq + 31u) / 32u;
+        auto capacity = [&](cudaError_t e, const char *what) {
+                (void)cudaGetLastError();
+                return fail(c, e == cudaErrorMemoryAllocation ? TRN_ERR_CAPACITY : TRN_ERR_CUDA,
+                            std::string("trn_percolate: ") + what + " (" + std::to_string(total) + " matches): " + cudaGetErrorString(e) + "; split the batch");
+        };
+        if (const cudaError_t e = B.d_out.ensure(std::max<size_t>(16, total * 4)); e != cudaSuccess)
+                return capacity(e, "the matches cannot be staged on the device");
+        if (const cudaError_t e = B.h_ids.ensure(std::max<size_t>(16, total * 4)); e != cudaSuccess)
+                return capacity(e, "the pinned result cannot be allocated");
+        if (ndense) {
+                if (const cudaError_t e = B.d_bitmaps.ensure(size_t(ndense) * words * 4); e != cudaSuccess)
+                        return capacity(e, "the bitmaps of the documents with many matches cannot be allocated");
+                CK(cudaMemsetAsync(B.d_bitmaps.p, 0, size_t(ndense) * words * 4, c->stream));
+        }
+        CK(upload(B.d_dense_slot, slot.data(), slot.size() * 4));
+        P.out_off      = B.d_out_off.as<unsigned long long>();
+        P.out          = B.d_out.as<uint32_t>();
+        P.bitmaps      = B.d_bitmaps.as<uint32_t>();
+        P.dense_slot   = B.d_dense_slot.as<uint32_t>();
+        P.bitmap_words = words;
+
+        // ---- write pass
+        CK(cudaEventRecord(B.ev[2], c->stream));
+        CK(launches(true));
+        CK(cudaEventRecord(B.ev[3], c->stream));
+        CK(cudaMemcpyAsync(B.h_ids.p, B.d_out.p, total * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        float countMs{0}, writeMs{0};
+        (void)cudaEventElapsedTime(&countMs, B.ev[0], B.ev[1]);
+        (void)cudaEventElapsedTime(&writeMs, B.ev[2], B.ev[3]);
+        out->ndocs      = ndocs;
+        out->long_docs  = uint32_t(docs[1].size());
+        out->dense_docs = ndense;
+        out->total      = total;
+        out->offsets    = hoff;
+        out->queries    = B.h_ids.as<uint32_t>();
+        out->candidates = cand;
+        out->count_ms   = countMs;
+        out->write_ms   = writeMs;
+        out->total_ms   = float(now_ms() - t0);
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, uint8_t *status, uint32_t *cover_off,
+                                         uint32_t *cover_terms, uint64_t cap, uint64_t *ncover, char *err, size_t errcap) {
+        auto say = [&](const std::string &m) {
+                if (err && errcap)
+                        snprintf(err, errcap, "%s", m.c_str());
+        };
+        if ((nq && (!queries || !status)) || !cover_off || !ncover || (cap && !cover_terms)) {
+                say("trn_debug_percolator_plan: bad arguments");
+                return TRN_ERR_ARG;
+        }
+        PercPlan    P;
+        std::string e;
+        if (const int rc = perc_plan(queries, nq, nterms, term_cost, P, e)) {
+                say(e);
+                return rc;
+        }
+        *ncover = P.covers.size();
+        if (P.covers.size() > cap) {
+                say("trn_debug_percolator_plan: " + std::to_string(P.covers.size()) + " cover terms do not fit");
+                return TRN_ERR_CAPACITY;
+        }
+        for (uint32_t q = 0; q < nq; ++q) {
+                status[q]    = P.status[q];
+                cover_off[q] = P.queries[q].cover_begin;
+        }
+        cover_off[nq] = uint32_t(P.covers.size());
+        std::copy(P.covers.begin(), P.covers.end(), cover_terms);
         return TRN_OK;
 }

@@ -1074,6 +1074,7 @@ __global__ void __launch_bounds__(kThreads) k_decode_terms(DevIndex ix, const ui
 #include "encode_lucene.cuh"
 #include "collect.cuh"
 #include "intersect.cuh"
+#include "percolate.cuh"
 
 // ------------------------------------------------------------------------------------------------ launch wrappers
 uint32_t exec_stage_bytes(int codec) {

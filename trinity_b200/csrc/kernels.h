@@ -50,6 +50,9 @@ cudaError_t launch_isect(const IsectParams &P, bool lucene, bool passb, int num_
 cudaError_t launch_isect_compact(const IsectParams &P, uint64_t total_slots, const uint64_t *base, uint32_t *cursor, unsigned long long *out_mask, uint32_t *out_first,
                                  int num_sms, cudaStream_t stream);
 cudaError_t launch_isect_carry(const IsectParams &P, unsigned long long *carry, cudaStream_t stream);
+// percolator (percolate.cuh): the count (write false) and write passes of trn_percolate over one launch's documents
+size_t      perc_smem_bytes(uint32_t max_len, uint32_t max_hash, bool write);
+cudaError_t launch_perc(const PercParams &P, bool write, int num_sms, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
 } // namespace trn

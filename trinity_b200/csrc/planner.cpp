@@ -57,7 +57,58 @@ static bool plan_depth_ok(const trn_qnode *n, uint32_t nn) {
         }
         return true;
 }
+} // namespace
 
+bool trn::validate_plan(const trn_qnode *n, uint32_t nn, uint32_t root, uint32_t nterms, bool allow_phrase, std::string &err, bool &unsupported, bool &has_phrase) {
+        if (root >= nn) {
+                err = "root out of range";
+                return false;
+        }
+        if (!plan_depth_ok(n, nn)) {
+                err = "query tree deeper than 64 levels";
+                return false;
+        }
+        for (uint32_t i = 0; i < nn; ++i) {
+                if (n[i].kind == TRN_NODE_TERM) {
+                        if (n[i].term != kEmptyTerm && n[i].term >= nterms) {
+                                err = "term id out of range";
+                                return false;
+                        }
+                } else if (n[i].kind == TRN_NODE_PHRASE) {
+                        if (!allow_phrase) {
+                                err         = "phrase nodes need the positions (materialize_hits): a LUCENE source executes them once its hits.data has been uploaded (trn_upload_hits)";
+                                unsupported = true;
+                                return false;
+                        }
+                        if (n[i].nchildren < 2 || n[i].nchildren > 16 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
+                                err = "a phrase holds 2..16 terms behind it in the node array";
+                                return false;
+                        }
+                        for (uint32_t k = 0; k < n[i].nchildren; ++k)
+                                if (n[n[i].first_child + k].kind != TRN_NODE_TERM) {
+                                        err = "the children of a phrase are terms";
+                                        return false;
+                                }
+                        has_phrase = true;
+                } else if (n[i].kind > TRN_NODE_PHRASE) {
+                        err = "unknown node kind";
+                        return false;
+                } else {
+                        // children must come after their parent (guarantees an acyclic tree)
+                        if (n[i].nchildren == 0 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
+                                err = "children must follow their parent in the node array";
+                                return false;
+                        }
+                }
+        }
+        if (!plan_is_tree(n, nn, root)) {
+                err = "a node is referenced by more than one parent (a plan is a tree)";
+                return false;
+        }
+        return true;
+}
+
+namespace {
 struct Compiler {
         const trn_qnode *           n;
         uint32_t                    nn;
@@ -441,52 +492,7 @@ struct Compiler {
         }
 
         bool validate() {
-                if (root >= nn) {
-                        err = "root out of range";
-                        return false;
-                }
-                if (!plan_depth_ok(n, nn)) {
-                        err = "query tree deeper than 64 levels";
-                        return false;
-                }
-                for (uint32_t i = 0; i < nn; ++i) {
-                        if (n[i].kind == TRN_NODE_TERM) {
-                                if (n[i].term != kEmptyTerm && n[i].term >= terms.size()) {
-                                        err = "term id out of range";
-                                        return false;
-                                }
-                        } else if (n[i].kind == TRN_NODE_PHRASE) {
-                                if (!allow_phrase) {
-                                        err         = "phrase nodes need the positions (materialize_hits): a LUCENE source executes them once its hits.data has been uploaded (trn_upload_hits)";
-                                        unsupported = true;
-                                        return false;
-                                }
-                                if (n[i].nchildren < 2 || n[i].nchildren > 16 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
-                                        err = "a phrase holds 2..16 terms behind it in the node array";
-                                        return false;
-                                }
-                                for (uint32_t k = 0; k < n[i].nchildren; ++k)
-                                        if (n[n[i].first_child + k].kind != TRN_NODE_TERM) {
-                                                err = "the children of a phrase are terms";
-                                                return false;
-                                        }
-                                has_phrase = true;
-                        } else if (n[i].kind > TRN_NODE_PHRASE) {
-                                err = "unknown node kind";
-                                return false;
-                        } else {
-                                // children must come after their parent (guarantees an acyclic tree)
-                                if (n[i].nchildren == 0 || n[i].first_child <= i || uint32_t(n[i].first_child) + n[i].nchildren > nn) {
-                                        err = "children must follow their parent in the node array";
-                                        return false;
-                                }
-                        }
-                }
-                if (!plan_is_tree(n, nn, root)) {
-                        err = "a node is referenced by more than one parent (a plan is a tree)";
-                        return false;
-                }
-                return true;
+                return validate_plan(n, nn, root, uint32_t(terms.size()), allow_phrase, err, unsupported, has_phrase);
         }
 
         // == DocsSetIterators::cost() (docset_iterators.cpp:10-64); a conjunction's cost is its lead's, which the reference's

@@ -71,6 +71,10 @@ struct BatchPlan {
 };
 using CollectPlan = BatchPlan::CollectPlan;
 
+// The structural checks every plan passes before it is compiled: root in range, depth <= 64, children behind their parent, a tree, term
+// ids below nterms (or kEmptyTerm), phrases of 2..16 terms.  A phrase when !allow_phrase sets `unsupported`; has_phrase reports one.
+bool validate_plan(const trn_qnode *nodes, uint32_t nn, uint32_t root, uint32_t nterms, bool allow_phrase, std::string &err, bool &unsupported, bool &has_phrase);
+
 // The collect programs of a batch in the default exec mode (TRN_MODE_MATCHED_TERMS): per query its distinct terms (at most 32, ascending
 // term index), its phrase nodes (at most 32) and its nodes in post order.  TRN_ERR_UNSUPPORTED beyond those limits.
 int plan_collect(const std::vector<DevTerm> &terms, const trn_query *queries, uint32_t nq, CollectPlan &out, std::string &err);
