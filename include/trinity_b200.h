@@ -533,6 +533,50 @@ int trn_percolate(trn_ctx *, const uint64_t *doc_offsets, const uint32_t *tokens
 int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, uint8_t *status, uint32_t *cover_off,
                               uint32_t *cover_terms, uint64_t cap, uint64_t *ncover, char *err, size_t errcap);
 
+/* ------------------------------------------------------------------------------------------------ indexer
+ * == SegmentIndexSession begin / insert / commit (indexer.h, indexer.cpp:14-153, 311-564) for one batch of tokenised documents: the
+ * documents are inverted on the device (a keys-only radix sort), encoded by the device encoders and come back as the `index` (and LUCENE
+ * `hits.data`) bytes the reference's commit() would have written for the same documents; trn_segment_write makes a segment directory of them.
+ *   docids[ndocs]            the documents' ids, in any order, > 0, no id twice
+ *   doc_offsets[ndocs + 1]   document d is tokens[doc_offsets[d] .. doc_offsets[d + 1]); doc_offsets[0] = 0; an empty document is legal and
+ *                            is not counted in docs_cnt (indexer.cpp:361-364)
+ *   tokens[]                 term ids below nterms; term t stands for the reference's transient term id t + 1, which fixes the order of the
+ *                            chunks in the index: by (t + 1) & 31, then by t (indexer.cpp:388, 402-410, 423)
+ *   positions[]              the position of every token, in any order inside a document, equal positions allowed; NULL: token i of a
+ *                            document sits at position i + 1 (trn_percolate's convention)
+ * All pointers are HOST pointers.  The GOOGLE geometry is the reference's (32 / 8, a fresh countdown).  The hits carry no payloads.
+ * Refusals, never a wrong answer, each naming the document or term.  TRN_ERR_ARG: docID 0, a docID twice, a token >= nterms, doc_offsets
+ * not ascending, a position >= 16384 (Limits::MaxPosition), more than 65535 hits of one term in one document or more than 65535 distinct
+ * terms in one document (uint16_t counts of the reference), nterms > 2^24, ndocs > 2^26.  TRN_ERR_UNSUPPORTED: a position 0 (a hit without
+ * a position).  TRN_ERR_CAPACITY: an index or hits.data of 4 GiB or more, or working memory that cannot be allocated (split the batch).
+ * A refused call leaves the context's uploaded index, percolator registry and earlier results as they were. */
+typedef struct trn_indexed { /* owned by the ctx, valid until the next trn_index_documents */
+        const uint8_t * index;
+        uint64_t        index_bytes;
+        const uint8_t * hits; /* LUCENE hits.data; 0 bytes for GOOGLE */
+        uint64_t        hits_bytes;
+        const trn_term *terms; /* by term id; documents == 0: the term has no posting and is not in the segment */
+        uint32_t        nterms;
+        uint32_t        docs_cnt, total_terms; /* IndexSource::field_statistics (indexer.cpp:366, 446, 465, 473) */
+        uint64_t        sum_terms_docs, sum_term_hits;
+        uint32_t        max_docid;
+        uint32_t        sort_passes; /* radix passes run (documents + tokens): one per group of up to 8 key bits that can be non-zero */
+        float           sort_ms, postings_ms, encode_ms; /* CUDA events of the kernels alone: ranks + keys + sort, the postings pass, the encoder */
+        float           total_ms;                        /* host time of the whole call, copies included */
+} trn_indexed;
+int trn_index_documents(trn_ctx *, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
+                        uint32_t ndocs, uint32_t nterms, trn_indexed *out);
+/* Host code, no device: writes the segment directory `dir` as persist_segment / persist_terms do (indexer.cpp:241-300, codecs.cpp:17-27,
+ * terms.cpp:126-172 pack_terms, docidupdates.cpp:8-73 pack_updates): `index`, `hits.data` (LUCENE), `terms.data`, `terms.idx`, `id`, and
+ * `updated_documents.ids` when nupdated > 0.  terms[i] <-> names[i]; terms with documents == 0 are left out.  updated_docids = the ids of
+ * the documents this segment replaces in older segments plus the erased ids.  The last component of `dir` must be a number, the segment's
+ * generation (segment_index_source.cpp:18-21); the directory is created when missing.  TRN_ERR_ARG: such a name, an empty name or one
+ * longer than 64 bytes (Limits::MaxTermLength), two equal names, an id twice in updated_docids (the reference's "Already committed
+ * document").  TRN_ERR_STATE: a file cannot be written. */
+int trn_segment_write(const char *dir, int codec, const uint8_t *index, uint64_t index_bytes, const uint8_t *hits, uint64_t hits_bytes, const trn_term *terms,
+                      const char *const *names, uint32_t nterms, uint64_t sum_term_hits, uint32_t total_terms, uint64_t sum_terms_docs, uint32_t docs_cnt,
+                      const uint32_t *updated_docids, uint64_t nupdated, char *err, size_t errcap);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,13 +7,14 @@ all decode / docset / scoring work happens in the sm_90a kernels of libtrinity_b
 from __future__ import annotations
 
 import ctypes as C
+import os
 from dataclasses import dataclass
 from typing import Iterable, List, Optional, Sequence
 
 import numpy as np
 
 from ._ffi import (HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnIntersections, TrnIsectReq, TrnMatches, TrnPercolation, TrnPercolatorInfo, TrnQuery,
-                   TrnResult, TrnTerm, TrnTimings, lib)
+                   TrnIndexed, TrnResult, TrnTerm, TrnTimings, lib)
 
 CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
@@ -759,6 +760,38 @@ class GpuIndexSource:
         self._ck(self._L.trn_percolate(self._h, _ptr(offs), _ptr(tok) if len(tok) else None, len(docs), C.byref(r)))
         return PercolationResult(r)
 
+    def index_documents(self, codec: int, docids, docs: Sequence[np.ndarray], nterms: int, positions: Optional[Sequence[np.ndarray]] = None) -> "IndexedSegment":
+        """== SegmentIndexSession begin / insert / commit for a batch: docs are uint32 term-id arrays (every id below nterms), docids their
+        ids (any order, > 0, none twice); positions: per document the position of every token, None = token i at i + 1.  The inversion
+        and the encode run on the device; the result holds the bytes commit() would have written."""
+        d = _u32(docids)
+        if len(d) != len(docs) or (positions is not None and len(positions) != len(docs)):
+            raise TrinityError("index_documents: one docID (and one positions array) per document")
+        offs = np.zeros(len(docs) + 1, np.uint64)
+        offs[1:] = np.cumsum([len(x) for x in docs])
+        tok = _u32(np.concatenate([np.asarray(x, np.uint32) for x in docs]) if len(docs) else [])
+        pos = None
+        if positions is not None:
+            pos = _u32(np.concatenate([np.asarray(x, np.uint32) for x in positions]) if len(docs) else [])
+            if len(pos) != len(tok):
+                raise TrinityError("index_documents: one position per token")
+        return self.index_documents_flat(codec, d, offs, tok, nterms, pos)
+
+    def index_documents_flat(self, codec: int, docids: np.ndarray, doc_offsets: np.ndarray, tokens: np.ndarray, nterms: int,
+                             positions: Optional[np.ndarray] = None) -> "IndexedSegment":
+        """index_documents over the flat arrays of the C ABI (doc_offsets: uint64, ndocs + 1 entries)"""
+        d, tok = _u32(docids), _u32(tokens)
+        offs = np.ascontiguousarray(doc_offsets, np.uint64)
+        pos = None if positions is None else _u32(positions)
+        r = TrnIndexed()
+        self._ck(self._L.trn_index_documents(self._h, codec, _ptr(d), _ptr(offs), _ptr(tok) if len(tok) else None,
+                                             _ptr(pos) if pos is not None and len(pos) else None, len(d), nterms, C.byref(r)))
+        return IndexedSegment(codec, r, d)
+
+    def index_tokens(self, codec: int, docids, token_lists: Sequence[Sequence[str]], tdict: "TermDictionary") -> "IndexedSegment":
+        """index_documents() with the tokens named: each resolved through the dictionary, whose size is nterms (an unknown name is refused)"""
+        return self.index_documents(codec, docids, [np.array([tdict.term_id(t) for t in toks], np.uint32) for toks in token_lists], len(tdict))
+
     def close(self):
         if getattr(self, "_h", None):
             self._L.trn_destroy(self._h)
@@ -924,3 +957,61 @@ class Segment:
             self._L.trn_segment_close(self._h)
         except Exception:
             pass
+
+
+def segment_write(path: str, codec: int, index: np.ndarray, hits: Optional[np.ndarray], terms: np.ndarray, names: Sequence[str], field_statistics: dict,
+                  updated_docids=()):
+    """Writes the segment directory `path` (its last component a number, the generation) as Trinity's persist_segment / persist_terms do:
+    index, hits.data (LUCENE), terms.data, terms.idx, id, and updated_documents.ids when there are updated (replaced or erased) docIDs.
+    terms[i] <-> names[i]; terms without documents are left out.  Host code; Segment(path) and the reference's SegmentIndexSource open it."""
+    index = np.ascontiguousarray(index, np.uint8)
+    hits = np.zeros(0, np.uint8) if hits is None else np.ascontiguousarray(hits, np.uint8)
+    terms = np.ascontiguousarray(terms, TERM_DTYPE)
+    if len(names) != len(terms):
+        raise TrinityError("segment_write: one name per term")
+    enc = [n.encode("utf-8", "surrogateescape") if isinstance(n, str) else bytes(n) for n in names]
+    arr = (C.c_char_p * len(enc))(*enc)
+    upd = _u32(updated_docids)
+    fs = field_statistics
+    err = C.create_string_buffer(512)
+    os.makedirs(os.path.dirname(os.path.abspath(str(path))), exist_ok=True)  # the C call creates the generation's directory itself
+    rc = lib().trn_segment_write(str(path).encode(), codec, _ptr(index) if index.size else None, index.size, _ptr(hits) if hits.size else None, hits.size,
+                                 _ptr(terms) if len(terms) else None, C.cast(arr, C.c_void_p) if len(enc) else None, len(terms), int(fs["sumTermHits"]),
+                                 int(fs["totalTerms"]), int(fs["sumTermsDocs"]), int(fs["docsCnt"]), _ptr(upd) if len(upd) else None, len(upd), err, 512)
+    if rc != 0:
+        raise TrinityError(f"rc={rc}: {err.value.decode('utf-8', 'replace')}")
+
+
+class IndexedSegment:
+    """GpuIndexSource.index_documents: the index (and LUCENE hits.data) bytes of a batch of documents, the term_index_ctx tuple of every
+    term id (documents == 0: the term has no posting), the field statistics commit() records, and the device times of the call."""
+
+    def __init__(self, codec: int, r, docids: np.ndarray):
+        self.codec = codec
+        self.docids = docids.copy()  # of the batch, as given
+        self.index = np.ctypeslib.as_array(r.index, shape=(int(r.index_bytes),)).copy() if r.index_bytes else np.zeros(0, np.uint8)
+        self.hits = np.ctypeslib.as_array(r.hits, shape=(int(r.hits_bytes),)).copy() if r.hits_bytes else np.zeros(0, np.uint8)
+        n = int(r.nterms)
+        self.terms = np.ctypeslib.as_array(C.cast(r.terms, C.POINTER(C.c_uint8)), shape=(n * 12,)).view(TERM_DTYPE).copy()
+        self.field_statistics = {"sumTermHits": int(r.sum_term_hits), "totalTerms": int(r.total_terms), "sumTermsDocs": int(r.sum_terms_docs),
+                                 "docsCnt": int(r.docs_cnt)}
+        self.max_docid = int(r.max_docid)
+        self.sort_passes = int(r.sort_passes)
+        self.timings = {"sort_ms": float(r.sort_ms), "postings_ms": float(r.postings_ms), "encode_ms": float(r.encode_ms), "total_ms": float(r.total_ms)}
+
+    def write(self, path: str, names: Sequence[str], replaced=(), erased=()):
+        """the segment directory of this batch: names[t] = the name of term id t; replaced = docIDs of this batch that older segments also
+        hold, erased = docIDs deleted from older segments (both go to updated_documents.ids; an erased docID cannot be indexed here)"""
+        both = np.intersect1d(self.docids, _u32(list(erased)))
+        if len(both):
+            raise TrinityError(f"IndexedSegment.write: docID {int(both[0])} is both indexed and erased (Already committed document)")
+        segment_write(path, self.codec, self.index, self.hits, self.terms, names, self.field_statistics, list(replaced) + list(erased))
+
+    def upload(self, gpu: "GpuIndexSource", names: Optional[Sequence[str]] = None):
+        """uploads the index (the terms that have documents, in term-id order) and, for LUCENE, its hits; returns the term ids kept, or a
+        TermDictionary of their names when names are given"""
+        keep = np.flatnonzero(self.terms["documents"])
+        gpu.upload(self.codec, self.index, self.terms[keep], self.max_docid)
+        if self.codec == CODEC_LUCENE:
+            gpu.upload_hits(self.index, self.hits)
+        return keep if names is None else TermDictionary([names[int(t)] for t in keep])

@@ -24,6 +24,7 @@ EXPORTS = [
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
+    "trn_index_documents", "trn_segment_write",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -85,7 +86,14 @@ class TrnPercolation(C.Structure):
                 ("write_ms", C.c_float), ("total_ms", C.c_float)]
 
 
-CONSIDER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
+class TrnIndexed(C.Structure):
+    _fields_ = [("index", C.POINTER(C.c_uint8)), ("index_bytes", C.c_uint64), ("hits", C.POINTER(C.c_uint8)), ("hits_bytes", C.c_uint64),
+                ("terms", C.c_void_p), ("nterms", C.c_uint32), ("docs_cnt", C.c_uint32), ("total_terms", C.c_uint32),
+                ("sum_terms_docs", C.c_uint64), ("sum_term_hits", C.c_uint64), ("max_docid", C.c_uint32), ("sort_passes", C.c_uint32),
+                ("sort_ms", C.c_float), ("postings_ms", C.c_float), ("encode_ms", C.c_float), ("total_ms", C.c_float)]
+
+
+CONSIDER_FN =C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
 
 
 class TrnTimings(C.Structure):
@@ -186,5 +194,7 @@ def lib() -> C.CDLL:
     sig("trn_percolator_register", i32, vp, vp, u32, u32, vp, P(TrnPercolatorInfo))
     sig("trn_percolate", i32, vp, vp, vp, u32, P(TrnPercolation))
     sig("trn_debug_percolator_plan", i32, vp, u32, u32, vp, vp, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
+    sig("trn_index_documents", i32, vp, i32, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
+    sig("trn_segment_write", i32, C.c_char_p, i32, vp, u64, vp, u64, vp, vp, u32, u64, u32, u64, u32, vp, u64, C.c_char_p, C.c_size_t)
     _lib = L
     return L

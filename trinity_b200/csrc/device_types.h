@@ -379,4 +379,47 @@ struct PercParams {
         uint32_t                  bitmap_words;
 };
 
+// ---- indexer (trn_index_documents; index_docs.cuh)
+static constexpr uint32_t kIndexMaxTerms = 1u << 24; // term_order bits of a sort key
+static constexpr uint32_t kIndexMaxDocs  = 1u << 26; // doc_rank bits of a sort key
+// slots of IndexParams::errors: the lowest offending document ordinal / token / posting / document rank of every kind (~0: none)
+// terms (transient ids 1 .. nterms, term t has id t + 1) that precede bucket b of commit()'s 32 buckets (id & 31, indexer.cpp:388): the ids
+// 0 .. nterms whose residue is below b, without id 0
+__host__ __device__ inline uint32_t index_bucket_start(uint32_t b, uint32_t nterms) {
+        const uint32_t full = (nterms + 1u) >> 5, rem = (nterms + 1u) & 31u;
+        return full * b + (b < rem ? b : rem) - (b ? 1u : 0u);
+}
+// the place of term t in the encode order ((t + 1) & 31, t), and the term at a place
+__host__ __device__ inline uint32_t index_term_order(uint32_t t, uint32_t nterms) {
+        const uint32_t u = t + 1u, b = u & 31u;
+        return index_bucket_start(b, nterms) + (u >> 5) - (b ? 0u : 1u);
+}
+__host__ __device__ inline uint32_t index_term_at(uint32_t order, uint32_t nterms) {
+        uint32_t b = 0;
+        while (b < 31u && index_bucket_start(b + 1u, nterms) <= order)
+                ++b;
+        return (((order - index_bucket_start(b, nterms)) + (b ? 0u : 1u)) << 5 | b) - 1u;
+}
+enum : uint32_t { IDX_ERR_DOC0, IDX_ERR_DUP, IDX_ERR_TOKEN, IDX_ERR_POS, IDX_ERR_POS0, IDX_ERR_FREQ, IDX_ERR_DOCTERMS, IDX_ERR_KINDS };
+struct IndexParams {
+        // the batch: document d = tokens[doc_off[d] .. doc_off[d + 1]), token i at positions[i] (null: at i - doc_off[d] + 1)
+        const unsigned long long *doc_off;
+        const uint32_t *          tokens;
+        const uint32_t *          positions;
+        uint32_t                  ndocs, nterms;
+        uint64_t                  ntokens;
+        const uint32_t *          rank_of;  // per document ordinal: its rank in docID order
+        const uint32_t *          docid_of; // per rank: the docID
+        unsigned long long *      keys;     // per token: term_order << 40 | doc_rank << 14 | position
+        unsigned long long *      errors;   // IDX_ERR_KINDS slots
+        // the postings pass over the sorted keys
+        const uint32_t *          post_flag, *term_flag; // per token: opens a posting / a term
+        const unsigned long long *post_scan, *term_scan; // their exclusive scans (ntokens + 1)
+        unsigned long long *      post_begin; // per posting + 1: its first hit
+        unsigned long long *      term_begin; // per present term + 1: its first posting
+        uint32_t *                term_order; // per present term: its place in the encode order
+        uint32_t *                out_docids, *out_freqs, *out_positions;
+        uint32_t *                doc_terms;  // per rank: distinct terms (zeroed); null when nterms <= 65535 cannot exceed the limit
+};
+
 } // namespace trn

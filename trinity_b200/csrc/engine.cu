@@ -194,6 +194,17 @@ struct trn_ctx {
                                         cudaEventDestroy(e);
                 }
         } pq;
+        // indexer (trn_index_documents): the last result (its working memory lives for one call only)
+        struct IndexBufs {
+                std::vector<uint8_t>  index, hits;
+                std::vector<trn_term> terms;
+                cudaEvent_t           ev[5]{nullptr, nullptr, nullptr, nullptr, nullptr};
+                void release() {
+                        for (cudaEvent_t e : ev)
+                                if (e)
+                                        cudaEventDestroy(e);
+                }
+        } ix;
 };
 
 #define CK(call)                                                                                                                                               \
@@ -314,6 +325,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         c->mt.release();
         c->it.release();
         c->pq.release();
+        c->ix.release();
         if (c->copy_stream)
                 cudaStreamDestroy(c->copy_stream);
         delete c;
@@ -1519,45 +1531,43 @@ extern "C" int trn_merge_topk(trn_ctx *c, const void *docids, const void *scores
 }
 
 // =================================================================================================== device-side encoder (GOOGLE)
-extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
-                                 uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
-                                 float *device_ms) {
-        if (!c)
-                return TRN_ERR_ARG;
-        if (!term_begin || !nterms || !out_bytes || !terms || block_docs == 0 || block_docs > 128 || skiplist_step == 0 ||
-            (countdown && (*countdown == 0 || *countdown > skiplist_step)))
-                return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
-        const uint64_t nposts = term_begin[nterms];
-        if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
-                return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
-        CK(cudaSetDevice(c->device));
+// Term-major postings resident in HBM, in the layout the encode kernels read: trn_encode_google / trn_encode_lucene upload the caller's,
+// trn_index_documents builds them on the device.  h_term_begin = the host's copy of term_begin (block and unit numbering is host work).
+struct DevPostings {
+        const uint64_t *          h_term_begin;
+        uint32_t                  nterms;
+        const unsigned long long *term_begin;
+        const uint32_t *          docids, *freqs, *positions; // positions null: 1..freq
+};
+struct FreeBufs {
+        std::vector<DevBuf *> v;
+        ~FreeBufs() {
+                for (auto b : v)
+                        b->release();
+        }
+};
+
+// The encode itself: sizes, scans and the write over device-resident postings; the chunks stay in d_out.  chunk[t] / toff[t] = bytes and
+// offset of term t's chunk, *out_bytes their total (set before the capacity refusals, as trn_encode_google documents), *nblocks the blocks
+// committed (the countdown's advance).  cap = the caller's buffer (have_out false: none).
+static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block_docs, uint32_t skiplist_step, uint32_t phase0, bool have_out, uint64_t cap,
+                                uint64_t *out_bytes, DevBuf &d_out, std::vector<uint64_t> &chunk, std::vector<uint64_t> &toff, uint64_t *nblocks_out,
+                                float *device_ms) {
+        const uint64_t *const term_begin = P.h_term_begin;
+        const uint32_t        nterms     = P.nterms;
+        const uint64_t        nposts     = term_begin[nterms];
+        const bool            positions  = P.positions != nullptr;
         std::vector<uint64_t> blk_begin(nterms + 1);
         uint64_t              nblocks{0};
         for (uint32_t t = 0; t < nterms; ++t) {
-                if (term_begin[t + 1] < term_begin[t] || term_begin[t + 1] - term_begin[t] > 0xffffffffull)
-                        return fail(c, TRN_ERR_ARG, "trn_encode_google: term_begin must ascend (at most 2^32 - 1 documents per term)");
                 blk_begin[t] = nblocks;
                 nblocks += (term_begin[t + 1] - term_begin[t] + block_docs - 1) / block_docs;
         }
         blk_begin[nterms] = nblocks;
-        uint64_t nhits{0};
-        if (positions)
-                for (uint64_t i = 0; i < nposts; ++i)
-                        nhits += freqs[i];
-        const uint32_t phase0 = countdown ? (skiplist_step - *countdown) % skiplist_step : 0u;
-        DevBuf d_tb, d_bb, d_doc, d_fr, d_pos, d_hb, d_bsz, d_bterm, d_boff, d_part, d_toff, d_cb, d_out, d_err;
-        struct Free {
-                std::vector<DevBuf *> v;
-                ~Free() {
-                        for (auto b : v)
-                                b->release();
-                }
-        } fr{{&d_tb, &d_bb, &d_doc, &d_fr, &d_pos, &d_hb, &d_bsz, &d_bterm, &d_boff, &d_part, &d_toff, &d_cb, &d_out, &d_err}};
+        DevBuf   d_bb, d_hb, d_bsz, d_bterm, d_boff, d_part, d_toff, d_cb, d_err;
+        FreeBufs fr{{&d_bb, &d_hb, &d_bsz, &d_bterm, &d_boff, &d_part, &d_toff, &d_cb, &d_err}};
         const size_t parts = size_t(std::max(nposts, nblocks) / 4096 + 4);
-        CK(d_tb.ensure((size_t(nterms) + 1) * 8));
         CK(d_bb.ensure((size_t(nterms) + 1) * 8));
-        CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
-        CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
         CK(d_bsz.ensure(std::max<size_t>(4, nblocks * 4)));
         CK(d_bterm.ensure(std::max<size_t>(4, nblocks * 4)));
         CK(d_boff.ensure((nblocks + 1) * 8));
@@ -1565,27 +1575,18 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         CK(d_toff.ensure((size_t(nterms) + 1) * 8));
         CK(d_cb.ensure(size_t(nterms) * 8));
         CK(d_err.ensure(4));
-        CK(cudaMemcpyAsync(d_tb.p, term_begin, (size_t(nterms) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_bb.p, blk_begin.data(), (size_t(nterms) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-        if (nposts) {
-                CK(cudaMemcpyAsync(d_doc.p, docids, nposts * 4, cudaMemcpyHostToDevice, c->stream));
-                CK(cudaMemcpyAsync(d_fr.p, freqs, nposts * 4, cudaMemcpyHostToDevice, c->stream));
-        }
-        if (positions) {
-                CK(d_pos.ensure(std::max<size_t>(4, nhits * 4)));
+        if (positions)
                 CK(d_hb.ensure((nposts + 1) * 8));
-                if (nhits)
-                        CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
-        }
         CK(cudaMemsetAsync(d_err.p, 0, 4, c->stream));
         EncParams E{};
-        E.term_begin    = d_tb.as<unsigned long long>();
+        E.term_begin    = P.term_begin;
         E.blk_begin     = d_bb.as<unsigned long long>();
         E.nterms        = nterms;
         E.nblocks       = nblocks;
-        E.docids        = d_doc.as<uint32_t>();
-        E.freqs         = d_fr.as<uint32_t>();
-        E.positions     = positions ? d_pos.as<uint32_t>() : nullptr;
+        E.docids        = P.docids;
+        E.freqs         = P.freqs;
+        E.positions     = P.positions;
         E.hit_begin     = positions ? d_hb.as<unsigned long long>() : nullptr;
         E.block_docs    = block_docs;
         E.skiplist_step = skiplist_step;
@@ -1598,14 +1599,15 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         cudaEvent_t e0 = c->ev0, e1 = c->ev1, e2 = c->evk0, e3 = c->evk1;
         CK(cudaEventRecord(e0, c->stream));
         if (positions)
-                CK(launch_enc_scan(d_fr.as<uint32_t>(), nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
+                CK(launch_enc_scan(P.freqs, nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
         CK(launch_enc_google_sizes(E, c->stream));
         CK(launch_enc_scan(d_bsz.as<uint32_t>(), nblocks, d_part.as<unsigned long long>(), d_boff.as<unsigned long long>(), c->stream));
         CK(launch_enc_term_sizes(E, d_cb.as<unsigned long long>(), c->stream));
         CK(cudaEventRecord(e1, c->stream));
         // chunk offsets: a prefix sum over the terms on the host (the output size must be known here anyway)
-        std::vector<uint64_t> chunk(nterms), toff(nterms + 1);
-        uint32_t              herr{0};
+        chunk.assign(nterms, 0);
+        toff.assign(size_t(nterms) + 1, 0);
+        uint32_t herr{0};
         CK(cudaMemcpyAsync(chunk.data(), d_cb.p, size_t(nterms) * 8, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaMemcpyAsync(&herr, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
@@ -1620,7 +1622,7 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         *out_bytes   = total;
         if (total >= (1ull << 32))
                 return fail(c, TRN_ERR_CAPACITY, "google encoder: the index of one source is limited to 4 GiB (range32_t, codecs.h:17-55)");
-        if (total > cap || !out)
+        if (total > cap || !have_out)
                 return fail(c, TRN_ERR_CAPACITY, "trn_encode_google: output buffer too small");
         CK(d_out.ensure(std::max<size_t>(4, total)));
         E.out = d_out.as<uint8_t>();
@@ -1629,15 +1631,8 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         CK(cudaMemsetAsync(d_out.p, 0, std::max<size_t>(4, total), c->stream)); // a term without documents is its zero u16
         CK(launch_enc_google_write(E, c->stream));
         CK(cudaEventRecord(e3, c->stream));
-        CK(cudaMemcpyAsync(out, d_out.p, total, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
-        for (uint32_t t = 0; t < nterms; ++t) {
-                terms[t].documents = uint32_t(term_begin[t + 1] - term_begin[t]);
-                terms[t].chunk_off = uint32_t(toff[t]);
-                terms[t].chunk_len = uint32_t(chunk[t]);
-        }
-        if (countdown)
-                *countdown = skiplist_step - uint32_t((uint64_t(phase0) + nblocks) % skiplist_step);
+        *nblocks_out = nblocks;
         if (device_ms) {
                 float a{0}, b{0};
                 CK(cudaEventElapsedTime(&a, e0, e1));
@@ -1648,24 +1643,71 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         return TRN_OK;
 }
 
-// =================================================================================================== device-side encoder (LUCENE)
-extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
-                                 uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
-                                 trn_term *terms, float *device_ms) {
+extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                                 uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
+                                 float *device_ms) {
         if (!c)
                 return TRN_ERR_ARG;
-        if (!term_begin || !nterms || !index_bytes || !hits_bytes || !terms)
-                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        if (!term_begin || !nterms || !out_bytes || !terms || block_docs == 0 || block_docs > 128 || skiplist_step == 0 ||
+            (countdown && (*countdown == 0 || *countdown > skiplist_step)))
+                return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
         const uint64_t nposts = term_begin[nterms];
         if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
-                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+                return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
+        CK(cudaSetDevice(c->device));
+        for (uint32_t t = 0; t < nterms; ++t)
+                if (term_begin[t + 1] < term_begin[t] || term_begin[t + 1] - term_begin[t] > 0xffffffffull)
+                        return fail(c, TRN_ERR_ARG, "trn_encode_google: term_begin must ascend (at most 2^32 - 1 documents per term)");
+        uint64_t nhits{0};
+        if (positions)
+                for (uint64_t i = 0; i < nposts; ++i)
+                        nhits += freqs[i];
+        const uint32_t phase0 = countdown ? (skiplist_step - *countdown) % skiplist_step : 0u;
+        DevBuf         d_tb, d_doc, d_fr, d_pos, d_out;
+        FreeBufs       fr{{&d_tb, &d_doc, &d_fr, &d_pos, &d_out}};
+        CK(d_tb.ensure((size_t(nterms) + 1) * 8));
+        CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(cudaMemcpyAsync(d_tb.p, term_begin, (size_t(nterms) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        if (nposts) {
+                CK(cudaMemcpyAsync(d_doc.p, docids, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_fr.p, freqs, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        if (positions) {
+                CK(d_pos.ensure(std::max<size_t>(4, nhits * 4)));
+                if (nhits)
+                        CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        const DevPostings     P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), positions ? d_pos.as<uint32_t>() : nullptr};
+        std::vector<uint64_t> chunk, toff;
+        uint64_t              nblocks{0};
+        if (const int r = encode_google_device(c, P, block_docs, skiplist_step, phase0, out != nullptr, cap, out_bytes, d_out, chunk, toff, &nblocks, device_ms))
+                return r;
+        CK(cudaMemcpyAsync(out, d_out.p, *out_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        for (uint32_t t = 0; t < nterms; ++t) {
+                terms[t].documents = uint32_t(term_begin[t + 1] - term_begin[t]);
+                terms[t].chunk_off = uint32_t(toff[t]);
+                terms[t].chunk_len = uint32_t(chunk[t]);
+        }
+        if (countdown)
+                *countdown = skiplist_step - uint32_t((uint64_t(phase0) + nblocks) % skiplist_step);
+        return TRN_OK;
+}
+
+// =================================================================================================== device-side encoder (LUCENE)
+// The encode itself over device-resident postings; index and hits.data stay in d_iout / d_hout.  toff[t] = offset of term t's chunk
+// (nterms + 1), *index_bytes / *hits_bytes the totals (set before the capacity refusals).  have_index / have_hits: the caller has buffers.
+static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_index, uint64_t index_cap, uint64_t *index_bytes, bool have_hits, uint64_t hits_cap,
+                                uint64_t *hits_bytes, DevBuf &d_iout, DevBuf &d_hout, std::vector<uint64_t> &toff, float *device_ms) {
+        const uint64_t *const term_begin = P.h_term_begin;
+        const uint32_t        nterms     = P.nterms;
+        const uint64_t        nposts     = term_begin[nterms];
         constexpr uint32_t N = Codecs::Lucene::BLOCK_SIZE;
         // doc units: every term's full blocks, then its tail; the chunk headers and skiplists around them are fixed by the block counts
         std::vector<uint64_t> dunit(nterms + 1), fixed(nterms + 1), hunit(nterms + 1), th(nterms + 1);
         uint64_t              ndunits{0}, fx{0};
         for (uint32_t t = 0; t < nterms; ++t) {
-                if (term_begin[t + 1] < term_begin[t] || term_begin[t + 1] - term_begin[t] > 0xffffffffull)
-                        return fail(c, TRN_ERR_ARG, "trn_encode_lucene: term_begin must ascend (at most 2^32 - 1 documents per term)");
                 const uint64_t nfull = (term_begin[t + 1] - term_begin[t]) / N;
                 dunit[t]             = ndunits;
                 fixed[t]             = fx;
@@ -1674,46 +1716,30 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
         }
         dunit[nterms] = ndunits;
         fixed[nterms] = fx;
-        CK(cudaSetDevice(c->device));
-        DevBuf d_tb, d_du, d_hu, d_fx, d_doc, d_fr, d_pos, d_hb, d_th, d_dsz, d_hsz, d_dterm, d_hterm, d_doff, d_hoff, d_part, d_toff, d_hto, d_iout, d_hout, d_err;
-        struct Free {
-                std::vector<DevBuf *> v;
-                ~Free() {
-                        for (auto b : v)
-                                b->release();
-                }
-        } fr{{&d_tb, &d_du, &d_hu, &d_fx, &d_doc, &d_fr, &d_pos, &d_hb, &d_th, &d_dsz, &d_hsz, &d_dterm, &d_hterm, &d_doff, &d_hoff, &d_part, &d_toff, &d_hto,
-              &d_iout, &d_hout, &d_err}};
+        DevBuf   d_du, d_hu, d_fx, d_hb, d_th, d_dsz, d_hsz, d_dterm, d_hterm, d_doff, d_hoff, d_part, d_toff, d_hto, d_err;
+        FreeBufs fr{{&d_du, &d_hu, &d_fx, &d_hb, &d_th, &d_dsz, &d_hsz, &d_dterm, &d_hterm, &d_doff, &d_hoff, &d_part, &d_toff, &d_hto, &d_err}};
         const size_t tw = (size_t(nterms) + 1) * 8;
-        CK(d_tb.ensure(tw));
         CK(d_du.ensure(tw));
         CK(d_hu.ensure(tw));
         CK(d_fx.ensure(tw));
         CK(d_th.ensure(tw));
         CK(d_toff.ensure(tw));
         CK(d_hto.ensure(tw));
-        CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
-        CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
         CK(d_hb.ensure((nposts + 1) * 8));
         CK(d_dsz.ensure(ndunits * 4));
         CK(d_dterm.ensure(ndunits * 4));
         CK(d_doff.ensure((ndunits + 1) * 8));
         CK(d_err.ensure(4));
-        CK(cudaMemcpyAsync(d_tb.p, term_begin, tw, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_du.p, dunit.data(), tw, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_fx.p, fixed.data(), tw, cudaMemcpyHostToDevice, c->stream));
-        if (nposts) {
-                CK(cudaMemcpyAsync(d_doc.p, docids, nposts * 4, cudaMemcpyHostToDevice, c->stream));
-                CK(cudaMemcpyAsync(d_fr.p, freqs, nposts * 4, cudaMemcpyHostToDevice, c->stream));
-        }
         CK(cudaMemsetAsync(d_err.p, 0, 4, c->stream));
         // (1) hits of every posting (scan of the freqs) and of every term; the host needs the per-term totals to number the hit units
         CK(d_part.ensure(size_t(std::max(nposts, ndunits) / 4096 + 4) * 8));
         float          ms{0}, a{0};
         cudaEvent_t    e0 = c->ev0, e1 = c->ev1;
         CK(cudaEventRecord(e0, c->stream));
-        CK(launch_enc_scan(d_fr.as<uint32_t>(), nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
-        CK(launch_enc_lucene_term_hits(d_tb.as<unsigned long long>(), d_hb.as<unsigned long long>(), nterms, d_th.as<unsigned long long>(), c->stream));
+        CK(launch_enc_scan(P.freqs, nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
+        CK(launch_enc_lucene_term_hits(P.term_begin, d_hb.as<unsigned long long>(), nterms, d_th.as<unsigned long long>(), c->stream));
         CK(cudaEventRecord(e1, c->stream));
         CK(cudaMemcpyAsync(th.data(), d_th.p, tw, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
@@ -1731,22 +1757,18 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
         CK(d_hoff.ensure((nhunits + 1) * 8));
         CK(d_part.ensure(size_t(nhunits / 4096 + 4) * 8));
         CK(cudaMemcpyAsync(d_hu.p, hunit.data(), tw, cudaMemcpyHostToDevice, c->stream));
-        if (positions && nhits) {
-                CK(d_pos.ensure(nhits * 4));
-                CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
-        }
         EncLuceneParams E{};
-        E.term_begin  = d_tb.as<unsigned long long>();
+        E.term_begin  = P.term_begin;
         E.dunit_begin = d_du.as<unsigned long long>();
         E.hunit_begin = d_hu.as<unsigned long long>();
         E.nterms      = nterms;
         E.ndunits     = ndunits;
         E.nhunits     = nhunits;
-        E.docids      = d_doc.as<uint32_t>();
-        E.freqs       = d_fr.as<uint32_t>();
-        E.positions   = positions && nhits ? d_pos.as<uint32_t>() : nullptr;
+        E.docids      = P.docids;
+        E.freqs       = P.freqs;
+        E.positions   = nhits ? P.positions : nullptr;
         E.hit_begin   = d_hb.as<unsigned long long>();
-        E.dsz         = d_dsz.as<uint32_t>();
+        E.dsz       = d_dsz.as<uint32_t>();
         E.hsz         = d_hsz.as<uint32_t>();
         E.dterm       = d_dterm.as<uint32_t>();
         E.hterm       = d_hterm.as<uint32_t>();
@@ -1761,8 +1783,9 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
         CK(launch_enc_scan(d_hsz.as<uint32_t>(), nhunits, d_part.as<unsigned long long>(), d_hoff.as<unsigned long long>(), c->stream));
         CK(launch_enc_lucene_terms(E, d_fx.as<unsigned long long>(), d_toff.as<unsigned long long>(), d_hto.as<unsigned long long>(), c->stream));
         CK(cudaEventRecord(e1, c->stream));
-        std::vector<uint64_t> toff(nterms + 1), hto(nterms + 1);
+        std::vector<uint64_t> hto(nterms + 1);
         uint32_t              herr{0};
+        toff.assign(size_t(nterms) + 1, 0);
         CK(cudaMemcpyAsync(toff.data(), d_toff.p, tw, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaMemcpyAsync(hto.data(), d_hto.p, tw, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaMemcpyAsync(&herr, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
@@ -1776,7 +1799,7 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
         *hits_bytes          = htotal;
         if (total >= (1ull << 32) || htotal >= (1ull << 32))
                 return fail(c, TRN_ERR_CAPACITY, "lucene encoder: the index and hits.data of one source are limited to 4 GiB (u32 chunk and hits offsets)");
-        if (total > index_cap || htotal > hits_cap || !index_out || (htotal && !hits_out))
+        if (total > index_cap || htotal > hits_cap || !have_index || (htotal && !have_hits))
                 return fail(c, TRN_ERR_CAPACITY, "trn_encode_lucene: output buffer too small");
         CK(d_iout.ensure(std::max<size_t>(4, total)));
         CK(d_hout.ensure(std::max<size_t>(4, htotal)));
@@ -1786,20 +1809,355 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
         CK(cudaEventRecord(e0, c->stream));
         CK(launch_enc_lucene_write(E, c->stream));
         CK(cudaEventRecord(e1, c->stream));
-        CK(cudaMemcpyAsync(index_out, d_iout.p, total, cudaMemcpyDeviceToHost, c->stream));
-        if (htotal)
-                CK(cudaMemcpyAsync(hits_out, d_hout.p, htotal, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         CK(cudaEventElapsedTime(&a, e0, e1));
         ms += a;
+        if (device_ms)
+                *device_ms = ms;
+        c->have_kernel_events = false;
+        return TRN_OK;
+}
+
+extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                                 uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
+                                 trn_term *terms, float *device_ms) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (!term_begin || !nterms || !index_bytes || !hits_bytes || !terms)
+                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        const uint64_t nposts = term_begin[nterms];
+        if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
+                return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        for (uint32_t t = 0; t < nterms; ++t)
+                if (term_begin[t + 1] < term_begin[t] || term_begin[t + 1] - term_begin[t] > 0xffffffffull)
+                        return fail(c, TRN_ERR_ARG, "trn_encode_lucene: term_begin must ascend (at most 2^32 - 1 documents per term)");
+        uint64_t nhits{0};
+        if (positions)
+                for (uint64_t i = 0; i < nposts; ++i)
+                        nhits += freqs[i];
+        CK(cudaSetDevice(c->device));
+        DevBuf   d_tb, d_doc, d_fr, d_pos, d_iout, d_hout;
+        FreeBufs fr{{&d_tb, &d_doc, &d_fr, &d_pos, &d_iout, &d_hout}};
+        const size_t tw = (size_t(nterms) + 1) * 8;
+        CK(d_tb.ensure(tw));
+        CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
+        CK(cudaMemcpyAsync(d_tb.p, term_begin, tw, cudaMemcpyHostToDevice, c->stream));
+        if (nposts) {
+                CK(cudaMemcpyAsync(d_doc.p, docids, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_fr.p, freqs, nposts * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        if (nhits) {
+                CK(d_pos.ensure(nhits * 4));
+                CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        const DevPostings     P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), nhits ? d_pos.as<uint32_t>() : nullptr};
+        std::vector<uint64_t> toff;
+        if (const int r = encode_lucene_device(c, P, index_out != nullptr, index_cap, index_bytes, hits_out != nullptr, hits_cap, hits_bytes, d_iout, d_hout, toff, device_ms))
+                return r;
+        CK(cudaMemcpyAsync(index_out, d_iout.p, *index_bytes, cudaMemcpyDeviceToHost, c->stream));
+        if (*hits_bytes)
+                CK(cudaMemcpyAsync(hits_out, d_hout.p, *hits_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
         for (uint32_t t = 0; t < nterms; ++t) {
                 terms[t].documents = uint32_t(term_begin[t + 1] - term_begin[t]);
                 terms[t].chunk_off = uint32_t(toff[t]);
                 terms[t].chunk_len = uint32_t(toff[t + 1] - toff[t]);
         }
-        if (device_ms)
-                *device_ms = ms;
-        c->have_kernel_events = false;
+        return TRN_OK;
+}
+
+// =================================================================================================== indexer
+// == SegmentIndexSession begin / insert / commit for one batch of documents (indexer.cpp:14-153, 311-564): the doc-major -> term-major
+// inversion is a keys-only radix sort on the device (index_docs.cuh), its output feeds the device encoders without a host round trip.
+namespace {
+struct IndexPass {
+        uint32_t shift, bits;
+};
+// the passes of the LSD sort over the key bits that can be non-zero (`active`): groups of up to 8 bits starting at an active bit and ending
+// at one; a digit that is constant over all keys is never sorted by
+std::vector<IndexPass> plan_radix_passes(uint64_t active) {
+        std::vector<IndexPass> v;
+        for (uint32_t b = 0; b < 64;) {
+                if (!((active >> b) & 1u)) {
+                        ++b;
+                        continue;
+                }
+                uint32_t bits = std::min(8u, 64u - b);
+                while (bits > 1 && !((active >> (b + bits - 1)) & 1u))
+                        --bits;
+                v.push_back({b, bits});
+                b += bits;
+        }
+        return v;
+}
+uint64_t low_bits_for(uint64_t maxv) { // mask of the bits the values 0 .. maxv use
+        uint32_t b = 0;
+        while (b < 64 && (maxv >> b))
+                ++b;
+        return b == 64 ? ~0ull : (1ull << b) - 1;
+}
+} // namespace
+
+// working memory of the indexer: an allocation failure is a refusal (split the batch), not a CUDA error
+#define CKM(call)                                                                                                                                              \
+        do {                                                                                                                                                   \
+                cudaError_t e__ = (call);                                                                                                                      \
+                if (e__ == cudaErrorMemoryAllocation) {                                                                                                        \
+                        cudaGetLastError();                                                                                                                    \
+                        return fail(c, TRN_ERR_CAPACITY, "trn_index_documents: working memory cannot be allocated on the device; split the batch");           \
+                }                                                                                                                                              \
+                if (e__ != cudaSuccess) {                                                                                                                      \
+                        c->err = std::string(#call) + ": " + cudaGetErrorString(e__);                                                                          \
+                        return TRN_ERR_CUDA;                                                                                                                   \
+                }                                                                                                                                              \
+        } while (0)
+
+// sorts n keys by the planned passes; the result is in *sorted (a or b).  No host synchronisation.
+static int index_radix_sort(trn_ctx *c, DevBuf &a, DevBuf &b, uint64_t n, const std::vector<IndexPass> &passes, DevBuf &counts, DevBuf &part, DevBuf &offs,
+                            unsigned long long **sorted) {
+        const uint64_t ntiles = (n + 4095) / 4096;
+        uint32_t       maxbits{1};
+        for (const auto &p : passes)
+                maxbits = std::max(maxbits, p.bits);
+        const uint64_t ncounts = (uint64_t(1) << maxbits) * ntiles;
+        CKM(counts.ensure(ncounts * 4));
+        CKM(offs.ensure((ncounts + 1) * 8));
+        CKM(part.ensure((ncounts / 4096 + 4) * 8));
+        unsigned long long *in = a.as<unsigned long long>(), *out = b.as<unsigned long long>();
+        for (const auto &p : passes) {
+                CK(launch_radix_pass(in, out, n, p.shift, p.bits, counts.as<uint32_t>(), part.as<unsigned long long>(), offs.as<unsigned long long>(), c->stream));
+                std::swap(in, out);
+        }
+        *sorted = in;
+        return TRN_OK;
+}
+
+extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
+                                   uint32_t ndocs, uint32_t nterms, trn_indexed *out) {
+        if (!c)
+                return TRN_ERR_ARG;
+        const double t_begin = now_ms();
+        if (!docids || !doc_offsets || !out || !ndocs || !nterms || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || doc_offsets[0] != 0)
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: bad arguments");
+        if (nterms > kIndexMaxTerms)
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: " + std::to_string(nterms) + " terms: at most 2^24 per call");
+        if (ndocs > kIndexMaxDocs)
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: " + std::to_string(ndocs) + " documents: at most 2^26 per call");
+        uint64_t maxlen{0};
+        uint32_t docs_cnt{0}, max_docid{0};
+        for (uint32_t d = 0; d < ndocs; ++d) {
+                if (doc_offsets[d + 1] < doc_offsets[d])
+                        return fail(c, TRN_ERR_ARG, "trn_index_documents: document " + std::to_string(d) + ": doc_offsets must ascend");
+                const uint64_t len = doc_offsets[d + 1] - doc_offsets[d];
+                if (!positions && len > 16383u)
+                        return fail(c, TRN_ERR_ARG, "trn_index_documents: document " + std::to_string(d) + " (docID " + std::to_string(docids[d]) + "): " +
+                                                        std::to_string(len) + " tokens: positions must be below 16384 (Limits::MaxPosition)");
+                maxlen = std::max(maxlen, len);
+                docs_cnt += len != 0;
+                max_docid = std::max(max_docid, docids[d]);
+        }
+        const uint64_t ntok = doc_offsets[ndocs];
+        if (ntok && !tokens)
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: bad arguments");
+        CK(cudaSetDevice(c->device));
+        auto &X = c->ix;
+        for (auto &e : X.ev)
+                if (!e)
+                        CK(cudaEventCreate(&e));
+        const auto doc_of_token = [&](uint64_t i) { return uint32_t(std::upper_bound(doc_offsets, doc_offsets + ndocs + 1, i) - doc_offsets) - 1u; };
+        const auto who          = [&](uint32_t d) { return "trn_index_documents: document " + std::to_string(d) + " (docID " + std::to_string(docids[d]) + "): "; };
+
+        DevBuf   d_docids, d_doff, d_tok, d_pos, d_ka, d_kb, d_rank, d_docid_of, d_err, d_counts, d_part, d_offs, d_pflag, d_tflag, d_pscan, d_tscan, d_pbegin, d_tb, d_order,
+            d_odoc, d_ofreq, d_opos, d_docterms, d_out, d_hout;
+        FreeBufs fr{{&d_docids, &d_doff, &d_tok, &d_pos, &d_ka, &d_kb, &d_rank, &d_docid_of, &d_err, &d_counts, &d_part, &d_offs, &d_pflag, &d_tflag, &d_pscan,
+                     &d_tscan, &d_pbegin, &d_tb, &d_order, &d_odoc, &d_ofreq, &d_opos, &d_docterms, &d_out, &d_hout}};
+        uint64_t herr[IDX_ERR_KINDS];
+        // ---- documents: ranks in docID order, docID 0 and duplicates
+        CKM(d_docids.ensure(size_t(ndocs) * 4));
+        CKM(d_doff.ensure((size_t(ndocs) + 1) * 8));
+        CKM(d_ka.ensure(std::max<uint64_t>(ndocs, ntok) * 8));
+        CKM(d_kb.ensure(std::max<uint64_t>(ndocs, ntok) * 8));
+        CKM(d_rank.ensure(size_t(ndocs) * 4));
+        CKM(d_docid_of.ensure(size_t(ndocs) * 4));
+        CKM(d_err.ensure(sizeof herr));
+        CKM(d_tok.ensure(std::max<uint64_t>(1, ntok) * 4));
+        if (positions)
+                CKM(d_pos.ensure(std::max<uint64_t>(1, ntok) * 4));
+        CK(cudaMemcpyAsync(d_docids.p, docids, size_t(ndocs) * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_doff.p, doc_offsets, (size_t(ndocs) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        if (ntok) {
+                CK(cudaMemcpyAsync(d_tok.p, tokens, ntok * 4, cudaMemcpyHostToDevice, c->stream));
+                if (positions)
+                        CK(cudaMemcpyAsync(d_pos.p, positions, ntok * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        CK(cudaMemsetAsync(d_err.p, 0xff, sizeof herr, c->stream));
+        const uint64_t doc_active = low_bits_for(ndocs - 1u) | (low_bits_for(max_docid) << 32);
+        const uint64_t key_active = low_bits_for(positions ? 16383u : maxlen) | (low_bits_for(ndocs - 1u) << 14) | (low_bits_for(nterms - 1u) << 40);
+        const auto     doc_passes = plan_radix_passes(doc_active), key_passes = plan_radix_passes(key_active);
+        CK(cudaEventRecord(X.ev[0], c->stream));
+        CK(launch_index_doc_keys(d_docids.as<uint32_t>(), ndocs, d_ka.as<unsigned long long>(), c->stream));
+        unsigned long long *sorted{nullptr};
+        if (const int r = index_radix_sort(c, d_ka, d_kb, ndocs, doc_passes, d_counts, d_part, d_offs, &sorted))
+                return r;
+        CK(launch_index_doc_ranks(sorted, ndocs, d_rank.as<uint32_t>(), d_docid_of.as<uint32_t>(), d_err.as<unsigned long long>(), c->stream));
+        // ---- tokens: keys, the sort
+        IndexParams P{};
+        P.doc_off   = d_doff.as<unsigned long long>();
+        P.tokens    = d_tok.as<uint32_t>();
+        P.positions = positions ? d_pos.as<uint32_t>() : nullptr;
+        P.ndocs     = ndocs;
+        P.nterms    = nterms;
+        P.ntokens   = ntok;
+        P.rank_of   = d_rank.as<uint32_t>();
+        P.docid_of  = d_docid_of.as<uint32_t>();
+        P.keys      = d_ka.as<unsigned long long>();
+        P.errors    = d_err.as<unsigned long long>();
+        CK(launch_index_keys(P, c->stream));
+        if (const int r = index_radix_sort(c, d_ka, d_kb, ntok, key_passes, d_counts, d_part, d_offs, &sorted))
+                return r;
+        CK(cudaEventRecord(X.ev[1], c->stream));
+        // ---- postings: flags and their scans
+        CKM(d_pflag.ensure(std::max<uint64_t>(1, ntok) * 4));
+        CKM(d_tflag.ensure(std::max<uint64_t>(1, ntok) * 4));
+        CKM(d_pscan.ensure((ntok + 1) * 8));
+        CKM(d_tscan.ensure((ntok + 1) * 8));
+        CKM(d_part.ensure((ntok / 4096 + 4) * 8));
+        CK(launch_post_flags(sorted, ntok, d_pflag.as<uint32_t>(), d_tflag.as<uint32_t>(), c->stream));
+        CK(launch_enc_scan(d_pflag.as<uint32_t>(), ntok, d_part.as<unsigned long long>(), d_pscan.as<unsigned long long>(), c->stream));
+        CK(launch_enc_scan(d_tflag.as<uint32_t>(), ntok, d_part.as<unsigned long long>(), d_tscan.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(X.ev[2], c->stream));
+        uint64_t nposts{0}, npresent{0};
+        CK(cudaMemcpyAsync(&nposts, d_pscan.as<unsigned long long>() + ntok, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(&npresent, d_tscan.as<unsigned long long>() + ntok, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(herr, d_err.p, sizeof herr, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        if (herr[IDX_ERR_DOC0] != ~0ull)
+                return fail(c, TRN_ERR_ARG, who(uint32_t(herr[IDX_ERR_DOC0])) + "docID 0 is not a document");
+        if (herr[IDX_ERR_DUP] != ~0ull)
+                return fail(c, TRN_ERR_ARG, who(uint32_t(herr[IDX_ERR_DUP])) + "the docID is given twice (Already committed document, indexer.cpp:219-222)");
+        if (herr[IDX_ERR_TOKEN] != ~0ull) {
+                const uint64_t i = herr[IDX_ERR_TOKEN];
+                return fail(c, TRN_ERR_ARG, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) + " is term " + std::to_string(tokens[i]) +
+                                                ", not below nterms = " + std::to_string(nterms));
+        }
+        if (herr[IDX_ERR_POS] != ~0ull) {
+                const uint64_t i = herr[IDX_ERR_POS];
+                return fail(c, TRN_ERR_ARG, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) + " has position " +
+                                                std::to_string(positions ? positions[i] : 0u) + ": positions must be below 16384 (Limits::MaxPosition)");
+        }
+        if (herr[IDX_ERR_POS0] != ~0ull) {
+                const uint64_t i = herr[IDX_ERR_POS0];
+                return fail(c, TRN_ERR_UNSUPPORTED, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) +
+                                                        " has position 0: hits without a position are not indexed");
+        }
+        // ---- postings: docids, freqs, positions, term_begin in the layout the encode kernels read
+        CKM(d_pbegin.ensure((nposts + 1) * 8));
+        CKM(d_tb.ensure((npresent + 1) * 8));
+        CKM(d_order.ensure(std::max<uint64_t>(1, npresent) * 4));
+        CKM(d_odoc.ensure(std::max<uint64_t>(1, nposts) * 4));
+        CKM(d_ofreq.ensure(std::max<uint64_t>(1, nposts) * 4));
+        CKM(d_opos.ensure(std::max<uint64_t>(1, ntok) * 4));
+        if (nterms > 65535u) {
+                CKM(d_docterms.ensure(size_t(ndocs) * 4));
+                CK(cudaMemsetAsync(d_docterms.p, 0, size_t(ndocs) * 4, c->stream));
+        }
+        P.post_flag     = d_pflag.as<uint32_t>();
+        P.term_flag     = d_tflag.as<uint32_t>();
+        P.post_scan     = d_pscan.as<unsigned long long>();
+        P.term_scan     = d_tscan.as<unsigned long long>();
+        P.post_begin    = d_pbegin.as<unsigned long long>();
+        P.term_begin    = d_tb.as<unsigned long long>();
+        P.term_order    = d_order.as<uint32_t>();
+        P.out_docids    = d_odoc.as<uint32_t>();
+        P.out_freqs     = d_ofreq.as<uint32_t>();
+        P.out_positions = d_opos.as<uint32_t>();
+        P.doc_terms     = nterms > 65535u ? d_docterms.as<uint32_t>() : nullptr;
+        CK(cudaEventRecord(X.ev[3], c->stream));
+        CK(launch_post_write(P, sorted, c->stream));
+        CK(launch_post_freqs(P, nposts, c->stream));
+        CK(cudaEventRecord(X.ev[4], c->stream));
+        std::vector<uint64_t> h_tb(npresent + 1);
+        std::vector<uint32_t> h_order(npresent);
+        CK(cudaMemcpyAsync(h_tb.data(), d_tb.p, (npresent + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        if (npresent)
+                CK(cudaMemcpyAsync(h_order.data(), d_order.p, npresent * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(herr, d_err.p, sizeof herr, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        if (herr[IDX_ERR_FREQ] != ~0ull) {
+                const uint64_t p = herr[IDX_ERR_FREQ];
+                uint32_t       doc{0};
+                CK(cudaMemcpy(&doc, d_odoc.as<uint32_t>() + p, 4, cudaMemcpyDeviceToHost));
+                const size_t j = size_t(std::upper_bound(h_tb.begin(), h_tb.end(), p) - h_tb.begin()) - 1;
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: docID " + std::to_string(doc) + " holds term " + std::to_string(index_term_at(h_order[j], nterms)) +
+                                                " more than 65535 times (a uint16_t count, indexer.cpp:102-103)");
+        }
+        if (herr[IDX_ERR_DOCTERMS] != ~0ull) {
+                uint32_t doc{0};
+                CK(cudaMemcpy(&doc, d_docid_of.as<uint32_t>() + herr[IDX_ERR_DOCTERMS], 4, cudaMemcpyDeviceToHost));
+                return fail(c, TRN_ERR_ARG, "trn_index_documents: docID " + std::to_string(doc) + " holds more than 65535 distinct terms (a uint16_t count, indexer.cpp:49,111)");
+        }
+        float sort_ms{0}, a_ms{0}, b_ms{0}, enc_ms{0};
+        CK(cudaEventElapsedTime(&sort_ms, X.ev[0], X.ev[1]));
+        CK(cudaEventElapsedTime(&a_ms, X.ev[1], X.ev[2]));
+        CK(cudaEventElapsedTime(&b_ms, X.ev[3], X.ev[4]));
+        for (DevBuf *b : {&d_docids, &d_doff, &d_tok, &d_pos, &d_ka, &d_kb, &d_rank, &d_docid_of, &d_counts, &d_part, &d_offs, &d_pflag, &d_tflag, &d_pscan, &d_tscan,
+                          &d_pbegin, &d_order, &d_docterms})
+                b->release();
+        // ---- encode the device-resident postings: terms in index order, the reference's geometry, a fresh session
+        std::vector<uint8_t>  index, hits;
+        std::vector<trn_term> terms(nterms, trn_term{0, 0, 0});
+        std::vector<uint64_t> chunk, toff;
+        uint64_t              index_bytes{0}, hits_bytes{0};
+        if (npresent) {
+                const DevPostings DP{h_tb.data(), uint32_t(npresent), d_tb.as<unsigned long long>(), d_odoc.as<uint32_t>(), d_ofreq.as<uint32_t>(), d_opos.as<uint32_t>()};
+                int               r;
+                if (codec == TRN_CODEC_GOOGLE) {
+                        uint64_t nblocks{0};
+                        r = encode_google_device(c, DP, 32, 8, 0, true, ~0ull, &index_bytes, d_out, chunk, toff, &nblocks, &enc_ms);
+                } else
+                        r = encode_lucene_device(c, DP, true, ~0ull, &index_bytes, true, ~0ull, &hits_bytes, d_out, d_hout, toff, &enc_ms);
+                if (r == TRN_ERR_CUDA && c->err.find("out of memory") != std::string::npos)
+                        return fail(c, TRN_ERR_CAPACITY, "trn_index_documents: working memory cannot be allocated on the device; split the batch");
+                if (r)
+                        return r;
+                try {
+                        index.resize(index_bytes);
+                        hits.resize(hits_bytes);
+                } catch (const std::bad_alloc &) {
+                        return fail(c, TRN_ERR_CAPACITY, "trn_index_documents: the result cannot be allocated on the host");
+                }
+                CK(cudaMemcpyAsync(index.data(), d_out.p, index_bytes, cudaMemcpyDeviceToHost, c->stream));
+                if (hits_bytes)
+                        CK(cudaMemcpyAsync(hits.data(), d_hout.p, hits_bytes, cudaMemcpyDeviceToHost, c->stream));
+                CK(cudaStreamSynchronize(c->stream));
+                for (size_t j = 0; j < npresent; ++j) {
+                        trn_term &t = terms[index_term_at(h_order[j], nterms)];
+                        t.documents = uint32_t(h_tb[j + 1] - h_tb[j]);
+                        t.chunk_off = uint32_t(toff[j]);
+                        t.chunk_len = uint32_t(toff[j + 1] - toff[j]);
+                }
+        }
+        X.index.swap(index);
+        X.hits.swap(hits);
+        X.terms.swap(terms);
+        *out                = trn_indexed{};
+        out->index          = X.index.data();
+        out->index_bytes    = X.index.size();
+        out->hits           = X.hits.data();
+        out->hits_bytes     = X.hits.size();
+        out->terms          = X.terms.data();
+        out->nterms         = nterms;
+        out->docs_cnt       = docs_cnt;
+        out->total_terms    = uint32_t(npresent);
+        out->sum_terms_docs = nposts;
+        out->sum_term_hits  = ntok;
+        out->max_docid      = max_docid;
+        out->sort_passes    = uint32_t(doc_passes.size() + key_passes.size());
+        out->sort_ms        = sort_ms;
+        out->postings_ms    = a_ms + b_ms;
+        out->encode_ms      = enc_ms;
+        out->total_ms       = float(now_ms() - t_begin);
         return TRN_OK;
 }
 

@@ -1075,6 +1075,7 @@ __global__ void __launch_bounds__(kThreads) k_decode_terms(DevIndex ix, const ui
 #include "collect.cuh"
 #include "intersect.cuh"
 #include "percolate.cuh"
+#include "index_docs.cuh"
 
 // ------------------------------------------------------------------------------------------------ launch wrappers
 uint32_t exec_stage_bytes(int codec) {

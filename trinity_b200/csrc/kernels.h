@@ -53,6 +53,16 @@ cudaError_t launch_isect_carry(const IsectParams &P, unsigned long long *carry, 
 // percolator (percolate.cuh): the count (write false) and write passes of trn_percolate over one launch's documents
 size_t      perc_smem_bytes(uint32_t max_len, uint32_t max_hash, bool write);
 cudaError_t launch_perc(const PercParams &P, bool write, int num_sms, cudaStream_t stream);
+// indexer (index_docs.cuh): document ranks, sort keys, one pass of the keys-only radix sort, the postings pass of trn_index_documents
+cudaError_t launch_index_doc_keys(const uint32_t *docids, uint32_t ndocs, unsigned long long *keys, cudaStream_t stream);
+cudaError_t launch_index_doc_ranks(const unsigned long long *keys, uint32_t ndocs, uint32_t *rank_of, uint32_t *docid_of, unsigned long long *errors,
+                                   cudaStream_t stream);
+cudaError_t launch_index_keys(const IndexParams &P, cudaStream_t stream);
+cudaError_t launch_radix_pass(const unsigned long long *in, unsigned long long *out, uint64_t n, uint32_t shift, uint32_t bits, uint32_t *counts,
+                              unsigned long long *partials, unsigned long long *offsets, cudaStream_t stream);
+cudaError_t launch_post_flags(const unsigned long long *keys, uint64_t n, uint32_t *post_flag, uint32_t *term_flag, cudaStream_t stream);
+cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *keys, cudaStream_t stream);
+cudaError_t launch_post_freqs(const IndexParams &P, uint64_t nposts, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
 } // namespace trn
