@@ -336,6 +336,10 @@ int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, const trn_t
  * first tile and the end tile (exclusive) it covers, all inside one 2^17-docID run. */
 int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
                          uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n, char *err, size_t errcap);
+/* The same for the flat ANDs with exactly one operand without a resident bitmap (the others with one): their run-major tickets follow the
+ * all-bitmap ones (TRN_MIXED_RUNS=0 turns them off).  Same arguments and rows as trn_debug_dense_runs. */
+int trn_debug_mixed_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
+                         uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n, char *err, size_t errcap);
 
 /* Host-only view of the dense-term selection (tests, tooling; no GPU needed): the terms trn_upload_index would keep a resident docID
  * bitmap for on a context that trn_create made with this environment (TRN_DENSE_BITMAPS, TRN_DENSE_BUDGET).  A GOOGLE term qualifies when

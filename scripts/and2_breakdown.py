@@ -1,4 +1,5 @@
-"""Time the and2 batch of bench.py by route class, with the all-bitmap flat ANDs on their run-major tickets and with TRN_DENSE_RUNS=0.
+"""Time the and2 batch of bench.py by route class: with the flat ANDs on their run-major tickets (the default), with TRN_MIXED_RUNS=0 (the
+flat ANDs with one bitmap operand on per-tile tickets) and with TRN_DENSE_RUNS=0 TRN_MIXED_RUNS=0 (every flat AND on per-tile tickets).
 
 Builds bench.py's GOOGLE index and and2 batch, splits the batch into
   both    flat AND, both operands with a resident bitmap
@@ -6,7 +7,7 @@ Builds bench.py's GOOGLE index and and2 batch, splits the batch into
   none    flat AND, no bitmap
   cand    candidate-driven
 and times each class as its own device-resident batch (exec_batch_device, as bench.py; CUDA events over --steps steps after --warmup) on
-two sources over the same index, created with TRN_DENSE_RUNS=1 and =0, alternating.  Per class it prints ms per step, (query, tile) work
+three sources over the same index, created with those settings, alternating.  Per class it prints ms per step, (query, tile) work
 items (candidate-driven: lead-term groups), matches, result words, and the modelled HBM bytes of bitmap reads: per-tile order (every
 item reads its operands' tile words) and run-major order (every bitmap run read once).  Needs a GPU; prints the card and its power limit.
 
@@ -27,12 +28,16 @@ import bench  # noqa: E402
 import trinity_b200 as tb  # noqa: E402
 
 
-def source(synth, ndocs, runs):
-    os.environ["TRN_DENSE_RUNS"] = "1" if runs else "0"
+SETTINGS = {"runs": {}, "mixed_tiles": {"TRN_MIXED_RUNS": "0"}, "tiles": {"TRN_DENSE_RUNS": "0", "TRN_MIXED_RUNS": "0"}}
+
+
+def source(synth, ndocs, env):
+    os.environ.update(env)
     try:
         g = tb.GpuIndexSource(0)
     finally:
-        os.environ.pop("TRN_DENSE_RUNS")
+        for k in env:
+            os.environ.pop(k)
     g.upload(tb.CODEC_GOOGLE, np.asarray(synth.index), np.asarray(synth.terms), ndocs)
     return g
 
@@ -50,7 +55,7 @@ def main():
 
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     synth = tb.SynthIndex(tb.CODEC_GOOGLE, args.ndocs, args.nterms, threads=max(1, len(os.sched_getaffinity(0))))
-    srcs = {"runs": source(synth, args.ndocs, True), "tiles": source(synth, args.ndocs, False)}
+    srcs = {k: source(synth, args.ndocs, env) for k, env in SETTINGS.items()}
     g = srcs["runs"]
     texts, _ = bench.gen_queries("and2", args.nq, args.nterms)
     tdict = tb.TermDictionary(synth.names)
@@ -96,7 +101,7 @@ def main():
                 old_b += tiles * len(nd) * (tile // 8)
                 used |= set(nd)
         # run-major order reads each bitmap the class uses once; the other classes keep the per-tile order
-        new_b = sum(bitmap_bytes(t) for t in used) if name == "both" else old_b
+        new_b = sum(bitmap_bytes(t) for t in used) if name in ("both", "one") else old_b
         ms = {k: [] for k in srcs}
         for _ in range(args.rounds):
             for key, s in srcs.items():
@@ -112,8 +117,8 @@ def main():
                 ms[key].append(e0.elapsed_time(e1) / args.steps)
         res = g.exec_batch(sub, tb.MODE_DOCS_COMPACT, copy=False)
         print(json.dumps({"class": name, "queries": len(qs), "work_items": items, "matches": int(res.match_counts.sum()),
-                          "result_bytes": res.result_bytes(), "ms_per_step_runs": [round(x, 3) for x in ms["runs"]],
-                          "ms_per_step_tiles": [round(x, 3) for x in ms["tiles"]], "bitmap_bytes_per_tile_order": old_b,
+                          "result_bytes": res.result_bytes(), **{f"ms_per_step_{k}": [round(x, 3) for x in v] for k, v in ms.items()},
+                          "bitmap_bytes_per_tile_order": old_b,
                           "bitmap_bytes_run_major": new_b}))
     for s in srcs.values():
         s.close()

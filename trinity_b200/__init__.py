@@ -304,6 +304,15 @@ def debug_plan(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequen
 def debug_dense_runs(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequence[np.ndarray], mode: int, k: int = 100, max_docid: int = 0):
     """(qtiles, tickets): the same plan's (tile_lo, ntiles) of every query, and the run-major tickets of its all-bitmap flat ANDs in launch
     order, one row (query, first tile, end tile) each — the tiles [first, end) of one 2^17-docID run"""
+    return _debug_run_tickets(lib().trn_debug_dense_runs, codec, index, terms, queries, mode, k, max_docid)
+
+
+def debug_mixed_runs(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequence[np.ndarray], mode: int, k: int = 100, max_docid: int = 0):
+    """as debug_dense_runs, for the flat ANDs with exactly one operand without a resident bitmap"""
+    return _debug_run_tickets(lib().trn_debug_mixed_runs, codec, index, terms, queries, mode, k, max_docid)
+
+
+def _debug_run_tickets(fn, codec, index, terms, queries, mode, k, max_docid):
     index = np.ascontiguousarray(index, dtype=np.uint8)
     terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)
     arr, keep = _pack_queries(queries)
@@ -311,10 +320,10 @@ def debug_dense_runs(codec: int, index: np.ndarray, terms: np.ndarray, queries: 
     n = C.c_uint64()
     err = C.create_string_buffer(256)
     args = (codec, _ptr(index), index.size, _ptr(terms), len(terms), max_docid, C.cast(arr, C.c_void_p), len(queries), mode, k, _ptr(qtiles))
-    rc = lib().trn_debug_dense_runs(*args, None, 0, C.byref(n), err, 256)
+    rc = fn(*args, None, 0, C.byref(n), err, 256)
     tickets = np.zeros((max(n.value, 1), 3), np.uint32)
     if rc == -6:  # TRN_ERR_CAPACITY: sized, now filled
-        rc = lib().trn_debug_dense_runs(*args, _ptr(tickets), n.value, C.byref(n), err, 256)
+        rc = fn(*args, _ptr(tickets), n.value, C.byref(n), err, 256)
     if rc != 0:
         raise TrinityError(err.value.decode("utf-8", "replace") or f"rc={rc}")
     return qtiles[: len(queries)].copy(), tickets[: n.value].copy()

@@ -13,7 +13,7 @@ static constexpr uint32_t kEmptyTerm = 0xffffffffu;
 static constexpr uint32_t kDenseAlignShift = 17;
 static constexpr uint32_t kDenseNone       = 0xffffffffu;
 
-// all-bitmap flat ANDs (BatchPlan::dense_runs): a ticket {query, first tile} covers the query's tiles from `first` to the end of the
+// run tickets of flat ANDs (BatchPlan::dense_runs, mixed_runs): a ticket {query, first tile} covers the query's tiles from `first` to the end of the
 // 2^kDenseAlignShift-docID run that holds it (or to the end of the query's tiles [tile_lo, tile_lo + ntiles), whichever comes first)
 __host__ __device__ inline uint32_t dense_run_end(uint32_t first, uint32_t tile_lo, uint32_t ntiles, uint32_t exec_shift) {
         const uint32_t e = (first | ((1u << (kDenseAlignShift - exec_shift)) - 1u)) + 1u, qe = tile_lo + ntiles;
@@ -166,7 +166,9 @@ struct ExecParams {
         uint32_t        gen_items; // number of tickets of this launch (items of the queries it runs)
         uint32_t        gen_sel;   // k_exec_docs: 0 = tickets follow DevQuery::gen_base, 1 = gen_base2
         const uint2 *   dense_runs;  // k_exec_docs, step-program launch: tickets [0, dense_items) are the all-bitmap flat ANDs' (query, run) pairs
-        uint32_t        dense_items; // (BatchPlan::dense_runs); the tickets of gen_items follow them
+        uint32_t        dense_items; // (BatchPlan::dense_runs)
+        const uint2 *   mixed_runs;  // ... then tickets [dense_items, dense_items + mixed_items): the flat ANDs with one decoded operand
+        uint32_t        mixed_items; // (BatchPlan::mixed_runs); the tickets of gen_items follow them
         uint32_t        has_phrase; // some plan of the batch holds OP_PHRASE: launch the instantiation that executes it
         uint32_t        nslots; // bitmap slots per worker (CTA for k_exec_tiles, warp for k_exec_docs)
         uint32_t        stage_bytes; // per-warp staging bytes of k_exec_tiles (codec dependent)

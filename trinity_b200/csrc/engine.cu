@@ -105,7 +105,7 @@ struct trn_ctx {
         std::vector<uint32_t> h_dense_off;          // host copy of d_dense_off (trn_debug_dense_bitmap)
         std::vector<DevTerm> h_terms;
         // batch scratch (grow-only)
-        DevBuf d_queries, d_steps, d_dense_runs, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
+        DevBuf d_queries, d_steps, d_dense_runs, d_mixed_runs, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
             d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_a, d_dec_b, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
         PinBuf h_offsets, h_docids, h_scores, h_counts, h_small, h_chunk, h_item_desc;
         DevBuf d_hits, d_hit_base, d_hblk_off, d_hit_term; // LUCENE positions (trn_upload_hits)
@@ -234,6 +234,7 @@ static PlanConfig initial_plan_config() {
         pc.docs_stage_bytes      = exec_docs_stage_bytes();
         pc.cand_smem_bytes[0]    = exec_docs_cand_smem_bytes(false);
         pc.cand_smem_bytes[1]    = exec_docs_cand_smem_bytes(true);
+        pc.mixed_smem_bytes      = exec_docs_mixed_smem_bytes();
         return pc;
 }
 
@@ -306,7 +307,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs,&c->d_small[0], &c->d_small[1], &c->d_item_off,
+        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_a, &c->d_dec_b, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores})
@@ -715,6 +716,11 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 CK(c->d_dense_runs.ensure(size_t(denseItems) * sizeof(uint2)));
                 CK(cudaMemcpyAsync(c->d_dense_runs.p, plan.dense_runs.data(), size_t(denseItems) * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
         }
+        const uint32_t mixedItems = uint32_t(plan.mixed_runs.size());
+        if (mixedItems) {
+                CK(c->d_mixed_runs.ensure(size_t(mixedItems) * sizeof(uint2)));
+                CK(cudaMemcpyAsync(c->d_mixed_runs.p, plan.mixed_runs.data(), size_t(mixedItems) * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+        }
         CK(cudaMemsetAsync(small, 0, smallBytes, c->stream));
 
         ExecParams P;
@@ -727,6 +733,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         P.gen_items    = uint32_t(plan.gen_items);
         P.dense_runs   = denseItems ? c->d_dense_runs.as<uint2>() : nullptr;
         P.dense_items  = denseItems;
+        P.mixed_runs   = mixedItems ? c->d_mixed_runs.as<uint2>() : nullptr;
+        P.mixed_items  = mixedItems;
         P.has_phrase   = plan.any_phrase ? 1u : 0u;
         P.nslots       = plan.nslots;
         P.exec_shift   = execShift;
@@ -752,7 +760,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         uint32_t launches{0};
         if (totalItems) {
                 const bool     warpKernel = !scored;
-                const uint64_t ownItems   = plan.gen_items + denseItems; // tickets of the step-program launch
+                const uint64_t ownItems   = plan.gen_items + denseItems + mixedItems; // tickets of the step-program launch
                 CK(cudaEventRecord(k0, c->stream));
                 if (nflat && plan.flat_items) {
                         // flat scored disjunctions: per-leaf BM25 tables once per batch, then k_score_flat
@@ -804,6 +812,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         P2.gen_sel    = 1;
                         P2.dense_runs  = nullptr;
                         P2.dense_items = 0;
+                        P2.mixed_runs  = nullptr;
+                        P2.mixed_items = 0;
                         P2.ticket     = reinterpret_cast<uint32_t *>(small + 4);
                         const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true);
                         if (perSM <= 0)
@@ -1428,9 +1438,10 @@ extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, 
         return TRN_OK;
 }
 
-extern "C" int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
-                                    const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
-                                    char *err, size_t errcap) {
+// trn_debug_dense_runs / trn_debug_mixed_runs: the run tickets of BatchPlan::dense_runs (mixed == false) or mixed_runs
+static int debug_run_tickets(bool mixed, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                             const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
+                             char *err, size_t errcap) {
         if (!qtiles || !n)
                 return TRN_ERR_ARG;
         BatchPlan plan;
@@ -1440,17 +1451,30 @@ extern "C" int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nb
                 qtiles[2 * q]     = plan.queries[q].tile_lo;
                 qtiles[2 * q + 1] = plan.queries[q].ntiles;
         }
-        *n = plan.dense_runs.size();
+        const std::vector<uint2> &runs = mixed ? plan.mixed_runs : plan.dense_runs;
+        *n                             = runs.size();
         if (cap < *n)
                 return TRN_ERR_CAPACITY;
         for (uint64_t t = 0; t < *n; ++t) {
-                const uint2     e  = plan.dense_runs[t];
+                const uint2     e  = runs[t];
                 const DevQuery &dq = plan.queries[e.x];
                 tickets[3 * t]     = e.x;
                 tickets[3 * t + 1] = e.y;
                 tickets[3 * t + 2] = dense_run_end(e.y, dq.tile_lo, dq.ntiles, plan.exec_shift);
         }
         return TRN_OK;
+}
+
+extern "C" int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                                    const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
+                                    char *err, size_t errcap) {
+        return debug_run_tickets(false, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
+}
+
+extern "C" int trn_debug_mixed_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                                    const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
+                                    char *err, size_t errcap) {
+        return debug_run_tickets(true, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
 }
 
 extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,

@@ -693,6 +693,37 @@ __device__ __forceinline__ void tile_emit(const ExecParams &P, const uint32_t *r
         emit_pad(P, t, seg, W, lane);
 }
 
+// The segments of a run ticket's tiles (dense_run_exec, mixed_run_exec): lane j < nt holds tile j's documents | encoding << 30 (as
+// item_desc) and its segment size.  ONE seg_cursor reservation and one match_counts / word_counts add for the run; every tile gets its
+// record, empty ones included.  Returns the run's base (~0 when the reservation overflowed); myoff: the offset of tile `lane` in it.
+__device__ __forceinline__ unsigned long long run_reserve(const ExecParams &P, uint32_t q, uint32_t item0, uint32_t nt, uint32_t mydesc, uint32_t mysize,
+                                                          uint32_t &myoff, int lane) {
+        const uint32_t mytot = mydesc & 0x3fffffffu;
+        const uint32_t incl = warp_incl_scan(mysize, lane), size = __shfl_sync(0xffffffffu, incl, 31);
+        const uint32_t total = __reduce_add_sync(0xffffffffu, mytot);
+        unsigned long long base = 0;
+        if (lane == 0 && size) {
+                base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(size));
+                atomicAdd(&P.match_counts[q], static_cast<unsigned long long>(total));
+                if (P.item_desc)
+                        atomicAdd(&P.word_counts[q], static_cast<unsigned long long>(size));
+                if (base + size > P.seg_capacity) {
+                        *P.overflow = 1;
+                        base        = ~0ull;
+                }
+        }
+        base  = __shfl_sync(0xffffffffu, base, 0);
+        myoff = incl - mysize;
+        if (uint32_t(lane) < nt) {
+                TileCount t;
+                t.total = mytot;
+                t.size  = mysize;
+                t.enc   = mydesc >> 30;
+                tile_record(P, item0 + uint32_t(lane), t, !mytot ? 0ull : base == ~0ull ? ~0ull : base + myoff);
+        }
+        return base;
+}
+
 // All-bitmap flat AND (BatchPlan::dense_runs): ticket e = {query, first tile} covers the query's tiles of one 2^kDenseAlignShift-docID run,
 // which lies wholly inside every operand's bitmap, so nothing is decoded and no block directory is searched.  The run-major order of the
 // tickets keeps every query that reads a run's bitmap words in flight together: each run of each bitmap comes from HBM about once per batch.
@@ -754,31 +785,10 @@ __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
                         mysize = tc.size;
                 }
         }
-        const uint32_t mytot = mydesc & 0x3fffffffu;
-        const uint32_t incl = warp_incl_scan(mysize, lane), size = __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t total = __reduce_add_sync(0xffffffffu, mytot);
-        unsigned long long base = 0;
-        if (lane == 0 && size) {
-                base = atomicAdd(P.seg_cursor, static_cast<unsigned long long>(size));
-                atomicAdd(&P.match_counts[q], static_cast<unsigned long long>(total));
-                if (compact)
-                        atomicAdd(&P.word_counts[q], static_cast<unsigned long long>(size));
-                if (base + size > P.seg_capacity) {
-                        *P.overflow = 1;
-                        base        = ~0ull;
-                }
-        }
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (uint32_t(lane) < nt) {
-                TileCount t;
-                t.total = mytot;
-                t.size  = mysize;
-                t.enc   = mydesc >> 30;
-                tile_record(P, item0 + uint32_t(lane), t, !mytot ? 0ull : base == ~0ull ? ~0ull : base + (incl - mysize));
-        }
+        uint32_t                 myoff;
+        const unsigned long long base = run_reserve(P, q, item0, nt, mydesc, mysize, myoff, lane);
         if (base == ~0ull)
                 return;
-        const uint32_t myoff = incl - mysize;
         for (uint32_t j = 0; j < nt; ++j) {
                 const uint32_t d = __shfl_sync(0xffffffffu, mydesc, int(j)), off = __shfl_sync(0xffffffffu, myoff, int(j));
                 TileCount      t;
@@ -796,6 +806,205 @@ __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
 
 #include "exec_docs_flat.cuh"
 #include "exec_docs_cand.cuh"
+
+// Flat AND with exactly one operand without a bitmap (BatchPlan::mixed_runs): ticket e = {query, first tile} covers the query's tiles of one
+// 2^kDenseAlignShift-docID run, as in dense_run_exec.  The operand without a bitmap (the lead) is decoded once for the run, 32 blocks at a time
+// (lane = block, google_block_to_array into the candidate array); then lane = candidate of one lead block, so one round's probes of a
+// bitmap fall into a few sectors, and each candidate is tested against every other operand's bitmap and the masked documents, the loads of
+// four rounds in flight together.  The run-major order keeps the queries that probe a bitmap run in flight together (its words come from
+// HBM about once per batch), and the run pays one directory search, one ticket and one reservation instead of one per tile.
+// Pass 1 counts the survivors per tile and finds full 256-docID buckets, so every tile takes tile_encoding's choice; the run's segments
+// take one reservation; pass 2 decodes and probes again (blocks and words now come from L2) and writes every survivor at its rank in its
+// tile: a plain docID, a U16 offset or a U8B offset byte (the count bytes: one add per bucket and round), or, for a tile whose result
+// takes the bitmap form (dense: rare), its bit ORed into the tile's words.  Every byte is what the per-tile path writes.
+static constexpr uint32_t kMixedCntWords = 16; // survivors per tile of the run (a run holds at most 2^(17 - 13) tiles)
+static constexpr uint32_t kMixedSmem     = (kCandWords + kMixedCntWords) * 4u + kGatherBufBytes; // candidates | counters | one gather buffer
+
+__device__ __forceinline__ uint32_t lanemask_lt() {
+        uint32_t m;
+        asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
+        return m;
+}
+
+__device__ void mixed_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, uint32_t *smem, int lane) {
+        const uint32_t  q    = e.x, t0 = e.y;
+        const DevQuery &Q    = P.queries[q];
+        const uint32_t  nt   = dense_run_end(t0, Q.tile_lo, Q.ntiles, P.exec_shift) - t0; // 1 .. 16 tiles
+        const uint32_t  lo0  = t0 << P.exec_shift, span = nt << P.exec_shift;         // the run's docIDs [lo0, lo0 + span) (the end may be 2^32)
+        uint32_t *const tcnt  = smem + kCandWords; // (the candidate array starts at smem)
+        uint8_t *const  stage = reinterpret_cast<uint8_t *>(tcnt + kMixedCntWords);
+        // lane k: operand k; with a bitmap, its word of docID lo0
+        uint32_t nleaf = 0, myTerm = kEmptyTerm, myw = kDenseNone;
+        for (uint32_t si = 0; si < Q.nsteps; ++si) {
+                const DevStep st = P.steps[Q.step_begin + si];
+                if (st.op == OP_LEAF) {
+                        if (uint32_t(lane) == nleaf)
+                                myTerm = st.term;
+                        ++nleaf;
+                }
+        }
+        if (uint32_t(lane) < nleaf) {
+                const uint32_t o = __ldg(P.ix.dense_off + myTerm);
+                if (o != kDenseNone)
+                        myw = o + ((lo0 - ((P.ix.terms[myTerm].first_doc >> kDenseAlignShift) << kDenseAlignShift)) >> 5);
+        }
+        const unsigned dmask    = __ballot_sync(0xffffffffu, myw != kDenseNone);
+        const uint32_t leadTerm = __shfl_sync(0xffffffffu, myTerm, __ffs(int(__ballot_sync(0xffffffffu, uint32_t(lane) < nleaf && myw == kDenseNone))) - 1);
+        uint32_t       bA, bB; // the lead's blocks of the run
+        tile_block_range(P.ix, P.ix.terms[leadTerm], lo0, span, bA, bB);
+
+        // the lead's blocks of the run, 32 at a time; visit(rel, ok) once per round (lane = candidate c = lo0 + rel of one block; ok: c lies
+        // in the run and every operand holds it).  The rounds come in docID order.  (lo0 is a multiple of 2^13: c and rel agree in their
+        // low 13 bits.)
+        auto walk = [&](auto visit) {
+                for (uint32_t g = bA; g <= bB; g += 32u) {
+                        const uint32_t b    = g + uint32_t(lane);
+                        const bool     have = b <= bB;
+                        uint32_t       off = 0, prev = 0, last = 0, n = 0;
+                        if (have) {
+                                const DevTerm  &T  = P.ix.terms[leadTerm];
+                                const uint32_t *bl = P.ix.blk_last + T.dir_begin;
+                                off                = __ldg(P.ix.blk_off + T.dir_begin + b);
+                                last               = __ldg(bl + b);
+                                prev               = b ? __ldg(bl + b - 1u) : 0u;
+                                n                  = (b + 1u == T.nblocks) ? (T.documents - 32u * (T.nblocks - 1u)) : 32u;
+                        }
+                        gather_issue(P.ix.index, off, have, stage, lane);
+                        gather_wait<0>();
+                        if (have)
+                                google_block_to_array(P.ix.index, off, stage, lane, n, prev, last, smem + lane * kCandStride);
+                        __syncwarp();
+                        const uint32_t rounds = min(32u, bB - g + 1u);
+                        for (uint32_t j0 = 0; j0 < rounds; j0 += 4u) {
+                                uint32_t rel[4]; // span: no candidate
+#pragma unroll
+                                for (uint32_t u = 0; u < 4u; ++u) {
+                                        const uint32_t nj = __shfl_sync(0xffffffffu, n, int(j0 + u)); // (0 past the group's last block)
+                                        rel[u]            = uint32_t(lane) < nj ? smem[(j0 + u) * kCandStride + lane] - lo0 : span;
+                                        rel[u]            = rel[u] < span ? rel[u] : span; // (a block may straddle the run's ends)
+                                }
+                                for (unsigned dm = dmask; dm; dm &= dm - 1u) {
+                                        const uint32_t *bm = P.ix.dense + __shfl_sync(0xffffffffu, myw, __ffs(int(dm)) - 1);
+                                        uint32_t        v[4];
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                v[u] = rel[u] < span ? __ldg(bm + (rel[u] >> 5)) : 0u;
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                rel[u] = (v[u] >> (rel[u] & 31u)) & 1u ? rel[u] : span;
+                                }
+                                if (P.ix.masked) {
+                                        const uint32_t *mk = P.ix.masked + (lo0 >> 5);
+                                        uint32_t        v[4];
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                v[u] = rel[u] < span ? __ldg(mk + (rel[u] >> 5)) : 0u;
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                rel[u] = (v[u] >> (rel[u] & 31u)) & 1u ? span : rel[u];
+                                }
+#pragma unroll
+                                for (uint32_t u = 0; u < 4u; ++u)
+                                        visit(rel[u], rel[u] < span);
+                        }
+                        __syncwarp(); // every lane has read the candidates: the next group may overwrite them
+                }
+        };
+
+        // ---- pass 1: survivors per tile; a 256-docID bucket is full when its first and last docID survive 255 survivors apart
+        if (lane < int(kMixedCntWords))
+                tcnt[lane] = 0;
+        __syncwarp();
+        uint32_t seen = 0, fdoc = 1, fidx = 0, fullm = 0; // survivors so far; the latest bucket start among them (docID, rank); tiles with a full bucket
+        walk([&](uint32_t rel, bool ok) {
+                const uint32_t m = __ballot_sync(0xffffffffu, ok);
+                if (!m)
+                        return;
+                const uint32_t lt = lanemask_lt(), c = lo0 + rel;
+                const uint32_t idx = seen + __popc(m & lt);
+                const uint32_t ti  = ok ? rel >> P.exec_shift : 0xffffffffu;
+                const uint32_t grp = __match_any_sync(0xffffffffu, ti);
+                if (ok && !(grp & lt))
+                        atomicAdd(&tcnt[ti], uint32_t(__popc(grp)));
+                const bool full = ok && (c & 255u) == 255u && c - 255u == fdoc && idx - fidx == 255u;
+                fullm |= __reduce_or_sync(0xffffffffu, full ? 1u << ti : 0u);
+                const uint32_t sm = __ballot_sync(0xffffffffu, ok && (c & 255u) == 0u);
+                if (sm) {
+                        const int s = 31 - __clz(int(sm));
+                        fdoc        = __shfl_sync(0xffffffffu, c, s);
+                        fidx        = __shfl_sync(0xffffffffu, idx, s);
+                }
+                seen += __popc(m);
+        });
+        const bool compact = P.item_desc != nullptr;
+        uint32_t   mydesc = 0, mysize = 0; // lane j: tile j's documents | encoding << 30 (as item_desc), and its segment size
+        for (uint32_t j = 0; j < nt; ++j) {
+                const TileCount tc = tile_encoding(lane == 0 ? tcnt[j] : 0u, (fullm >> j) & 1u, compact, W, NW);
+                if (uint32_t(lane) == j) {
+                        mydesc = tc.total | tc.enc << 30;
+                        mysize = tc.size;
+                }
+        }
+        uint32_t                 myoff;
+        const unsigned long long base = run_reserve(P, q, Q.item_base + (t0 - Q.tile_lo), nt, mydesc, mysize, myoff, lane);
+        if (base == ~0ull || !seen)
+                return;
+        const uint32_t mytot = mydesc & 0x3fffffffu, myfirst = warp_incl_scan(mytot, lane) - mytot; // lane j: rank of tile j's first survivor in the run
+        const uint32_t nbk   = W >> 8;
+        bool           anyU8B = false;
+        for (uint32_t j = 0; compact && j < nt; ++j) { // U8B count bytes and bitmap-form words start at zero
+                const uint32_t d = __shfl_sync(0xffffffffu, mydesc, int(j));
+                if ((d & 0x3fffffffu) && (d >> 30) != kEncU16) {
+                        uint32_t      *seg = P.seg_docids + (base + __shfl_sync(0xffffffffu, myoff, int(j)));
+                        const uint32_t nz  = (d >> 30) == kEncU8B ? nbk >> 2 : NW;
+                        for (uint32_t i = lane; i < nz; i += 32)
+                                seg[i] = 0;
+                        anyU8B = anyU8B || (d >> 30) == kEncU8B;
+                }
+        }
+        __syncwarp();
+
+        // ---- pass 2: every survivor at its rank in its tile, or (bitmap form) its bit in the tile's words
+        seen = 0;
+        walk([&](uint32_t rel, bool ok) {
+                const uint32_t m = __ballot_sync(0xffffffffu, ok);
+                if (!m)
+                        return;
+                const uint32_t lt = lanemask_lt();
+                const uint32_t ti = ok ? rel >> P.exec_shift : 0u;
+                const uint32_t d = __shfl_sync(0xffffffffu, mydesc, int(ti)), off = __shfl_sync(0xffffffffu, myoff, int(ti));
+                const uint32_t r   = seen + __popc(m & lt) - __shfl_sync(0xffffffffu, myfirst, int(ti));
+                const uint32_t enc = d >> 30;
+                seen += __popc(m);
+                uint32_t *const seg = P.seg_docids + (base + off);
+                const bool      u8b = ok && compact && enc == kEncU8B;
+                if (ok) {
+                        if (!compact)
+                                seg[r] = lo0 + rel;
+                        else if (enc == kEncU16)
+                                reinterpret_cast<uint16_t *>(seg)[r] = uint16_t(rel & (W - 1u));
+                        else if (u8b)
+                                reinterpret_cast<uint8_t *>(seg)[nbk + r] = uint8_t(rel);
+                        else
+                                atomicOr(seg + ((rel >> 5) & (NW - 1u)), 1u << (rel & 31u));
+                }
+                if (anyU8B) { // the count bytes stay below 256: a tile with a full bucket is not U8B
+                        const uint32_t bk  = u8b ? rel >> 8 : 0xffffffffu;
+                        const uint32_t grp = __match_any_sync(0xffffffffu, bk);
+                        if (u8b && !(grp & lt))
+                                atomicAdd(seg + ((bk & (nbk - 1u)) >> 2), uint32_t(__popc(grp)) << (8u * (bk & 3u)));
+                }
+        });
+        for (uint32_t j = 0; compact && j < nt; ++j) { // the pad bytes of U8B and the pad half-word of U16
+                const uint32_t d = __shfl_sync(0xffffffffu, mydesc, int(j)), off = __shfl_sync(0xffffffffu, myoff, int(j));
+                TileCount      t;
+                t.total = d & 0x3fffffffu;
+                t.enc   = d >> 30;
+                t.size  = 0;
+                if (t.total)
+                        emit_pad(P, t, P.seg_docids + (base + off), W, lane);
+        }
+}
 
 // min 7 CTAs/SM: shared memory allows 7 at the default tile; without the bound ptxas stops at 64 registers and spills
 // TREE: the flat-tree launch (every query of its ticket space is a flat-tree plan) — that instantiation holds nothing but the tree
@@ -833,15 +1042,20 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 if (lane == 0)
                         gitem = atomicAdd(P.ticket, 1u);
                 gitem = __shfl_sync(0xffffffffu, gitem, 0);
-                if (gitem >= P.dense_items + P.gen_items)
+                if (gitem >= P.dense_items + P.mixed_items + P.gen_items)
                         break;
                 if constexpr (!PH && !TREE && !LUC) {
                         if (gitem < P.dense_items) { // all-bitmap flat AND: the query's tiles of one run
                                 dense_run_exec(P, P.dense_runs[gitem], W, NW, lane);
                                 continue;
                         }
+                        if (gitem - P.dense_items < P.mixed_items) { // flat AND with one decoded operand: the query's tiles of one run
+                                __syncwarp();
+                                mixed_run_exec(P, P.mixed_runs[gitem - P.dense_items], W, NW, slots, lane);
+                                continue;
+                        }
                 }
-                gitem -= P.dense_items;
+                gitem -= P.dense_items + P.mixed_items;
                 if (curq == 0xffffffffu || gitem < qgen || gitem - qgen >= Q.ntiles) {
                         uint32_t qlo = 0, qhi = P.nq;
                         while (qhi - qlo > 1) {
@@ -1070,6 +1284,10 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
 
 uint32_t exec_docs_cand_smem_bytes(bool with_membership) {
         return with_membership ? kCandSmemMask : kCandSmem;
+}
+
+uint32_t exec_docs_mixed_smem_bytes() {
+        return kMixedSmem;
 }
 
 uint32_t exec_docs_stage_bytes() {

@@ -10,6 +10,7 @@ int         exec_max_ctas_per_sm(uint32_t tile_shift, uint32_t nslots, int mode,
 cudaError_t launch_exec_tiles(const ExecParams &P, int grid, cudaStream_t stream);
 uint32_t    exec_docs_stage_bytes();
 uint32_t    exec_docs_cand_smem_bytes(bool with_membership); // per-warp shared memory of the candidate-driven path (membership bytes: trees with terms that are not necessary)
+uint32_t    exec_docs_mixed_smem_bytes(); // per-warp shared memory of the mixed flat ANDs' run tickets (the candidate array, one gather buffer, counters)
 size_t      exec_docs_smem_bytes(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes);
 int         exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes, bool tree = false, bool lucene = false);
 cudaError_t launch_exec_docs(const ExecParams &P, int grid, cudaStream_t stream);

@@ -1226,6 +1226,8 @@ PlanConfig trn::plan_config_from_env() {
         }
         if (const char *e = getenv("TRN_DENSE_RUNS"))
                 pc.dense_runs = atoi(e) != 0;
+        if (const char *e = getenv("TRN_MIXED_RUNS"))
+                pc.mixed_runs = atoi(e) != 0;
         return pc;
 }
 
@@ -1562,56 +1564,71 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
         // step program.  One whose operands all have a resident bitmap decodes nothing: it joins the run-major ticket space (dense_runs) —
         // except beside a phrase plan, whose instantiation of k_exec_docs does not carry that path.
         const bool runs = dense_off && cfg.dense_runs && google && !scored && !out.any_phrase;
-        std::vector<uint32_t> group; // the queries of dense_runs
+        // A flat AND with exactly one operand without a bitmap decodes that operand (the lead) once per run and probes the others' bitmaps
+        // per candidate (exec_docs.cuh mixed_run_exec) — when the warp's share of shared memory holds the path's candidate array.
+        const bool mixedRuns = dense_off && cfg.mixed_runs && google && !scored && !out.any_phrase &&
+                               out.nslots * ((1u << execShift) / 8u) + cfg.docs_stage_bytes >= cfg.mixed_smem_bytes;
+        std::vector<uint32_t> group, mixed; // the queries of dense_runs, of mixed_runs
         for (uint32_t q = 0; q < nq; ++q) {
                 auto &dq = out.queries[q];
                 if (dq.route == TRN_ROUTE_FLAT_AND) {
-                        uint32_t nleaf{0};
-                        bool     dense{runs && dq.ntiles};
+                        uint32_t nleaf{0}, ndecoded{0};
+                        bool     known{dq.ntiles != 0};
                         for (uint32_t si = 0; si < dq.nsteps; ++si) {
                                 const DevStep &st = steps[dq.step_begin + si];
                                 if (st.op == OP_LEAF) {
                                         ++nleaf;
-                                        dense = dense && st.term != kEmptyTerm && dense_off[st.term] != kDenseNone;
+                                        known = known && st.term != kEmptyTerm;
+                                        ndecoded += (!dense_off || st.term == kEmptyTerm || dense_off[st.term] == kDenseNone) ? 1u : 0u;
                                 }
                         }
                         if (nleaf > out.nslots)
                                 dq.route = TRN_ROUTE_STEPS;
-                        else if (dense)
+                        else if (runs && known && ndecoded == 0)
                                 group.push_back(q);
+                        else if (mixedRuns && known && ndecoded == 1 && nleaf >= 2 && nleaf <= 32)
+                                mixed.push_back(q);
                 }
         }
-        if (!group.empty()) {
-                // (run, query) pairs, counting-sorted by run (queries ascending within a run).  Every tile of such a query lies inside every
-                // operand's bitmap span (the query's range is the intersection of the operands' ranges), and so does the run that holds it.
-                const uint32_t rs = kDenseAlignShift - execShift;
-                uint32_t       r0{0xffffffffu}, r1{0};
-                for (uint32_t q : group) {
+        // (run, query) pairs, counting-sorted by run (queries ascending within a run).  Every tile of such a query lies inside every
+        // bitmap operand's span (the query's range is the intersection of the operands' ranges), and so does the run that holds it.
+        const uint32_t rs          = kDenseAlignShift - execShift;
+        auto           run_tickets = [&](const std::vector<uint32_t> &qs, std::vector<uint2> &tickets) {
+                if (qs.empty())
+                        return;
+                uint32_t r0{0xffffffffu}, r1{0};
+                for (uint32_t q : qs) {
                         const auto &dq = out.queries[q];
                         r0             = std::min(r0, dq.tile_lo >> rs);
                         r1             = std::max(r1, (dq.tile_lo + dq.ntiles - 1u) >> rs);
                 }
                 std::vector<uint32_t> at(size_t(r1 - r0) + 2, 0);
-                for (uint32_t q : group) {
+                for (uint32_t q : qs) {
                         const auto &dq = out.queries[q];
                         for (uint32_t r = dq.tile_lo >> rs; r <= (dq.tile_lo + dq.ntiles - 1u) >> rs; ++r)
                                 ++at[r - r0 + 1];
                 }
                 for (size_t i = 1; i < at.size(); ++i)
                         at[i] += at[i - 1];
-                out.dense_runs.resize(at.back());
-                for (uint32_t q : group) {
+                tickets.resize(at.back());
+                for (uint32_t q : qs) {
                         const auto &dq = out.queries[q];
                         for (uint32_t r = dq.tile_lo >> rs; r <= (dq.tile_lo + dq.ntiles - 1u) >> rs; ++r)
-                                out.dense_runs[at[r - r0]++] = uint2{q, std::max(dq.tile_lo, r << rs)};
+                                tickets[at[r - r0]++] = uint2{q, std::max(dq.tile_lo, r << rs)};
                 }
+        };
+        run_tickets(group, out.dense_runs);
+        run_tickets(mixed, out.mixed_runs);
+        if (!group.empty() || !mixed.empty()) {
                 // the step-program launch's own tickets without them (the items keep their item_base)
                 out.gen_items = 0;
-                for (uint32_t q = 0, g = 0; q < nq; ++q) {
+                for (uint32_t q = 0, g = 0, m = 0; q < nq; ++q) {
                         auto &dq    = out.queries[q];
                         dq.gen_base = uint32_t(out.gen_items);
                         if (g < group.size() && group[g] == q)
                                 ++g;
+                        else if (m < mixed.size() && mixed[m] == q)
+                                ++m;
                         else if (dq.route != TRN_ROUTE_FLAT_TREE)
                                 out.gen_items += dq.ntiles;
                 }

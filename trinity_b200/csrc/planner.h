@@ -34,10 +34,12 @@ struct PlanConfig {
         bool     dense_bitmaps{true}; // TRN_DENSE_BITMAPS=0: no resident docID bitmaps of dense terms (select_dense_terms)
         double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
         bool     dense_runs{true};    // TRN_DENSE_RUNS=0: all-bitmap flat ANDs take (query, tile) tickets like the other flat ANDs (BatchPlan::dense_runs)
+        bool     mixed_runs{true};    // TRN_MIXED_RUNS=0: flat ANDs with one decoded operand take (query, tile) tickets (BatchPlan::mixed_runs)
         // kernel limits (kernels.h)
         uint32_t score_flat_max_leaves{0};          // leaves of a k_score_flat query
         uint32_t docs_stage_bytes{0};               // per-warp staging bytes of k_exec_docs
         uint32_t cand_smem_bytes[2]{0, 0};          // per-warp shared memory of the candidate-driven path, [with membership bits]
+        uint32_t mixed_smem_bytes{0};               // per-warp shared memory of the mixed flat ANDs' run tickets
 };
 
 // the knobs of PlanConfig from the environment (the index fields and the kernel limits keep their defaults)
@@ -57,6 +59,9 @@ struct BatchPlan {
         // flat ANDs whose operands all have a resident bitmap (DocumentsOnly, no phrase plan in the batch): one ticket per (query, 2^17-docID
         // run) pair, {query, first tile} (dense_run_end: device_types.h), ordered run-major, in front of the step-program launch's gen_items
         std::vector<uint2>     dense_runs;
+        // flat ANDs with exactly one operand without a resident bitmap (the lead, decoded; the others probed in their bitmaps), same
+        // conditions: the same {query, first tile} tickets over the same runs, run-major, between dense_runs and gen_items
+        std::vector<uint2>     mixed_runs;
         uint64_t               seg_cap{0};     // upper bound of the batch's matches (result segments)
         uint64_t               cand_total{0};  // top-k candidate entries
         uint64_t               postings{0}, bytes{0};
