@@ -176,7 +176,8 @@ int trn_query_truth_table(const trn_qnode *nodes, uint32_t nnodes, uint32_t root
  * `term` where slot src has the document), 4 COUNT_ADD / 5 COUNT_GE (MatchSome counters); mode: 0 SET 1 OR 2 AND 3 ANDNOT 4 NONE;
  * flags: 1 = the leaf scores where it matches, 2 = stop when dst becomes empty.  Needs no GPU.
  * scored: 0 = DocumentsOnly program, 1 = scored program, 2 = DocumentsOnly program in its flat-tree form (every leaf owns a bitmap announced
- * by a leading [LEAF, mode NONE, dst = leaf slot] marker and filled by one flat pass over the tile; slot operations only afterwards). */
+ * by a leading [LEAF, mode NONE, dst = leaf slot] marker and filled by one flat pass over the tile; slot operations only afterwards).
+ * Phrases compile on a GOOGLE index (7 PHRASE with mode = k, then ceil(k / 4) 8 ARG steps of term ids), as trn_debug_plan plans them. */
 typedef struct trn_debug_step {
         uint8_t  op, mode, dst, src, flags, pad[3];
         uint32_t term;

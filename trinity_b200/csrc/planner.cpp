@@ -1151,6 +1151,7 @@ extern "C" int trn_debug_compile(int codec, const uint8_t *index, uint64_t nbyte
         const std::vector<DevTerm> ht = dev_terms(dir, terms, nterms);
         std::vector<DevStep> steps;
         Compiler             cc(nodes, nnodes, ht, scored == 1, root, steps);
+        cc.allow_phrase         = codec == TRN_CODEC_GOOGLE; // as trn_debug_plan: the hits are inline (LUCENE would need its hits.data)
         int                  rs = cc.run();
         if (rs < 0)
                 return seterr(cc.err, cc.unsupported ? TRN_ERR_UNSUPPORTED : TRN_ERR_ARG);
@@ -1511,14 +1512,14 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                         dq.route = flatScored ? TRN_ROUTE_SCORE_FLAT : TRN_ROUTE_EXEC_TILES;
                 else
                         dq.route = candidate ? TRN_ROUTE_CANDIDATE : treeFlat ? TRN_ROUTE_FLAT_TREE : google ? flatList : TRN_ROUTE_STEPS;
+                const uint32_t qshift = flatScored ? cfg.scored_shift : (treeFlat ? cfg.tree_shift : execShift); // per-path tile
                 if (candidate) {
                 } else if (r.empty()) {
                         dq.tile_lo = 0;
                         dq.ntiles  = 0;
                 } else {
-                        const uint32_t qshift = flatScored ? cfg.scored_shift : (treeFlat ? cfg.tree_shift : execShift); // per-path tile
-                        dq.tile_lo            = r.lo >> qshift;
-                        dq.ntiles             = (r.hi >> qshift) - dq.tile_lo + 1;
+                        dq.tile_lo = r.lo >> qshift;
+                        dq.ntiles  = (r.hi >> qshift) - dq.tile_lo + 1;
                 }
                 dq.item_base = uint32_t(out.items);
                 dq.gen_base  = uint32_t(out.gen_items);
@@ -1531,7 +1532,13 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                 if (out.items >= (1ull << 32))
                         return fail(err, TRN_ERR_CAPACITY, "batch has more than 2^32 (query, tile) work items; split it");
                 const uint64_t rangeDocs = r.empty() ? 0 : uint64_t(r.hi) - r.lo + 1;
-                out.seg_cap += std::min(cc.bound(cc.root), rangeDocs);
+                uint64_t       segWords  = std::min(cc.bound(cc.root), rangeDocs);
+                // compact results (planned as DocumentsOnly): a tile wider than 2^16 docIDs has no offset form (exec_docs.cuh
+                // tile_encoding), so every tile that holds a match takes its bitmap, 2^qshift / 32 words however few documents it holds.
+                // (Sized by the docID count alone, a batch of sparse phrase queries at TRN_DOCS_SHIFT=17 overflowed its segment buffer.)
+                if (!candidate && qshift > 16u)
+                        segWords = std::max(segWords, std::min<uint64_t>(segWords, dq.ntiles) << (qshift - 5u));
+                out.seg_cap += segWords;
                 dq.cand_base = uint32_t(out.cand_total);
                 dq.cand_cap  = uint32_t(std::min<uint64_t>(uint64_t(dq.ntiles) * k, 0xffffffffull));
                 if (flatScored) {
