@@ -582,6 +582,64 @@ int trn_segment_write(const char *dir, int codec, const uint8_t *index, uint64_t
                       const char *const *names, uint32_t nterms, uint64_t sum_term_hits, uint32_t total_terms, uint64_t sum_terms_docs, uint32_t docs_cnt,
                       const uint32_t *updated_docids, uint64_t nupdated, char *err, size_t errcap);
 
+/* ------------------------------------------------------------------------------------------------ merge
+ * == MergeCandidatesCollection commit() + merge() (merge.cpp:6-35, 40-416) into a fresh IndexSession of out_codec: N index sources
+ * (generations) fold into one segment.  Candidates run newest generation first; candidate i's masked documents are the union of the
+ * updated_docids of every NEWER candidate.  Output terms come in terms_cmp order (bytewise, a prefix first); per term:
+ *   skip      one holder with 0 documents;
+ *   append    one holder of out_codec with an empty registry, disable_optimizations == 0: its chunk copied (LUCENE: with its positions
+ *             chunk, the header's hitsDataOffset rewritten);
+ *   re-encode every other case: of every docID, the newest holder's posting is written unless that holder's registry masks it; older
+ *             holders of the docID are never written.  A re-encoded term left without postings still writes its header (GOOGLE 2 bytes,
+ *             LUCENE 14) and is not an output term.
+ * Per source: names in terms_cmp order (strictly ascending, 1..64 bytes), terms[i] <-> names[i], LUCENE sources with their hits.data.
+ * All pointers are HOST pointers.  The re-encode path runs on the device: decode with hits, keep / rank, scatter, the device encoders,
+ * one assembly copy.  Refusals, never a wrong answer, each naming the source (and term): TRN_ERR_ARG more than 128 sources, two equal
+ * generations, a bad name or order, a tuple outside its source's bytes, a LUCENE source without hits.data, a malformed chunk;
+ * TRN_ERR_UNSUPPORTED a hit with a payload, or at a position outside 1..16383, of a posting that is written re-encoded (appended chunks
+ * keep their payloads; postings not written are never read); TRN_ERR_CAPACITY an output of 4 GiB or more, or
+ * working memory that cannot be allocated.  n = 0: an empty result.  A refused call leaves the context as it was. */
+#define TRN_MERGE_MAX_SOURCES 128
+typedef struct trn_merge_source {
+        int                codec;
+        uint64_t           generation;
+        const uint8_t *    index;
+        uint64_t           index_bytes;
+        const uint8_t *    hits; /* LUCENE hits.data */
+        uint64_t           hits_bytes;
+        const trn_term *   terms;
+        const char *const *names;
+        uint32_t           nterms;
+        const uint32_t *   updated_docids; /* replaced and erased documents of this generation, any order */
+        uint64_t           nupdated;
+} trn_merge_source;
+typedef struct trn_merged { /* owned by the ctx, valid until the next trn_merge_sources */
+        const uint8_t * index;
+        uint64_t        index_bytes;
+        const uint8_t * hits; /* LUCENE hits.data */
+        uint64_t        hits_bytes;
+        const trn_term *terms;       /* output terms in output (terms_cmp) order */
+        const uint32_t *term_source; /* the source (index into src[]) and that source's term index whose name term i carries */
+        const uint32_t *term_index;
+        uint32_t        nterms;
+        uint32_t        total_terms, docs_cnt; /* docs_cnt: distinct docIDs holding an output posting (merge() leaves it to the caller) */
+        uint64_t        sum_terms_docs, sum_term_hits; /* only the postings of the two decode loops count (merge.cpp:224-225, 363-364) */
+        uint32_t        appended, reencoded, orphaned;
+        uint64_t        postings_read, postings_written;
+        float           decode_ms, merge_ms, encode_ms, assemble_ms; /* CUDA events of the phases' kernels */
+        float           total_ms;                                    /* host time of the whole call, copies included */
+} trn_merged;
+int trn_merge_sources(trn_ctx *, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out);
+/* Host-only view of the merge planner (csrc/mergeplan.h; no GPU).  Arrays sized by the caller: order[n] = source of candidate i (newest
+ * first); per output term k (at most Σ nterms): route[k] (0 append, 1 re-encode), stats[k] (1: its postings count toward sum_terms_docs /
+ * sum_term_hits), parts [part_off[k], part_off[k + 1]) (nout + 1 offsets) of part_cand / part_term (candidate, term of that candidate's
+ * source; newest first); the registries as the sorted distinct updated docIDs upd_docid[nupd] (at most Σ nupdated) with upd_first[i] =
+ * the newest candidate that updates it: candidate j masks d iff upd_first(d) < j.  countdown_phase: the GOOGLE skiplist phase the
+ * re-encoded terms start from.  The refusals of trn_merge_sources that need no postings. */
+int trn_debug_merge_plan(int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, uint32_t *order, uint8_t *route,
+                         uint8_t *stats, uint32_t *part_off, uint32_t *part_cand, uint32_t *part_term, uint32_t *nout, uint64_t *nparts, uint32_t *upd_docid,
+                         uint32_t *upd_first, uint64_t *nupd, uint32_t *countdown_phase, char *err, size_t errcap);
+
 #ifdef __cplusplus
 }
 #endif

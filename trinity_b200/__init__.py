@@ -14,7 +14,7 @@ from typing import Iterable, List, Optional, Sequence
 import numpy as np
 
 from ._ffi import (HIT_DTYPE, QNODE_DTYPE, TERM_DTYPE, TrnIndexInfo, TrnIntersections, TrnIsectReq, TrnMatches, TrnPercolation, TrnPercolatorInfo, TrnQuery,
-                   TrnIndexed, TrnResult, TrnTerm, TrnTimings, lib)
+                   TrnIndexed, TrnMerged, TrnMergeSource, TrnResult, TrnTerm, TrnTimings, lib)
 
 CODEC_GOOGLE, CODEC_LUCENE = 0, 1
 MODE_DOCS_ONLY, MODE_SCORED_ALL, MODE_SCORED_TOPK = 0, 1, 2  # == ExecFlags::DocumentsOnly / AccumulatedScoreScheme (+ fused top-k sink)
@@ -797,6 +797,16 @@ class GpuIndexSource:
                                              _ptr(pos) if pos is not None and len(pos) else None, len(d), nterms, C.byref(r)))
         return IndexedSegment(codec, r, d)
 
+    def merge_sources(self, out_codec: int, sources: Sequence["MergeSource"], disable_optimizations: bool = False) -> "MergedSegment":
+        """== MergeCandidatesCollection commit() + merge() into a fresh IndexSession of out_codec (trn_merge_sources): the sources fold
+        newest generation first, each masked by the updated documents of the newer ones; the re-encoded terms run on the device"""
+        keep, arr = _merge_sources_c(sources)
+        r = TrnMerged()
+        self._ck(self._L.trn_merge_sources(self._h, out_codec, C.cast(arr, C.c_void_p) if len(sources) else None, len(sources),
+                                           int(bool(disable_optimizations)), C.byref(r)))
+        del keep
+        return MergedSegment(out_codec, r, sources)
+
     def index_tokens(self, codec: int, docids, token_lists: Sequence[Sequence[str]], tdict: "TermDictionary") -> "IndexedSegment":
         """index_documents() with the tokens named: each resolved through the dictionary, whose size is nterms (an unknown name is refused)"""
         return self.index_documents(codec, docids, [np.array([tdict.term_id(t) for t in toks], np.uint32) for toks in token_lists], len(tdict))
@@ -1024,3 +1034,119 @@ class IndexedSegment:
         if self.codec == CODEC_LUCENE:
             gpu.upload_hits(self.index, self.hits)
         return keep if names is None else TermDictionary([names[int(t)] for t in keep])
+
+
+@dataclass
+class MergeSource:
+    """one index source of a merge: its generation, index (and LUCENE hits.data) bytes, term tuples with their names in terms_cmp order
+    (the order Segment exposes), and the docIDs it replaced or erased in older sources"""
+    codec: int
+    generation: int
+    index: np.ndarray
+    terms: np.ndarray
+    names: Sequence[str]
+    hits: Optional[np.ndarray] = None
+    updated_docids: Optional[np.ndarray] = None
+
+    @staticmethod
+    def of_segment(seg: "Segment", path: str, generation: int) -> "MergeSource":
+        hp = os.path.join(str(path), "hits.data")
+        hits = np.fromfile(hp, np.uint8) if seg.codec == CODEC_LUCENE and os.path.exists(hp) else None
+        if seg.codec == CODEC_LUCENE and hits is None:
+            hits = np.zeros(0, np.uint8)
+        return MergeSource(seg.codec, generation, seg.index, seg.terms, seg.names, hits, seg.masked_documents)
+
+
+def _merge_sources_c(sources: Sequence[MergeSource]):
+    """the trn_merge_source array and everything it points into (kept alive by the caller)"""
+    keep = []
+    arr = (TrnMergeSource * max(1, len(sources)))()
+    for i, m in enumerate(sources):
+        idx = np.ascontiguousarray(m.index, np.uint8)
+        terms = np.ascontiguousarray(m.terms, TERM_DTYPE)
+        if len(m.names) != len(terms):
+            raise TrinityError(f"merge source {i}: one name per term")
+        enc = [n.encode("utf-8", "surrogateescape") if isinstance(n, str) else bytes(n) for n in m.names]
+        names = (C.c_char_p * max(1, len(enc)))(*enc)
+        hits = None if m.hits is None else np.ascontiguousarray(m.hits, np.uint8)
+        upd = _u32(np.zeros(0, np.uint32) if m.updated_docids is None else m.updated_docids)
+        # a non-null pointer for an empty LUCENE hits.data: it is present, only empty
+        hbuf = hits if hits is not None and hits.size else (np.zeros(1, np.uint8) if hits is not None else None)
+        keep += [idx, terms, enc, names, hbuf, upd]
+        arr[i] = TrnMergeSource(int(m.codec), int(m.generation), _ptr(idx) if idx.size else None, idx.size, _ptr(hbuf), 0 if hits is None else hits.size,
+                                _ptr(terms) if len(terms) else None, C.cast(names, C.c_void_p) if len(enc) else None, len(terms),
+                                _ptr(upd) if upd.size else None, upd.size)
+    keep.append(arr)
+    return keep, arr
+
+
+def debug_merge_plan(out_codec: int, sources: Sequence[MergeSource], disable_optimizations: bool = False) -> dict:
+    """the host planner of merge_sources (trn_debug_merge_plan; no GPU): candidate order, output terms with route / statistics flag /
+    participants (candidate, term), the registries as (docID, newest candidate updating it), the GOOGLE countdown phase"""
+    keep, arr = _merge_sources_c(sources)
+    n = len(sources)
+    T = sum(len(m.terms) for m in sources)
+    U = sum(0 if m.updated_docids is None else len(m.updated_docids) for m in sources)
+    order = np.zeros(max(1, n), np.uint32)
+    route, stats = np.zeros(max(1, T), np.uint8), np.zeros(max(1, T), np.uint8)
+    part_off, pc, pt = np.zeros(T + 1, np.uint32), np.zeros(max(1, T), np.uint32), np.zeros(max(1, T), np.uint32)
+    ud, uf = np.zeros(max(1, U), np.uint32), np.zeros(max(1, U), np.uint32)
+    nout, nparts, nupd, phase = C.c_uint32(), C.c_uint64(), C.c_uint64(), C.c_uint32()
+    err = C.create_string_buffer(512)
+    rc = lib().trn_debug_merge_plan(out_codec, C.cast(arr, C.c_void_p) if n else None, n, int(bool(disable_optimizations)), _ptr(order), _ptr(route),
+                                    _ptr(stats), _ptr(part_off), _ptr(pc), _ptr(pt), C.byref(nout), C.byref(nparts), _ptr(ud), _ptr(uf), C.byref(nupd),
+                                    C.byref(phase), err, 512)
+    del keep
+    if rc != 0:
+        raise TrinityError(f"rc={rc}: {err.value.decode('utf-8', 'replace')}")
+    k, q, u = nout.value, nparts.value, nupd.value
+    return {"order": order[:n].tolist(), "route": route[:k].tolist(), "stats": stats[:k].tolist(), "part_off": part_off[:k + 1].tolist(),
+            "parts": list(zip(pc[:q].tolist(), pt[:q].tolist())), "upd_docid": ud[:u].tolist(), "upd_first": uf[:u].tolist(),
+            "countdown_phase": phase.value}
+
+
+class MergedSegment:
+    """GpuIndexSource.merge_sources: the merged index (and LUCENE hits.data), the output terms with their names, the field statistics
+    (docsCnt: the distinct documents holding an output posting) and the phase times of the call"""
+
+    def __init__(self, codec: int, r, sources: Sequence[MergeSource]):
+        self.codec = codec
+        self.index = np.ctypeslib.as_array(r.index, shape=(int(r.index_bytes),)).copy() if r.index_bytes else np.zeros(0, np.uint8)
+        self.hits = np.ctypeslib.as_array(r.hits, shape=(int(r.hits_bytes),)).copy() if r.hits_bytes else np.zeros(0, np.uint8)
+        n = int(r.nterms)
+        if n:
+            self.terms = np.ctypeslib.as_array(C.cast(r.terms, C.POINTER(C.c_uint8)), shape=(n * 12,)).view(TERM_DTYPE).copy()
+            src, idx = np.ctypeslib.as_array(r.term_source, shape=(n,)), np.ctypeslib.as_array(r.term_index, shape=(n,))
+            self.names = [sources[int(s)].names[int(t)] for s, t in zip(src, idx)]
+        else:
+            self.terms, self.names = np.zeros(0, TERM_DTYPE), []
+        self.field_statistics = {"sumTermHits": int(r.sum_term_hits), "totalTerms": int(r.total_terms), "sumTermsDocs": int(r.sum_terms_docs),
+                                 "docsCnt": int(r.docs_cnt)}
+        self.counts = {"appended": int(r.appended), "reencoded": int(r.reencoded), "orphaned": int(r.orphaned), "postings_read": int(r.postings_read),
+                       "postings_written": int(r.postings_written)}
+        self.timings = {"decode_ms": float(r.decode_ms), "merge_ms": float(r.merge_ms), "encode_ms": float(r.encode_ms),
+                        "assemble_ms": float(r.assemble_ms), "total_ms": float(r.total_ms)}
+
+    def write(self, path: str):
+        """the merged segment directory (its last component the generation); no updated_documents.ids: it masks nothing itself"""
+        segment_write(path, self.codec, self.index, self.hits, self.terms, self.names, self.field_statistics)
+
+
+RETAIN_ALL, RETAIN_DOCUMENT_IDS_UPDATES, RETAIN_DELETE = 0, 1, 2
+
+
+def consider_tracked_sources(candidate_gens: Iterable[int], tracked_gens: Iterable[int]):
+    """== MergeCandidatesCollection::consider_tracked_sources (merge.cpp:418-447): for every tracked generation, ascending, whether the
+    application keeps its directory (RETAIN_ALL: not merged), keeps only its updated documents (RETAIN_DOCUMENT_IDS_UPDATES: merged, but an
+    older tracked source that was not merged still needs them) or deletes it (RETAIN_DELETE)"""
+    cands = set(int(g) for g in candidate_gens)
+    out, last_not_candidate = [], None
+    for i, g in enumerate(sorted(int(g) for g in tracked_gens)):
+        if g not in cands:
+            last_not_candidate = i
+            out.append((g, RETAIN_ALL))
+        elif last_not_candidate is not None:
+            out.append((g, RETAIN_DOCUMENT_IDS_UPDATES))
+        else:
+            out.append((g, RETAIN_DELETE))
+    return out

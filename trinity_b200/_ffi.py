@@ -24,7 +24,7 @@ EXPORTS = [
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
-    "trn_index_documents", "trn_segment_write",
+    "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_debug_merge_plan",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -91,6 +91,21 @@ class TrnIndexed(C.Structure):
                 ("terms", C.c_void_p), ("nterms", C.c_uint32), ("docs_cnt", C.c_uint32), ("total_terms", C.c_uint32),
                 ("sum_terms_docs", C.c_uint64), ("sum_term_hits", C.c_uint64), ("max_docid", C.c_uint32), ("sort_passes", C.c_uint32),
                 ("sort_ms", C.c_float), ("postings_ms", C.c_float), ("encode_ms", C.c_float), ("total_ms", C.c_float)]
+
+
+class TrnMergeSource(C.Structure):
+    _fields_ = [("codec", C.c_int), ("generation", C.c_uint64), ("index", C.c_void_p), ("index_bytes", C.c_uint64), ("hits", C.c_void_p),
+                ("hits_bytes", C.c_uint64), ("terms", C.c_void_p), ("names", C.c_void_p), ("nterms", C.c_uint32), ("updated_docids", C.c_void_p),
+                ("nupdated", C.c_uint64)]
+
+
+class TrnMerged(C.Structure):
+    _fields_ = [("index", C.POINTER(C.c_uint8)), ("index_bytes", C.c_uint64), ("hits", C.POINTER(C.c_uint8)), ("hits_bytes", C.c_uint64),
+                ("terms", C.c_void_p), ("term_source", C.POINTER(C.c_uint32)), ("term_index", C.POINTER(C.c_uint32)), ("nterms", C.c_uint32),
+                ("total_terms", C.c_uint32), ("docs_cnt", C.c_uint32), ("sum_terms_docs", C.c_uint64), ("sum_term_hits", C.c_uint64),
+                ("appended", C.c_uint32), ("reencoded", C.c_uint32), ("orphaned", C.c_uint32), ("postings_read", C.c_uint64),
+                ("postings_written", C.c_uint64), ("decode_ms", C.c_float), ("merge_ms", C.c_float), ("encode_ms", C.c_float),
+                ("assemble_ms", C.c_float), ("total_ms", C.c_float)]
 
 
 CONSIDER_FN =C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32)  # trn_consider_fn
@@ -197,5 +212,7 @@ def lib() -> C.CDLL:
     sig("trn_debug_percolator_plan", i32, vp, u32, u32, vp, vp, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     sig("trn_index_documents", i32, vp, i32, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
     sig("trn_segment_write", i32, C.c_char_p, i32, vp, u64, vp, u64, vp, vp, u32, u64, u32, u64, u32, vp, u64, C.c_char_p, C.c_size_t)
+    sig("trn_merge_sources", i32, vp, i32, vp, u32, i32, P(TrnMerged))
+    sig("trn_debug_merge_plan", i32, i32, vp, u32, i32, vp, vp, vp, vp, vp, vp, P(u32), P(u64), vp, vp, P(u64), P(u32), C.c_char_p, C.c_size_t)
     _lib = L
     return L

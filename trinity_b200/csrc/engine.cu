@@ -10,6 +10,7 @@
 #include "chunkplan.h"
 #include "isectplan.h"
 #include "percplan.h"
+#include "mergeplan.h"
 #include "kernels.h"
 #include "planner.h"
 #include <algorithm>
@@ -205,6 +206,18 @@ struct trn_ctx {
                                         cudaEventDestroy(e);
                 }
         } ix;
+        // merge (trn_merge_sources): the last result
+        struct MergeBufs {
+                std::vector<uint8_t>  index, hits;
+                std::vector<trn_term> terms;
+                std::vector<uint32_t> term_source, term_index;
+                cudaEvent_t           ev[8]{};
+                void release() {
+                        for (cudaEvent_t e : ev)
+                                if (e)
+                                        cudaEventDestroy(e);
+                }
+        } mg;
 };
 
 #define CK(call)                                                                                                                                               \
@@ -327,6 +340,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         c->it.release();
         c->pq.release();
         c->ix.release();
+        c->mg.release();
         if (c->copy_stream)
                 cudaStreamDestroy(c->copy_stream);
         delete c;
@@ -1723,7 +1737,8 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
 // The encode itself over device-resident postings; index and hits.data stay in d_iout / d_hout.  toff[t] = offset of term t's chunk
 // (nterms + 1), *index_bytes / *hits_bytes the totals (set before the capacity refusals).  have_index / have_hits: the caller has buffers.
 static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_index, uint64_t index_cap, uint64_t *index_bytes, bool have_hits, uint64_t hits_cap,
-                                uint64_t *hits_bytes, DevBuf &d_iout, DevBuf &d_hout, std::vector<uint64_t> &toff, float *device_ms) {
+                                uint64_t *hits_bytes, DevBuf &d_iout, DevBuf &d_hout, std::vector<uint64_t> &toff, float *device_ms,
+                                std::vector<uint64_t> *hits_toff = nullptr) {
         const uint64_t *const term_begin = P.h_term_begin;
         const uint32_t        nterms     = P.nterms;
         const uint64_t        nposts     = term_begin[nterms];
@@ -1838,6 +1853,8 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         ms += a;
         if (device_ms)
                 *device_ms = ms;
+        if (hits_toff)
+                hits_toff->swap(hto);
         c->have_kernel_events = false;
         return TRN_OK;
 }
@@ -2777,5 +2794,450 @@ extern "C" int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, 
         }
         cover_off[nq] = uint32_t(P.covers.size());
         std::copy(P.covers.begin(), P.covers.end(), cover_terms);
+        return TRN_OK;
+}
+
+// =================================================================================================== merge
+// == MergeCandidatesCollection::commit() + merge() (merge.cpp): the plan on the host (mergeplan.h), the postings on the device (merge.cuh),
+// the re-encoded terms through the device encoders in one call, the output assembled in output term order by one copy kernel.
+#define CKMG(call)                                                                                                                                             \
+        do {                                                                                                                                                   \
+                cudaError_t e__ = (call);                                                                                                                      \
+                if (e__ == cudaErrorMemoryAllocation) {                                                                                                        \
+                        cudaGetLastError();                                                                                                                    \
+                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: working memory cannot be allocated on the device; merge fewer sources");        \
+                }                                                                                                                                              \
+                if (e__ != cudaSuccess) {                                                                                                                      \
+                        c->err = std::string(#call) + ": " + cudaGetErrorString(e__);                                                                          \
+                        return TRN_ERR_CUDA;                                                                                                                   \
+                }                                                                                                                                              \
+        } while (0)
+
+extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out) {
+        if (!c)
+                return TRN_ERR_ARG;
+        const double t_begin = now_ms();
+        if (!out)
+                return fail(c, TRN_ERR_ARG, "trn_merge_sources: bad arguments");
+        MergePlan   P;
+        std::string perr;
+        if (const int r = plan_merge(out_codec, src, n, disable_optimizations != 0, P, perr))
+                return fail(c, r, perr);
+        const uint32_t nout = uint32_t(P.out.size() - 1);
+        const auto     who  = [&](uint32_t s) { return "trn_merge_sources: source " + std::to_string(s) + " (generation " + std::to_string(src[s].generation) + ")"; };
+        const auto     name = [&](uint32_t s, uint32_t t) { return who(s) + ", term [" + std::string(src[s].names[t]) + "]"; };
+        CK(cudaSetDevice(c->device));
+        auto &X = c->mg;
+        for (auto &e : X.ev)
+                if (!e)
+                        CK(cudaEventCreate(&e));
+        // ---- the sources' directories (host, as trn_upload_index / trn_upload_hits build them)
+        std::vector<uint8_t>              used(n, 0);
+        std::vector<BlockDirectory>       dirs(n);
+        std::vector<HitsDirectory>        hdirs(n);
+        std::vector<std::vector<DevTerm>> dts(n);
+        for (const auto &p : P.parts)
+                used[P.order[p.cand]] = 1;
+        const int threads = int(std::max(1u, std::min(64u, std::thread::hardware_concurrency())));
+        for (uint32_t s = 0; s < n; ++s) {
+                if (!used[s])
+                        continue;
+                const auto &S = src[s];
+                if (S.index_bytes >= (1ull << 32) || S.hits_bytes >= (1ull << 32))
+                        return fail(c, TRN_ERR_ARG, who(s) + ": an index or hits.data of 4 GiB or more is not one source (range32_t offsets)");
+                try {
+                        build_directory(S.codec, S.index, S.index_bytes, S.terms, S.nterms, threads, dirs[s]);
+                        dts[s] = dev_terms(dirs[s], S.terms, S.nterms);
+                        if (S.codec == TRN_CODEC_LUCENE) {
+                                std::vector<term_index_ctx> tc(S.nterms);
+                                for (uint32_t i = 0; i < S.nterms; ++i)
+                                        tc[i] = term_index_ctx{S.terms[i].documents, S.terms[i].chunk_off, S.terms[i].chunk_len};
+                                build_hits_directory(S.index, S.index_bytes, S.hits, S.hits_bytes, tc.data(), S.nterms, dirs[s], threads, hdirs[s]);
+                        }
+                } catch (const std::bad_alloc &) {
+                        return fail(c, TRN_ERR_CAPACITY, who(s) + ": out of host memory while building its directories");
+                } catch (const std::exception &e) {
+                        return fail(c, TRN_ERR_ARG, who(s) + ": " + e.what());
+                }
+                if (S.codec == TRN_CODEC_GOOGLE && dirs[s].block_docs && dirs[s].block_docs != Codecs::Google::N)
+                        return fail(c, TRN_ERR_ARG, who(s) + ": GOOGLE blocks of " + std::to_string(dirs[s].block_docs) + " documents (the format's are 32)");
+        }
+        // ---- lists: every participant of every output term, term after term, newest first
+        std::vector<MergeList>          lists;
+        std::vector<unsigned long long> list_blk{0}, list_post{0}, re_first; // re_first: the first posting of each re-encoded term
+        uint32_t                        maxdoc{0};
+        for (uint32_t k = 0; k < nout; ++k) {
+                const uint32_t b = P.out[k].part_begin, e = P.out[k + 1].part_begin;
+                if (P.out[k].route == MERGE_REENCODE)
+                        re_first.push_back(list_post.back());
+                for (uint32_t q = b; q < e; ++q) {
+                        const uint32_t s = P.order[P.parts[q].cand], t = P.parts[q].term;
+                        MergeList      L{};
+                        L.t        = dts[s][t];
+                        L.view     = s;
+                        L.term     = t;
+                        L.cand     = P.parts[q].cand;
+                        L.rank     = q - b;
+                        L.nparts   = e - b;
+                        L.reencode = P.out[k].route == MERGE_REENCODE;
+                        lists.push_back(L);
+                        list_blk.push_back(list_blk.back() + L.t.nblocks);
+                        list_post.push_back(list_post.back() + L.t.documents);
+                        maxdoc = std::max(maxdoc, L.t.last_doc);
+                }
+        }
+        const uint32_t nlists = uint32_t(lists.size());
+        const uint64_t nposts = list_post.back(), nblocks = list_blk.back();
+        const uint32_t nre    = uint32_t(re_first.size());
+        re_first.push_back(nposts);
+        // ---- upload: every used source's bytes and directories, one view per source
+        DevBuf   d_idx, d_hits, d_bl, d_bo, d_tf, d_hb, d_hbo, d_ht, d_views, d_lists, d_lblk, d_lpost, d_ud, d_uf, d_doc, d_fr, d_hc, d_hoff, d_pos, d_keep, d_ks,
+            d_bm, d_part, d_odoc, d_ofr, d_osrc, d_ohoff, d_opos, d_err, d_cnt, d_idx2, d_tb, d_th, d_enc, d_henc, d_segs, d_oi, d_oh;
+        FreeBufs fr{{&d_idx,  &d_hits, &d_bl,   &d_bo,   &d_tf,    &d_hb,   &d_hbo, &d_ht,  &d_views, &d_lists, &d_lblk, &d_lpost, &d_ud,
+                     &d_uf,   &d_doc,  &d_fr,   &d_hc,   &d_hoff,  &d_pos,  &d_keep, &d_ks, &d_bm,    &d_part,  &d_odoc, &d_ofr,   &d_osrc,
+                     &d_ohoff, &d_opos, &d_err, &d_cnt, &d_idx2, &d_tb,  &d_th,  &d_enc, &d_henc,  &d_segs,  &d_oi,   &d_oh}};
+        std::vector<uint64_t> ibase(n + 1, 0), hbase(n + 1, 0), dbase(n + 1, 0), tbase(n + 1, 0), hbbase(n + 1, 0), termbase(n + 1, 0);
+        for (uint32_t s = 0; s < n; ++s) {
+                const bool u = used[s];
+                ibase[s + 1]    = ibase[s] + (u ? (src[s].index_bytes + 511) / 256 * 256 : 0);
+                hbase[s + 1]    = hbase[s] + (u && src[s].codec == TRN_CODEC_LUCENE ? (src[s].hits_bytes + 511) / 256 * 256 : 0);
+                dbase[s + 1]    = dbase[s] + dirs[s].blk_last.size();
+                tbase[s + 1]    = tbase[s] + dirs[s].tile_first.size();
+                hbbase[s + 1]   = hbbase[s] + hdirs[s].hblk_off.size();
+                termbase[s + 1] = termbase[s] + hdirs[s].hb_begin.size();
+        }
+        CKMG(d_idx.ensure(std::max<uint64_t>(256, ibase[n])));
+        CKMG(d_hits.ensure(std::max<uint64_t>(256, hbase[n])));
+        CKMG(d_bl.ensure(std::max<uint64_t>(4, dbase[n] * 4)));
+        CKMG(d_bo.ensure(std::max<uint64_t>(4, dbase[n] * 4)));
+        CKMG(d_hb.ensure(std::max<uint64_t>(4, dbase[n] * 4)));
+        CKMG(d_tf.ensure(std::max<uint64_t>(4, tbase[n] * 4)));
+        CKMG(d_hbo.ensure(std::max<uint64_t>(4, hbbase[n] * 4)));
+        CKMG(d_ht.ensure(std::max<uint64_t>(8, termbase[n] * 8)));
+        CK(cudaMemsetAsync(d_idx.p, 0, std::max<uint64_t>(256, ibase[n]), c->stream));
+        CK(cudaMemsetAsync(d_hits.p, 0, std::max<uint64_t>(256, hbase[n]), c->stream));
+        std::vector<HitsView>             views(std::max(1u, n));
+        std::vector<std::vector<HitTerm>> hterms(n); // read by the asynchronous uploads until the stream synchronises
+        for (uint32_t s = 0; s < n; ++s) {
+                if (!used[s])
+                        continue;
+                const auto &S = src[s];
+                const auto &D = dirs[s];
+                const auto &H = hdirs[s];
+                if (S.index_bytes)
+                        CK(cudaMemcpyAsync(d_idx.as<uint8_t>() + ibase[s], S.index, S.index_bytes, cudaMemcpyHostToDevice, c->stream));
+                if (S.codec == TRN_CODEC_LUCENE && S.hits_bytes)
+                        CK(cudaMemcpyAsync(d_hits.as<uint8_t>() + hbase[s], S.hits, S.hits_bytes, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_bl.as<uint32_t>() + dbase[s], D.blk_last.data(), D.blk_last.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_bo.as<uint32_t>() + dbase[s], D.blk_off.data(), D.blk_off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                if (!D.tile_first.empty())
+                        CK(cudaMemcpyAsync(d_tf.as<uint32_t>() + tbase[s], D.tile_first.data(), D.tile_first.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                if (S.codec == TRN_CODEC_LUCENE) {
+                        std::vector<HitTerm> &ht = hterms[s];
+                        ht.resize(H.hb_begin.size());
+                        for (size_t i = 0; i < ht.size(); ++i)
+                                ht[i] = HitTerm{H.hb_begin[i], H.sum_hits[i]};
+                        if (!H.hit_base.empty())
+                                CK(cudaMemcpyAsync(d_hb.as<uint32_t>() + dbase[s], H.hit_base.data(), H.hit_base.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                        if (!H.hblk_off.empty())
+                                CK(cudaMemcpyAsync(d_hbo.as<uint32_t>() + hbbase[s], H.hblk_off.data(), H.hblk_off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                        if (!ht.empty())
+                                CK(cudaMemcpyAsync(d_ht.as<HitTerm>() + termbase[s], ht.data(), ht.size() * 8, cudaMemcpyHostToDevice, c->stream));
+                }
+                views[s] = HitsView{d_idx.as<uint8_t>() + ibase[s], d_bl.as<uint32_t>() + dbase[s], d_bo.as<uint32_t>() + dbase[s], d_tf.as<uint32_t>() + tbase[s],
+                                    d_hits.as<uint8_t>() + hbase[s], d_hb.as<uint32_t>() + dbase[s],  d_hbo.as<uint32_t>() + hbbase[s], d_ht.as<HitTerm>() + termbase[s],
+                                    S.codec};
+        }
+        const uint64_t nupd   = P.upd_docid.size();
+        const uint64_t nwords = (uint64_t(maxdoc) >> 5) + 1;
+        CKMG(d_views.ensure(views.size() * sizeof(HitsView)));
+        CKMG(d_lists.ensure(std::max<size_t>(1, nlists) * sizeof(MergeList)));
+        CKMG(d_lblk.ensure((size_t(nlists) + 1) * 8));
+        CKMG(d_lpost.ensure((size_t(nlists) + 1) * 8));
+        CKMG(d_ud.ensure(std::max<uint64_t>(4, nupd * 4)));
+        CKMG(d_uf.ensure(std::max<uint64_t>(4, nupd * 4)));
+        CKMG(d_doc.ensure(std::max<uint64_t>(4, nposts * 4)));
+        CKMG(d_fr.ensure(std::max<uint64_t>(4, nposts * 4)));
+        CKMG(d_hc.ensure(std::max<uint64_t>(4, nposts * 4)));
+        CKMG(d_hoff.ensure((nposts + 1) * 8));
+        CKMG(d_keep.ensure(std::max<uint64_t>(4, nposts * 4)));
+        CKMG(d_ks.ensure((nposts + 1) * 8));
+        CKMG(d_part.ensure((nposts / 4096 + 4) * 8));
+        CKMG(d_bm.ensure(nwords * 4));
+        CKMG(d_err.ensure(16));
+        CKMG(d_cnt.ensure(8));
+        CKMG(d_idx2.ensure((size_t(nre) + 1) * 8));
+        CKMG(d_tb.ensure((size_t(nre) + 1) * 8));
+        CKMG(d_th.ensure((size_t(nre) + 1) * 8));
+        CK(cudaMemcpyAsync(d_views.p, views.data(), views.size() * sizeof(HitsView), cudaMemcpyHostToDevice, c->stream));
+        if (nlists)
+                CK(cudaMemcpyAsync(d_lists.p, lists.data(), nlists * sizeof(MergeList), cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_lblk.p, list_blk.data(), (size_t(nlists) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_lpost.p, list_post.data(), (size_t(nlists) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        if (nupd) {
+                CK(cudaMemcpyAsync(d_ud.p, P.upd_docid.data(), nupd * 4, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_uf.p, P.upd_first.data(), nupd * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        CK(cudaMemcpyAsync(d_idx2.p, re_first.data(), (size_t(nre) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemsetAsync(d_bm.p, 0, nwords * 4, c->stream));
+        CK(cudaMemsetAsync(d_err.p, 0xff, 16, c->stream));
+        CK(cudaMemsetAsync(d_cnt.p, 0, 8, c->stream));
+        MergeParams M{};
+        M.views     = d_views.as<HitsView>();
+        M.lists     = d_lists.as<MergeList>();
+        M.nlists    = nlists;
+        M.list_blk  = d_lblk.as<unsigned long long>();
+        M.list_post = d_lpost.as<unsigned long long>();
+        M.nblocks   = nblocks;
+        M.nposts    = nposts;
+        M.docids    = d_doc.as<uint32_t>();
+        M.freqs     = d_fr.as<uint32_t>();
+        M.hcount    = d_hc.as<uint32_t>();
+        M.hoff      = d_hoff.as<unsigned long long>();
+        M.upd_docid = d_ud.as<uint32_t>();
+        M.upd_first = d_uf.as<uint32_t>();
+        M.nupd      = nupd;
+        M.keep      = d_keep.as<uint32_t>();
+        M.bitmap    = d_bm.as<uint32_t>();
+        M.kscan     = d_ks.as<unsigned long long>();
+        M.error     = d_err.as<unsigned long long>();
+        // ---- decode docIDs and freqs of every list; keep (which also drops the hits of every posting that is not written); the hits of
+        // the kept postings
+        uint64_t nhits{0}, nkept{0}, herr2[2]{~0ull, ~0ull}, docs_cnt{0};
+        float    dec_ms{0}, m1{0}, m2{0}, d2{0}, enc_ms{0}, asm_ms{0};
+        CK(cudaEventRecord(X.ev[0], c->stream));
+        CK(launch_merge_decode(M, c->stream));
+        CK(cudaEventRecord(X.ev[1], c->stream));
+        CK(launch_merge_keep(M, c->stream));
+        CK(launch_enc_scan(M.keep, nposts, d_part.as<unsigned long long>(), d_ks.as<unsigned long long>(), c->stream));
+        CK(launch_merge_popcount(M.bitmap, nwords, d_cnt.as<unsigned long long>(), c->stream));
+        CK(launch_merge_gather(M.kscan, d_idx2.as<unsigned long long>(), nre + 1, d_tb.as<unsigned long long>(), c->stream));
+        CK(cudaEventRecord(X.ev[2], c->stream));
+        CK(launch_enc_scan(M.hcount, nposts, d_part.as<unsigned long long>(), d_hoff.as<unsigned long long>(), c->stream));
+        CK(cudaMemcpyAsync(&nhits, d_hoff.as<unsigned long long>() + nposts, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CKMG(d_pos.ensure(std::max<uint64_t>(4, nhits * 4)));
+        M.positions = d_pos.as<uint32_t>();
+        CK(launch_merge_hits_decode(M, c->stream));
+        CK(cudaEventRecord(X.ev[3], c->stream));
+        std::vector<uint64_t> h_tb(size_t(nre) + 1), h_th(size_t(nre) + 1);
+        CK(cudaMemcpyAsync(h_tb.data(), d_tb.p, (size_t(nre) + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(herr2, d_err.p, 16, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(&docs_cnt, d_cnt.p, 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&dec_ms, X.ev[0], X.ev[1]));
+        CK(cudaEventElapsedTime(&m1, X.ev[1], X.ev[2]));
+        CK(cudaEventElapsedTime(&d2, X.ev[2], X.ev[3]));
+        dec_ms += d2;
+        for (int k = 0; k < 2; ++k)
+                if (herr2[k] != ~0ull) {
+                        const uint32_t   l = uint32_t(std::upper_bound(list_post.begin(), list_post.end(), herr2[k]) - list_post.begin()) - 1u;
+                        const MergeList &L = lists[l];
+                        return fail(c, TRN_ERR_UNSUPPORTED,
+                                    name(L.view, L.term) + (k == 0 ? ": a hit with a payload must be re-encoded; the device encoders write no payloads"
+                                                                   : ": a hit at position 0 or above 16383 must be re-encoded; the device encoders take positions 1..16383"));
+                }
+        nkept = h_tb[nre];
+        CKMG(d_odoc.ensure(std::max<uint64_t>(4, nkept * 4)));
+        CKMG(d_ofr.ensure(std::max<uint64_t>(4, nkept * 4)));
+        CKMG(d_osrc.ensure(std::max<uint64_t>(8, nkept * 8)));
+        CKMG(d_ohoff.ensure((nkept + 1) * 8));
+        CKMG(d_part.ensure((std::max(nposts, nkept) / 4096 + 4) * 8));
+        M.out_docids = d_odoc.as<uint32_t>();
+        M.out_freqs  = d_ofr.as<uint32_t>();
+        M.out_src    = d_osrc.as<unsigned long long>();
+        M.out_hoff   = d_ohoff.as<unsigned long long>();
+        CK(cudaEventRecord(X.ev[4], c->stream));
+        CK(launch_merge_scatter(M, c->stream));
+        CK(launch_enc_scan(M.out_freqs, nkept, d_part.as<unsigned long long>(), d_ohoff.as<unsigned long long>(), c->stream));
+        CK(launch_merge_gather(M.out_hoff, d_tb.as<unsigned long long>(), nre + 1, d_th.as<unsigned long long>(), c->stream));
+        CK(cudaMemcpyAsync(h_th.data(), d_th.p, (size_t(nre) + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CKMG(d_opos.ensure(std::max<uint64_t>(4, h_th[nre] * 4)));
+        M.out_positions = d_opos.as<uint32_t>();
+        CK(launch_merge_out_hits(M, nkept, c->stream));
+        CK(cudaEventRecord(X.ev[5], c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&m2, X.ev[4], X.ev[5]));
+        for (DevBuf *b : {&d_fr, &d_hc, &d_hoff, &d_pos, &d_keep, &d_ks, &d_bm, &d_osrc, &d_lists, &d_lblk, &d_lpost, &d_ud, &d_uf})
+                b->release();
+        // ---- encode every re-encoded term in one call (orphans included: their headers are part of the output)
+        std::vector<uint64_t> chunk, toff, hto;
+        uint64_t              enc_bytes{0}, enc_hbytes{0};
+        if (nre) {
+                const DevPostings DP{h_tb.data(), nre, d_tb.as<unsigned long long>(), M.out_docids, M.out_freqs, M.out_positions};
+                int               r;
+                if (out_codec == TRN_CODEC_GOOGLE) {
+                        uint64_t nb{0};
+                        r = encode_google_device(c, DP, Codecs::Google::N, Codecs::Google::SKIPLIST_STEP, P.countdown_phase, true, ~0ull, &enc_bytes, d_enc, chunk, toff,
+                                                 &nb, &enc_ms);
+                } else
+                        r = encode_lucene_device(c, DP, true, ~0ull, &enc_bytes, true, ~0ull, &enc_hbytes, d_enc, d_henc, toff, &enc_ms, &hto);
+                if (r == TRN_ERR_CUDA && c->err.find("out of memory") != std::string::npos)
+                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: working memory cannot be allocated on the device; merge fewer sources");
+                if (r == TRN_ERR_ARG || r == TRN_ERR_CAPACITY) { // the encoder's refusal, for the re-encoded terms as a whole: name the first
+                        uint32_t k = 0;
+                        while (P.out[k].route != MERGE_REENCODE)
+                                ++k;
+                        const MergePart &p0 = P.parts[P.out[k].part_begin];
+                        return fail(c, r, "trn_merge_sources: re-encoding the merged terms (the first [" + std::string(src[P.order[p0.cand]].names[p0.term]) +
+                                                  "] of " + who(P.order[p0.cand]) + "): " + c->err);
+                }
+                if (r)
+                        return r;
+        }
+        // ---- assembly: output term order, appended chunks from the sources' bytes, re-encoded ones from the encoder's output
+        const bool             lucene = out_codec == TRN_CODEC_LUCENE;
+        std::vector<MergeCopy> segs;
+        std::vector<trn_term>  terms;
+        std::vector<uint32_t>  tsrc, tidx;
+        uint64_t               io{0}, ho{0}, sum_docs{0}, sum_hits{0};
+        uint32_t               appended{0}, reencoded{0}, orphaned{0};
+        for (uint32_t k = 0, r = 0; k < nout; ++k) {
+                const MergePart &p0 = P.parts[P.out[k].part_begin];
+                const uint32_t   s0 = P.order[p0.cand];
+                uint64_t         len, hlen, docs;
+                const uint8_t   *isrc, *hsrc;
+                if (P.out[k].route == MERGE_APPEND) {
+                        const trn_term &T = src[s0].terms[p0.term];
+                        len               = T.chunk_len;
+                        docs              = T.documents;
+                        isrc              = d_idx.as<uint8_t>() + ibase[s0] + T.chunk_off;
+                        hlen              = 0;
+                        hsrc              = nullptr;
+                        if (lucene) {
+                                if (len < 14)
+                                        return fail(c, TRN_ERR_ARG, name(s0, p0.term) + ": a LUCENE chunk is at least 14 bytes");
+                                uint32_t hdo, pcs;
+                                std::memcpy(&hdo, src[s0].index + T.chunk_off, 4);
+                                std::memcpy(&pcs, src[s0].index + T.chunk_off + 8, 4);
+                                if (uint64_t(hdo) + pcs > src[s0].hits_bytes)
+                                        return fail(c, TRN_ERR_ARG, name(s0, p0.term) + ": its positions chunk lies outside the source's hits.data");
+                                hlen = pcs;
+                                hsrc = d_hits.as<uint8_t>() + hbase[s0] + hdo;
+                        }
+                        ++appended;
+                } else {
+                        len  = toff[r + 1] - toff[r];
+                        isrc = d_enc.as<uint8_t>() + toff[r];
+                        hlen = lucene ? hto[r + 1] - hto[r] : 0;
+                        hsrc = lucene ? d_henc.as<uint8_t>() + hto[r] : nullptr;
+                        docs = h_tb[r + 1] - h_tb[r];
+                        if (P.out[k].stats) {
+                                sum_docs += docs;
+                                sum_hits += h_th[r + 1] - h_th[r];
+                        }
+                        ++r;
+                        if (docs)
+                                ++reencoded;
+                        else
+                                ++orphaned;
+                }
+                if (ho >= (1ull << 32))
+                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
+                // a CTA per piece of at most kPiece bytes, so a long chunk is copied by many CTAs
+                constexpr uint64_t kPiece = 1u << 16;
+                for (uint64_t a = 0; a < len || a == 0; a += kPiece)
+                        segs.push_back(MergeCopy{isrc + a, io + a, std::min(kPiece, len - a), 0u, lucene && a == 0 ? 1u : 0u, uint32_t(ho)});
+                for (uint64_t a = 0; a < hlen; a += kPiece)
+                        segs.push_back(MergeCopy{hsrc + a, ho + a, std::min(kPiece, hlen - a), 1u, 0u, 0u});
+                if (docs) {
+                        terms.push_back(trn_term{uint32_t(docs), uint32_t(io), uint32_t(len)});
+                        tsrc.push_back(s0);
+                        tidx.push_back(p0.term);
+                }
+                io += len;
+                ho += hlen;
+                if (io >= (1ull << 32))
+                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged index reaches 4 GiB (range32_t chunk offsets)");
+        }
+        if (ho >= (1ull << 32))
+                return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
+        std::vector<uint8_t> index, hits;
+        try {
+                index.resize(io);
+                hits.resize(ho);
+        } catch (const std::bad_alloc &) {
+                return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the result cannot be allocated on the host");
+        }
+        CKMG(d_segs.ensure(std::max<size_t>(1, segs.size()) * sizeof(MergeCopy)));
+        CKMG(d_oi.ensure(std::max<uint64_t>(4, io)));
+        CKMG(d_oh.ensure(std::max<uint64_t>(4, ho)));
+        if (!segs.empty())
+                CK(cudaMemcpyAsync(d_segs.p, segs.data(), segs.size() * sizeof(MergeCopy), cudaMemcpyHostToDevice, c->stream));
+        CK(cudaEventRecord(X.ev[6], c->stream));
+        CK(launch_merge_assemble(d_segs.as<MergeCopy>(), uint32_t(segs.size()), d_oi.as<uint8_t>(), d_oh.as<uint8_t>(), c->stream));
+        CK(cudaEventRecord(X.ev[7], c->stream));
+        if (io)
+                CK(cudaMemcpyAsync(index.data(), d_oi.p, io, cudaMemcpyDeviceToHost, c->stream));
+        if (ho)
+                CK(cudaMemcpyAsync(hits.data(), d_oh.p, ho, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        CK(cudaEventElapsedTime(&asm_ms, X.ev[6], X.ev[7]));
+        X.index.swap(index);
+        X.hits.swap(hits);
+        X.terms.swap(terms);
+        X.term_source.swap(tsrc);
+        X.term_index.swap(tidx);
+        *out                  = trn_merged{};
+        out->index            = X.index.data();
+        out->index_bytes      = X.index.size();
+        out->hits             = X.hits.data();
+        out->hits_bytes       = X.hits.size();
+        out->terms            = X.terms.data();
+        out->term_source      = X.term_source.data();
+        out->term_index       = X.term_index.data();
+        out->nterms           = uint32_t(X.terms.size());
+        out->total_terms      = uint32_t(X.terms.size());
+        out->docs_cnt         = uint32_t(docs_cnt);
+        out->sum_terms_docs   = sum_docs;
+        out->sum_term_hits    = sum_hits;
+        out->appended         = appended;
+        out->reencoded        = reencoded;
+        out->orphaned         = orphaned;
+        out->postings_read    = nposts;
+        out->postings_written = nkept;
+        out->decode_ms        = dec_ms;
+        out->merge_ms         = m1 + m2;
+        out->encode_ms        = enc_ms;
+        out->assemble_ms      = asm_ms;
+        out->total_ms         = float(now_ms() - t_begin);
+        c->have_kernel_events = false;
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_merge_plan(int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, uint32_t *order, uint8_t *route,
+                                    uint8_t *stats, uint32_t *part_off, uint32_t *part_cand, uint32_t *part_term, uint32_t *nout, uint64_t *nparts,
+                                    uint32_t *upd_docid, uint32_t *upd_first, uint64_t *nupd, uint32_t *countdown_phase, char *err, size_t errcap) {
+        MergePlan   P;
+        std::string e;
+        const int   r = plan_merge(out_codec, src, n, disable_optimizations != 0, P, e);
+        if (r) {
+                if (err && errcap)
+                        std::snprintf(err, errcap, "%s", e.c_str());
+                return r;
+        }
+        const uint32_t no = uint32_t(P.out.size() - 1);
+        for (uint32_t j = 0; j < n; ++j)
+                order[j] = P.order[j];
+        for (uint32_t k = 0; k <= no; ++k) {
+                part_off[k] = P.out[k].part_begin;
+                if (k < no) {
+                        route[k] = P.out[k].route;
+                        stats[k] = P.out[k].stats;
+                }
+        }
+        for (size_t q = 0; q < P.parts.size(); ++q) {
+                part_cand[q] = P.parts[q].cand;
+                part_term[q] = P.parts[q].term;
+        }
+        for (size_t i = 0; i < P.upd_docid.size(); ++i) {
+                upd_docid[i] = P.upd_docid[i];
+                upd_first[i] = P.upd_first[i];
+        }
+        *nout            = no;
+        *nparts          = P.parts.size();
+        *nupd            = P.upd_docid.size();
+        *countdown_phase = P.countdown_phase;
         return TRN_OK;
 }

@@ -1076,6 +1076,7 @@ __global__ void __launch_bounds__(kThreads) k_decode_terms(DevIndex ix, const ui
 #include "intersect.cuh"
 #include "percolate.cuh"
 #include "index_docs.cuh"
+#include "merge.cuh"
 
 // ------------------------------------------------------------------------------------------------ launch wrappers
 uint32_t exec_stage_bytes(int codec) {

@@ -1,6 +1,7 @@
 // Launch wrappers implemented in kernels.cu
 #pragma once
 #include "device_types.h"
+#include "hitcursor.h"
 #include <cuda_runtime.h>
 
 namespace trn {
@@ -66,4 +67,45 @@ cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *ke
 cudaError_t launch_post_freqs(const IndexParams &P, uint64_t nposts, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
+// merge (merge.cuh): the device half of trn_merge_sources
+struct MergeList { // one participant list of an output term (lists of one term are consecutive, newest first)
+        DevTerm  t;        // the term in its source's block directory
+        uint32_t view;     // its source's entry in MergeParams::views
+        uint32_t term;     // term index in that source (the hits directory's HitTerm)
+        uint32_t cand;     // candidate (newest first): its registry masks d iff upd_first(d) < cand
+        uint32_t rank;     // participant rank inside the term (0 = newest)
+        uint32_t nparts;   // participants of the term
+        uint32_t reencode; // 0: an appended chunk (decoded for docs_cnt only)
+};
+struct MergeParams {
+        const HitsView *          views;
+        const MergeList *         lists;
+        uint32_t                  nlists;
+        const unsigned long long *list_blk, *list_post; // nlists + 1 prefix sums of blocks / postings
+        unsigned long long        nblocks, nposts;
+        uint32_t *                docids, *freqs, *hcount; // decoded postings; hcount = freq of a re-encoded posting, else 0
+        const unsigned long long *hoff;                    // scan of hcount
+        uint32_t *                positions;
+        const uint32_t *          upd_docid, *upd_first;
+        unsigned long long        nupd;
+        uint32_t *                keep, *bitmap;
+        const unsigned long long *kscan;
+        uint32_t *                out_docids, *out_freqs, *out_positions;
+        unsigned long long *      out_src;
+        const unsigned long long *out_hoff;
+        unsigned long long *      error; // first kept posting with [0] a payload hit, [1] a position outside 1..16383 (~0: none)
+};
+struct MergeCopy {
+        const uint8_t *    src;
+        unsigned long long dst, len;
+        uint32_t           to_hits, header, hits_off; // header: a LUCENE index chunk whose first u32 becomes hits_off
+};
+cudaError_t launch_merge_decode(const MergeParams &P, cudaStream_t stream);
+cudaError_t launch_merge_hits_decode(const MergeParams &P, cudaStream_t stream);
+cudaError_t launch_merge_keep(const MergeParams &P, cudaStream_t stream);
+cudaError_t launch_merge_scatter(const MergeParams &P, cudaStream_t stream);
+cudaError_t launch_merge_out_hits(const MergeParams &P, uint64_t nout, cudaStream_t stream);
+cudaError_t launch_merge_gather(const unsigned long long *a, const unsigned long long *idx, uint32_t n, unsigned long long *out, cudaStream_t stream);
+cudaError_t launch_merge_popcount(const uint32_t *bitmap, uint64_t nwords, unsigned long long *count, cudaStream_t stream);
+cudaError_t launch_merge_assemble(const MergeCopy *segs, uint32_t nsegs, uint8_t *index_out, uint8_t *hits_out, cudaStream_t stream);
 } // namespace trn

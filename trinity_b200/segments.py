@@ -12,7 +12,7 @@ from typing import List, Sequence
 
 import numpy as np
 
-from . import (EMPTY_TERM, NODE_TERM, GpuIndexSource, Segment, TermDictionary, bm25_idf, parse_query)
+from . import (EMPTY_TERM, NODE_TERM, GpuIndexSource, MergedSegment, MergeSource, Segment, TermDictionary, bm25_idf, parse_query)
 
 
 def generation_of(path: str) -> int:
@@ -23,6 +23,8 @@ def generation_of(path: str) -> int:
 class SegmentCollection:
     def __init__(self, paths: Sequence[str], device: int = 0, max_docid: int | None = None):
         paths = sorted((str(p) for p in paths), key=generation_of, reverse=True)
+        self.paths = paths
+        self.device = device
         self.generations = [generation_of(p) for p in paths]
         if len(set(self.generations)) != len(paths):
             raise ValueError("no two sources may share a generation")
@@ -44,6 +46,16 @@ class SegmentCollection:
             self.sources.append(g)
             if s.masked_documents.size:
                 newer = np.union1d(newer, s.masked_documents).astype(np.uint32)
+
+    def merge(self, out_codec: int, disable_optimizations: bool = False, device: int | None = None) -> MergedSegment:
+        """== MergeCandidatesCollection::merge over the collection's segments as they were opened (newest first, each masked by the
+        updated documents of the newer ones) into one segment of out_codec; MergedSegment.write(path) persists it"""
+        srcs = [MergeSource.of_segment(s, p, g) for s, p, g in zip(self.segments, self.paths, self.generations)]
+        g = GpuIndexSource(self.device if device is None else device)
+        try:
+            return g.merge_sources(out_codec, srcs, disable_optimizations)
+        finally:
+            g.close()
 
     def document_frequency(self, term: str) -> int:
         return self._df.get(term, 0)
