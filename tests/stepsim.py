@@ -6,21 +6,12 @@ import trinity_b200 as tb
 
 OP_LEAF, OP_SLOT, OP_CLEAR, OP_LEAFSCORE, OP_COUNT_ADD, OP_COUNT_GE = 0, 1, 2, 3, 4, 5
 M_SET, M_OR, M_AND, M_ANDNOT, M_NONE = 0, 1, 2, 3, 4
-F_SCORE, F_BREAK_IF_EMPTY, F_MASKED, F_MASKOP = 1, 2, 4, 8
+F_SCORE, F_BREAK_IF_EMPTY = 1, 2
 
 
-def run(steps, root_slot, nslots, lists, ndocs, tree=False, rng=None):
+def run(steps, root_slot, nslots, lists, ndocs, tree=False):
     """returns (match[ndocs+1], score[ndocs+1]); lists[t] = (docids, freqs).  tree: a flat-tree program — its leading
-    [LEAF, mode NONE, dst] markers name bitmaps that one flat decode pass fills before the slot operations run.  Markers flagged F_MASKED
-    are filled in a second pass, after the F_MASKOP operations: the kernel decodes only the blocks that hold a docID of the mask bitmap
-    (slot `src`), i.e. the leaf keeps every posting inside the mask and an arbitrary subset of the others — `rng` picks that subset
-    (None: none of them, the most aggressive reading)"""
-    if tree and any(int(st["op"]) == OP_LEAF and (int(st["flags"]) & F_MASKED) for st in steps):
-        first = [st for st in steps if int(st["op"]) == OP_LEAF and not (int(st["flags"]) & F_MASKED)]
-        second = [st for st in steps if int(st["op"]) == OP_LEAF and (int(st["flags"]) & F_MASKED)]
-        maskops = [st for st in steps if int(st["op"]) != OP_LEAF and (int(st["flags"]) & F_MASKOP)]
-        rest = [st for st in steps if int(st["op"]) != OP_LEAF and not (int(st["flags"]) & F_MASKOP)]
-        steps = first + maskops + second + rest
+    [LEAF, mode NONE, dst] markers name bitmaps that one flat decode pass fills before the slot operations run"""
     slots = [np.zeros(ndocs + 1, bool) for _ in range(nslots)]
     acc = np.zeros(ndocs + 1, np.float32)  # the kernels accumulate fp32 scores in step order
     dead = False
@@ -49,11 +40,6 @@ def run(steps, root_slot, nslots, lists, ndocs, tree=False, rng=None):
             m, s = leaf(int(st["term"]))
             if op == OP_LEAF:
                 if tree and mode == M_NONE:
-                    if int(st["flags"]) & F_MASKED:
-                        keep = slots[src].copy()
-                        if rng is not None:
-                            keep |= rng.random(ndocs + 1) < 0.5
-                        m = m & keep
                     slots[dst] = m.copy()
                 if mode == M_SET: slots[dst] = m.copy()
                 elif mode == M_OR: slots[dst] |= m

@@ -244,7 +244,7 @@ def debug_positions(codec: int, index: np.ndarray, hits: np.ndarray, term, docid
 
 def debug_compile(codec: int, index: np.ndarray, terms: np.ndarray, nodes: np.ndarray, scored):
     """(steps, root_slot, nslots): the bitmap-path step program of one plan, compiled on the host (no GPU needed).
-    scored: False / True, 2 = the DocumentsOnly program in its flat-tree form, 3 = flat-tree form with the masked second decode pass"""
+    scored: False / True, 2 = the DocumentsOnly program in its flat-tree form"""
     from ._ffi import STEP_DTYPE
     index = np.ascontiguousarray(index, dtype=np.uint8)
     terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)

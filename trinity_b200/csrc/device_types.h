@@ -79,9 +79,7 @@ static constexpr uint32_t kEncU32 = 0, kEncU16 = 1, kEncBitmap = 2, kEncU8B = 3;
 
 enum StepFlags : uint8_t {
         F_SCORE          = 1,
-        F_BREAK_IF_EMPTY = 2,
-        F_MASKED         = 4, // flat-tree leaf marker: decoded in the SECOND pass, only the blocks that hold a docID of the bitmap in slot `src`
-        F_MASKOP         = 8  // flat-tree slot operation of the mask section (runs between the two decode passes)
+        F_BREAK_IF_EMPTY = 2
 };
 
 struct DevStep {

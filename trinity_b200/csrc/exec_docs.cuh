@@ -1082,7 +1082,7 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 const uint32_t lo = tile << P.exec_shift, hi = lo + W;
                 bool           dead = false;
                 int            handled = 0;
-                if constexpr (TREE) { // flat-tree plan: its leaves in (at most) two decode passes, then its slot operations
+                if constexpr (TREE) { // flat-tree plan: its leaves in one decode pass, then its slot operations
                         handled = tree_exec_google(P, Q, TS, lo, W, NW, slots, stage, lane) ? 2 : 1;
                 } else if (!LUC && Q.route != TRN_ROUTE_STEPS) // (the flat AND / OR plans: the other routes never reach this launch)
                         handled = flat_exec_google(P, Q, lo, W, NW, slots, stage, lane);

@@ -209,10 +209,10 @@ __device__ void google_leaf_own(const DevIndex &ix, const DevTerm &T, uint32_t b
 // word each) — is loaded ONCE per query into lane registers (lane j: leaf j; lane k: operation k) and reused for all of its tiles.
 struct TreeState {
         uint32_t dir, nb, docs, first, last, tfb, tfbase; // lane j < nleaf: leaf j
-        uint32_t tfs;                                      // bits 0-7: tf_shift; 8-12: mask slot; 16: decoded in the masked second pass
+        uint32_t tfs;                                      // lane j < nleaf: leaf j's tf_shift
         uint32_t dense;                                    // lane j < nleaf: first word of leaf j's resident bitmap (kDenseNone: decoded)
-        uint32_t op, mop;                                  // lane k < nops / nmops: packed slot operation k of the main / mask section
-        uint32_t nleaf, nops, nmops, nmasked;              // (uniform)
+        uint32_t op;                                       // lane k < nops: packed slot operation k
+        uint32_t nleaf, nops;                              // (uniform)
 };
 
 __device__ __forceinline__ uint32_t tree_pack(const DevStep &st) {
@@ -220,25 +220,18 @@ __device__ __forceinline__ uint32_t tree_pack(const DevStep &st) {
 }
 
 __device__ void tree_load(const ExecParams &P, const DevQuery &Q, TreeState &S, int lane) {
-        S.nleaf = S.nops = S.nmops = S.nmasked = 0;
+        S.nleaf = S.nops = 0;
         S.dir = S.nb = S.docs = S.first = S.last = S.tfb = S.tfbase = 0;
         S.tfs = 32;
         S.dense = kDenseNone;
-        S.op = S.mop = 0;
-        uint32_t myTerm = kEmptyTerm, myMask = 0;
+        S.op = 0;
+        uint32_t myTerm = kEmptyTerm;
         for (uint32_t si = 0; si < Q.nsteps; ++si) {
                 const DevStep st = P.steps[Q.step_begin + si];
                 if (st.op == OP_LEAF) { // markers: leaf S.nleaf owns slot S.nleaf
-                        if (uint32_t(lane) == S.nleaf) {
+                        if (uint32_t(lane) == S.nleaf)
                                 myTerm = st.term;
-                                myMask = (st.flags & F_MASKED) ? (0x10000u | (uint32_t(st.src) << 8)) : 0u;
-                        }
-                        S.nmasked += (st.flags & F_MASKED) ? 1u : 0u;
                         ++S.nleaf;
-                } else if (st.flags & F_MASKOP) {
-                        if (uint32_t(lane) == S.nmops)
-                                S.mop = tree_pack(st);
-                        ++S.nmops;
                 } else {
                         if (uint32_t(lane) == S.nops)
                                 S.op = tree_pack(st);
@@ -258,12 +251,9 @@ __device__ void tree_load(const ExecParams &P, const DevQuery &Q, TreeState &S, 
                 if (P.ix.dense_off)
                         S.dense = __ldg(P.ix.dense_off + myTerm);
         }
-        S.tfs |= myMask;
 }
 
 // returns true when the plan's F_BREAK_IF_EMPTY fired (the tile matches nothing); else the root docset is in slot Q.root_slot.
-// Two decode passes (planner.cpp: flat_tree_masks): pass 0 decodes the first-pass leaves and runs the mask section; pass 1 decodes, of the
-// masked leaves, only the blocks whose docID range holds a set bit of their mask bitmap, and runs the plan's own slot operations.
 __device__ bool tree_exec_google(const ExecParams &P, const DevQuery &Q, const TreeState &S, uint32_t lo, uint32_t W, uint32_t NW, uint32_t *slots, uint8_t *stage, int lane) {
         const uint32_t nleaf = S.nleaf;
         // ---- leaf bitmaps start empty
@@ -275,146 +265,87 @@ __device__ bool tree_exec_google(const ExecParams &P, const DevQuery &Q, const T
         }
         const uint32_t dummy   = uint32_t(__cvta_generic_to_shared(stage + kGatherBufBytes)) + uint32_t(lane) * 4u;
         const uint32_t slots_s = uint32_t(__cvta_generic_to_shared(slots));
-        uint32_t *     queue   = reinterpret_cast<uint32_t *>(stage + kGatherBufBytes + 128u); // 64 entries: the needed (leaf, block) pairs of pass 1
         const uint32_t NW4     = NW >> 2;
         const uint32_t past    = P.ix.max_docid < 0x80000000u ? 0x80000000u - W : 0u;
         __syncwarp(); // the clears above are visible before the first store
-        for (uint32_t pass = 0; pass < 2u; ++pass) {
-                const bool masked = pass != 0u;
-                if (!masked || S.nmasked) {
-                        // ---- leaves of this pass with a resident bitmap: a vector copy of the tile's words (the tile lies inside the bitmap's span)
-                        const bool inTile = uint32_t(lane) < nleaf && S.nb && ((S.tfs >> 16) & 1u) == pass && lo <= S.last && lo + (W - 1u) >= S.first;
-                        for (unsigned dm = __ballot_sync(0xffffffffu, inTile && S.dense != kDenseNone); dm; dm &= dm - 1u) {
-                                const int      j  = __ffs(int(dm)) - 1;
-                                const uint32_t f  = __shfl_sync(0xffffffffu, S.first, j);
-                                const uint4 *  s4 = reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, S.dense, j) +
-                                                                                   ((lo - ((f >> kDenseAlignShift) << kDenseAlignShift)) >> 5));
-                                uint4 *d4 = reinterpret_cast<uint4 *>(slots) + size_t(j) * NW4;
-                                for (uint32_t i = lane; i < NW4; i += 32)
-                                        d4[i] = __ldg(s4 + i);
-                        }
-                        // ---- the tile's blocks of every other leaf of this pass
-                        uint32_t mybA = 0, mycnt = 0;
-                        if (inTile && S.dense == kDenseNone) {
-                                const uint32_t tfs = S.tfs & 0xffu;
-                                const uint32_t a   = first_block_ge(P.ix, S.dir, S.nb, S.first, S.last, S.tfb, S.tfbase, tfs, lo);
-                                if (a < S.nb) {
-                                        const uint32_t hi = lo + W; // wraps to 0 for the last tile of a 2^32 docID space
-                                        const uint32_t e  = (hi == 0u || hi > S.last) ? S.nb : first_block_ge(P.ix, S.dir, S.nb, S.first, S.last, S.tfb, S.tfbase, tfs, hi);
-                                        mybA              = a;
-                                        mycnt             = min(e, S.nb - 1u) - a + 1u;
-                                }
-                        }
-                        const uint32_t incl  = warp_incl_scan(mycnt, lane);
-                        const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-                        // (leaf, block) of flat entry f; all lanes take part
-                        auto locate = [&](uint32_t f, bool act, uint32_t &j, uint32_t &b) {
-                                j = 0;
-                                for (uint32_t k = 0; k + 1u < nleaf; ++k)
-                                        j += (f >= __shfl_sync(0xffffffffu, incl, int(k))) ? 1u : 0u;
-                                if (!act)
-                                        j = nleaf - 1u;
-                                const uint32_t jincl = __shfl_sync(0xffffffffu, incl, int(j)), jcnt = __shfl_sync(0xffffffffu, mycnt, int(j));
-                                b                    = __shfl_sync(0xffffffffu, mybA, int(j)) + (f - (jincl - jcnt));
-                        };
-                        auto fill = [&](FlatLane &L, uint32_t j, uint32_t b) {
-                                const uint32_t dir  = __shfl_sync(0xffffffffu, S.dir, int(j));
-                                const uint32_t nb   = __shfl_sync(0xffffffffu, S.nb, int(j));
-                                const uint32_t docs = __shfl_sync(0xffffffffu, S.docs, int(j));
-                                L.j                 = j;
-                                L.off = L.n = L.prev = L.last = 0;
-                                if (L.active) {
-                                        const uint32_t *bl = P.ix.blk_last + dir, *bo = P.ix.blk_off + dir;
-                                        L.off  = __ldg(bo + b);
-                                        L.last = __ldg(bl + b);
-                                        L.prev = b ? __ldg(bl + b - 1u) : 0u;
-                                        L.n    = (b + 1u == nb) ? (docs - 32u * (nb - 1u)) : 32u;
-                                }
-                        };
-                        uint32_t fnext = 0, qhead = 0, qn = 0; // (uniform) next unexamined flat entry; the queue of pass 1
-                        // the next group of up to 32 blocks to decode; returns false when the pass is done
-                        auto next = [&](FlatLane &L) -> bool {
-                                if (!masked) {
-                                        if (fnext >= total)
-                                                return false;
-                                        const uint32_t f = fnext + uint32_t(lane);
-                                        fnext += 32u;
-                                        L.active = f < total;
-                                        uint32_t j, b;
-                                        locate(f, L.active, j, b);
-                                        fill(L, j, b);
-                                        return true;
-                                }
-                                while (qn < 32u && fnext < total) { // examine 32 more entries: does the mask hold a docID of the block's range?
-                                        const uint32_t f   = fnext + uint32_t(lane);
-                                        const bool     act = f < total;
-                                        fnext += 32u;
-                                        uint32_t j, b;
-                                        locate(f, act, j, b);
-                                        const uint32_t dir = __shfl_sync(0xffffffffu, S.dir, int(j));
-                                        const uint32_t ms  = (__shfl_sync(0xffffffffu, S.tfs, int(j)) >> 8) & 31u;
-                                        bool           need{false};
-                                        if (act) {
-                                                const uint32_t *bl   = P.ix.blk_last + dir;
-                                                const uint32_t  last = __ldg(bl + b), prev = b ? __ldg(bl + b - 1u) : 0u;
-                                                const uint32_t  d0 = max(prev + 1u, lo), d1 = min(last, lo + (W - 1u));
-                                                if (d0 <= d1) {
-                                                        const uint32_t  r0 = d0 - lo, r1 = d1 - lo;
-                                                        const uint32_t *M  = slots + size_t(ms) * NW;
-                                                        uint32_t        w = r0 >> 5, v = M[w] & (0xffffffffu << (r0 & 31u));
-                                                        const uint32_t  w1 = r1 >> 5;
-                                                        while (w < w1 && !v)
-                                                                v = M[++w];
-                                                        if (w == w1)
-                                                                v &= 0xffffffffu >> (31u - (r1 & 31u));
-                                                        need = v != 0u;
-                                                }
-                                        }
-                                        const unsigned m = __ballot_sync(0xffffffffu, need);
-                                        if (need)
-                                                queue[(qhead + qn + __popc(m & ((1u << lane) - 1u))) & 63u] = (j << 28) | b;
-                                        qn += __popc(m);
-                                }
-                                if (!qn)
-                                        return false;
-                                __syncwarp();
-                                const uint32_t take = min(qn, 32u);
-                                L.active            = uint32_t(lane) < take;
-                                const uint32_t e    = L.active ? queue[(qhead + uint32_t(lane)) & 63u] : 0u;
-                                qhead += take;
-                                qn -= take;
-                                fill(L, e >> 28, e & 0x0fffffffu);
-                                return true;
-                        };
-                        uint32_t tail_a = dummy, tail_bits = 0;
-                        FlatLane cur;
-                        bool     more = next(cur);
-                        if (more)
-                                gather_issue(P.ix.index, cur.off, cur.active, stage, lane);
-                        while (more) {
-                                gather_wait<0>();
-                                OwnAcc bs;
-                                bs.init(slots_s + cur.j * NW * 4u, dummy);
-                                if (cur.active)
-                                        google_block_docs_lane(P.ix.index, cur.off, stage, lane, cur.n, cur.prev, cur.last, lo, W, bs, past);
-                                __syncwarp();
-                                if (tail_bits) // the previous group's last words, after every block that can share them has stored
-                                        asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(tail_a), "r"(tail_bits) : "memory");
-                                tail_a    = bs.cur_a;
-                                tail_bits = bs.cur;
-                                more      = next(cur);
-                                if (more)
-                                        gather_issue(P.ix.index, cur.off, cur.active, stage, lane);
-                        }
-                        if (tail_bits)
-                                asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(tail_a), "r"(tail_bits) : "memory");
-                        __syncwarp();
+        // ---- leaves with a resident bitmap: a vector copy of the tile's words (the tile lies inside the bitmap's span)
+        const bool inTile = uint32_t(lane) < nleaf && S.nb && lo <= S.last && lo + (W - 1u) >= S.first;
+        for (unsigned dm = __ballot_sync(0xffffffffu, inTile && S.dense != kDenseNone); dm; dm &= dm - 1u) {
+                const int      j  = __ffs(int(dm)) - 1;
+                const uint32_t f  = __shfl_sync(0xffffffffu, S.first, j);
+                const uint4 *  s4 = reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, S.dense, j) +
+                                                                   ((lo - ((f >> kDenseAlignShift) << kDenseAlignShift)) >> 5));
+                uint4 *d4 = reinterpret_cast<uint4 *>(slots) + size_t(j) * NW4;
+                for (uint32_t i = lane; i < NW4; i += 32)
+                        d4[i] = __ldg(s4 + i);
+        }
+        // ---- the tile's blocks of every other leaf
+        uint32_t mybA = 0, mycnt = 0;
+        if (inTile && S.dense == kDenseNone) {
+                const uint32_t a = first_block_ge(P.ix, S.dir, S.nb, S.first, S.last, S.tfb, S.tfbase, S.tfs, lo);
+                if (a < S.nb) {
+                        const uint32_t hi = lo + W; // wraps to 0 for the last tile of a 2^32 docID space
+                        const uint32_t e  = (hi == 0u || hi > S.last) ? S.nb : first_block_ge(P.ix, S.dir, S.nb, S.first, S.last, S.tfb, S.tfbase, S.tfs, hi);
+                        mybA              = a;
+                        mycnt             = min(e, S.nb - 1u) - a + 1u;
                 }
-                // ---- slot operations of this pass (pass 0: the mask section), 128 bits per lane and step
-                const uint32_t cnt = masked ? S.nops : S.nmops;
-                const uint32_t reg = masked ? S.op : S.mop;
-                for (uint32_t k = 0; k < cnt; ++k) {
-                        const uint32_t w    = __shfl_sync(0xffffffffu, reg, int(k));
+        }
+        const uint32_t incl  = warp_incl_scan(mycnt, lane);
+        const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+        // lane assignment of the group that starts at flat entry g; all lanes take part
+        auto assign = [&](uint32_t g) {
+                FlatLane       L;
+                const uint32_t f = g + uint32_t(lane);
+                L.active         = f < total;
+                uint32_t j       = 0;
+                for (uint32_t k = 0; k + 1u < nleaf; ++k)
+                        j += (f >= __shfl_sync(0xffffffffu, incl, int(k))) ? 1u : 0u;
+                if (!L.active)
+                        j = nleaf - 1u;
+                const uint32_t jincl = __shfl_sync(0xffffffffu, incl, int(j)), jcnt = __shfl_sync(0xffffffffu, mycnt, int(j));
+                const uint32_t b     = __shfl_sync(0xffffffffu, mybA, int(j)) + (f - (jincl - jcnt));
+                const uint32_t dir   = __shfl_sync(0xffffffffu, S.dir, int(j));
+                const uint32_t nb    = __shfl_sync(0xffffffffu, S.nb, int(j));
+                const uint32_t docs  = __shfl_sync(0xffffffffu, S.docs, int(j));
+                L.j                  = j;
+                L.off = L.n = L.prev = L.last = 0;
+                if (L.active) {
+                        const uint32_t *bl = P.ix.blk_last + dir, *bo = P.ix.blk_off + dir;
+                        L.off  = __ldg(bo + b);
+                        L.last = __ldg(bl + b);
+                        L.prev = b ? __ldg(bl + b - 1u) : 0u;
+                        L.n    = (b + 1u == nb) ? (docs - 32u * (nb - 1u)) : 32u;
+                }
+                return L;
+        };
+        uint32_t tail_a = dummy, tail_bits = 0;
+        FlatLane cur;
+        if (total) {
+                cur = assign(0);
+                gather_issue(P.ix.index, cur.off, cur.active, stage, lane);
+        }
+        for (uint32_t g = 0; g < total; g += 32u) {
+                gather_wait<0>();
+                OwnAcc bs;
+                bs.init(slots_s + cur.j * NW * 4u, dummy);
+                if (cur.active)
+                        google_block_docs_lane(P.ix.index, cur.off, stage, lane, cur.n, cur.prev, cur.last, lo, W, bs, past);
+                __syncwarp();
+                if (tail_bits) // the previous group's last words, after every block that can share them has stored
+                        asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(tail_a), "r"(tail_bits) : "memory");
+                tail_a    = bs.cur_a;
+                tail_bits = bs.cur;
+                if (g + 32u < total) {
+                        cur = assign(g + 32u);
+                        gather_issue(P.ix.index, cur.off, cur.active, stage, lane);
+                }
+        }
+        if (tail_bits)
+                asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(tail_a), "r"(tail_bits) : "memory");
+        __syncwarp();
+        // ---- slot operations, 128 bits per lane and step
+        for (uint32_t k = 0; k < S.nops; ++k) {
+                const uint32_t w    = __shfl_sync(0xffffffffu, S.op, int(k));
                 const uint32_t op   = w & 7u, mode = (w >> 3) & 7u, dsti = (w >> 6) & 31u, srci = (w >> 11) & 31u, flags = (w >> 16) & 3u, arg = (w >> 18) & 15u;
                 uint4 *        d4   = reinterpret_cast<uint4 *>(slots + size_t(dsti) * NW);
                 const uint4 *  s4   = reinterpret_cast<const uint4 *>(slots + size_t(srci) * NW);
@@ -477,7 +408,6 @@ __device__ bool tree_exec_google(const ExecParams &P, const DevQuery &Q, const T
                         if (!__any_sync(0xffffffffu, any != 0u))
                                 return true;
                 }
-        }
         }
         return false;
 }

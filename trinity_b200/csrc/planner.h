@@ -24,12 +24,6 @@ struct PlanConfig {
         uint32_t run_tiles{128};   // TRN_RUN_TILES: consecutive tiles per work item of the flat scored kernel (top-k state lives across a run)
         int      cand_cost{900};   // TRN_CAND_COST: modelled warp-instructions per 32 candidates of the candidate-driven conjunction (0 = never use it)
         bool     flat_scored{true}; // TRN_FLAT_SCORED=0: every scored query through the general step-program kernel (A/B switch)
-        bool     tree_masks{false}; // TRN_TREE_MASKS=1: flat-tree queries decode their frequent leaves in a masked second pass (flat_tree_masks). It
-                                    // halves the DRAM bytes, but the needed blocks of a tile fill a fraction of a 32-lane group, so the warp-instruction
-                                    // count does not drop and the benchmark's trees ran slower with it. Off by default. (Not a matter of WHICH leaves
-                                    // are admitted — TRN_TREE_MASK_NEED does not recover it: a few masked queries raise the launch-wide slot count and
-                                    // take resident warps from every query.)
-        double   tree_mask_need{0.6}; // TRN_TREE_MASK_NEED: a leaf is decoded in the masked pass when at most this share of its blocks is expected to survive its mask
         bool     allow_phrase{false}; // the kernels execute OP_PHRASE (GOOGLE: inline hits; LUCENE: once hits.data is uploaded)
         bool     dense_bitmaps{true}; // TRN_DENSE_BITMAPS=0: no resident docID bitmaps of dense terms (select_dense_terms)
         double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
