@@ -31,10 +31,12 @@ def considered_stream(group_docs, masked=(), orig_mask=None):
 
 
 # ------------------------------------------------------------------------------------------------ sequential transcription
-def consider_sequential(masks):
-    """ctx::consider over the considered masks, line by line (indexPrev is a uint8_t) -> {mask: cnt}"""
+def consider_sequential(masks, index_wrap=255):
+    """ctx::consider over the considered masks, line by line (indexPrev is a uint8_t: index_wrap = 255) -> {mask: cnt}; index_wrap = None
+    models an index that does not wrap, which the tests use to show that a case reaches the wrap"""
     matches = []  # [[v, cnt]]
     map_prev, index_prev = 0, 0
+    wrap = (lambda i: i) if index_wrap is None else (lambda i: i & index_wrap)
     for m in masks:
         if m == map_prev:
             matches[index_prev][1] += 1
@@ -48,7 +50,7 @@ def consider_sequential(masks):
             if (v & m) == m:
                 if m == v:
                     matches[i][1] += 1
-                index_prev = i & 255
+                index_prev = wrap(i)
                 absorbed = True
                 break
             elif (m & v) == v:
@@ -58,7 +60,7 @@ def consider_sequential(masks):
             else:
                 i += 1
         if not absorbed:
-            index_prev = n & 255
+            index_prev = wrap(n)
             matches.append([m, 1])
     return {v: c for v, c in matches}
 
