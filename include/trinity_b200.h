@@ -431,6 +431,19 @@ int trn_decode_terms(trn_ctx *, const uint32_t *term_ids, uint32_t nterms, int m
 int trn_encode_google(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
                       uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
                       float *device_ms);
+/* trn_encode_google for hits WITH payloads (google_codec.cpp:38-74, the TRACK_PAYLOADS layout): per hit varbyte(delta << 1 | changed),
+ * the size byte when it differs from the previous hit's of the same document (0 before a document's first hit), then the payload bytes.
+ * The other arguments mean what they mean for trn_encode_google; two more per-hit arrays (HOST pointers, sum(freqs) entries) sit beside
+ * positions[]:
+ *   payload_lens[]          the payload's size in bytes, 0..8
+ *   payloads[]              the payload: the low payload_lens[i] bytes of payloads[i] in memory order (what
+ *                           document_proxy::insert(term, pos, {(const uint8_t *)&v, len}) passes)
+ * Both NULL: no payloads, the bytes and kernels of trn_encode_google.  A hit at position 0 is written and counted when it has a payload.
+ * TRN_ERR_ARG: what trn_encode_google refuses, a position 0 without a payload, a payload of more than 8 bytes, one of the two arrays
+ * without the other, or payloads without positions. */
+int trn_encode_google_payloads(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                               const uint8_t *payload_lens, const uint64_t *payloads, uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown,
+                               uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms, float *device_ms);
 
 /* GPU-side Encoder, LUCENE layout == one fresh Codecs::Lucene::IndexSession fed begin_term / begin_document / new_hit / end_document /
  * end_term (lucene_codec.cpp:163-388; FastPFor<4> int-blocks of 128 values, one skiplist entry per full block) for hits without
@@ -446,6 +459,15 @@ int trn_encode_google(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, co
 int trn_encode_lucene(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
                       uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
                       trn_term *terms, float *device_ms);
+/* trn_encode_lucene for hits WITH payloads (lucene_codec.cpp:240-365): a full 128-hit block is intblock(position deltas)
+ * intblock(payload sizes) varbyte(sum of the sizes) and the payload bytes; a term's hit tail is varbyte(delta << 1 | changed) [size byte]
+ * per hit, `changed` against the previous hit of the tail (0 before its first, across documents), then every payload byte of the tail.
+ * payload_lens[] / payloads[] mean what they mean for trn_encode_google_payloads; both NULL: the bytes and kernels of trn_encode_lucene.
+ * TRN_ERR_ARG: what trn_encode_lucene refuses, a position 0 without a payload, a payload of more than 8 bytes, one of the two arrays
+ * without the other, or payloads without positions.  TRN_ERR_CAPACITY as for trn_encode_lucene. */
+int trn_encode_lucene_payloads(trn_ctx *, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                               const uint8_t *payload_lens, const uint64_t *payloads, uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes,
+                               uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes, trn_term *terms, float *device_ms);
 
 /* ------------------------------------------------------------------------------------------------ query-token intersections
  * == Trinity::intersect_impl(stopwordsMask, tokens, src, maskedDocumentsRegistry, out) (intersect.h:25-37, intersect.cpp:5-170), one call
@@ -571,6 +593,20 @@ typedef struct trn_indexed { /* owned by the ctx, valid until the next trn_index
 } trn_indexed;
 int trn_index_documents(trn_ctx *, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
                         uint32_t ndocs, uint32_t nterms, trn_indexed *out);
+/* trn_index_documents for hits WITH payloads (document_proxy::insert(term, pos, payload), indexer.h:115-147; indexer.cpp:14-30): two more
+ * per-token arrays (HOST pointers) beside tokens[] / positions[]:
+ *   payload_lens[]           the token's payload size in bytes, 0..8
+ *   payloads[]               its payload: the low payload_lens[i] bytes of payloads[i] in memory order
+ * Both NULL: trn_index_documents.  The device encoders write the hits with their payloads (trn_encode_google_payloads /
+ * trn_encode_lucene_payloads).  The refusals of trn_index_documents, except that a position 0 WITH a payload is indexed (the reference's
+ * encoders write it, and it counts in the freq and sum_term_hits), and:
+ *   TRN_ERR_ARG          a payload of more than 8 bytes (indexer.cpp:26), one of the two arrays without the other
+ *   TRN_ERR_UNSUPPORTED  two tokens of one document with the same term and position and different payloads, naming the document and term
+ *                        (the reference orders them with an unstable sort, indexer.cpp:55-57; equal payloads are fine); a position 0
+ *                        without a payload
+ *   TRN_ERR_CAPACITY     more than 2^32 - 1 tokens in the call (split the batch) */
+int trn_index_documents_payloads(trn_ctx *, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
+                                 const uint8_t *payload_lens, const uint64_t *payloads, uint32_t ndocs, uint32_t nterms, trn_indexed *out);
 /* Host code, no device: writes the segment directory `dir` as persist_segment / persist_terms do (indexer.cpp:241-300, codecs.cpp:17-27,
  * terms.cpp:126-172 pack_terms, docidupdates.cpp:8-73 pack_updates): `index`, `hits.data` (LUCENE), `terms.data`, `terms.idx`, `id`, and
  * `updated_documents.ids` when nupdated > 0.  terms[i] <-> names[i]; terms with documents == 0 are left out.  updated_docids = the ids of

@@ -40,6 +40,15 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _payload_arrays(lists):
+    """the per-hit payload sizes (uint8) and payloads (uint64) of (docids, freqs, positions, payload_lens, payloads) terms, concatenated"""
+    pl = np.ascontiguousarray(np.concatenate([np.asarray(l[3], np.uint8) for l in lists]), np.uint8)
+    pv = np.ascontiguousarray(np.concatenate([np.asarray(l[4], np.uint64) for l in lists]), np.uint64)
+    if len(pl) != len(pv):
+        raise TrinityError("one payload length and one payload per hit")
+    return pl, pv
+
+
 # ----------------------------------------------------------------------------------------------- index build (host)
 class IndexBuilder:
     """== Codecs::IndexSession + Codecs::Encoder (codecs.h:66-200).  Bytes are identical to the reference encoders'."""
@@ -706,30 +715,38 @@ class GpuIndexSource:
 
     def encode_google(self, lists, block_docs: int = 32, skiplist_step: int = 8, countdown: Optional[int] = None):
         """GPU-side Encoder (== Codecs::Google::Encoder, google_codec.cpp:9-176): builds the GOOGLE index of `lists` on the device.
-        lists: one (docids, freqs[, positions]) per term — positions (all of them or none) = the hits of the term's postings, concatenated.
-        Returns (index bytes, terms array, countdown after the last term, device_ms)."""
+        lists: one (docids, freqs[, positions[, payload_lens, payloads]]) per term — positions (all of them or none) = the hits of the
+        term's postings, concatenated; payload_lens (uint8, 0..8) / payloads (uint64, the payload in its low bytes) one per hit, all terms
+        or none (trn_encode_google_payloads).  Returns (index bytes, terms array, countdown after the last term, device_ms)."""
         lists = list(lists)
         with_pos = len(lists) > 0 and len(lists[0]) > 2 and lists[0][2] is not None
+        with_pay = with_pos and len(lists[0]) > 4 and lists[0][3] is not None
         tb = np.zeros(len(lists) + 1, np.uint64)
         for i, l in enumerate(lists):
             tb[i + 1] = tb[i] + len(l[0])
         d = np.concatenate([_u32(l[0]) for l in lists]) if lists else np.zeros(0, np.uint32)
         f = np.concatenate([_u32(l[1]) for l in lists]) if lists else np.zeros(0, np.uint32)
         p = np.concatenate([_u32(l[2]) for l in lists]) if with_pos else None
+        pl, pv = _payload_arrays(lists) if with_pay else (None, None)
         terms = np.zeros(len(lists), dtype=TERM_DTYPE)
         cd = C.c_uint32(countdown if countdown is not None else skiplist_step)
         nbytes, ms = C.c_uint64(), C.c_float()
         cap = 16 + 2 * len(lists) + int(d.size) * 11 + (int(f.sum()) * 5 if with_pos else int(f.sum())) + 8 * (int(d.size) // max(1, block_docs) + len(lists) + 1)
+        if with_pay:
+            cap += 9 * int(f.sum())  # a size byte and up to 8 payload bytes per hit
         out = np.zeros(cap, np.uint8)
-        self._ck(self._L.trn_encode_google(self._h, _ptr(tb), len(lists), _ptr(d), _ptr(f), _ptr(p), block_docs, skiplist_step, C.byref(cd),
-                                           _ptr(out), cap, C.byref(nbytes), _ptr(terms), C.byref(ms)))
+        self._ck(self._L.trn_encode_google_payloads(self._h, _ptr(tb), len(lists), _ptr(d), _ptr(f), _ptr(p), _ptr(pl), _ptr(pv), block_docs, skiplist_step,
+                                                    C.byref(cd), _ptr(out), cap, C.byref(nbytes), _ptr(terms), C.byref(ms)))
         return out[:nbytes.value].copy(), terms, int(cd.value), float(ms.value)
 
     def encode_lucene(self, lists):
         """GPU-side Encoder (== Codecs::Lucene::Encoder, lucene_codec.cpp:163-388): builds the LUCENE index and its hits.data on the device.
-        lists: one (docids, freqs[, positions]) per term, as for encode_google.  Returns (index bytes, hits bytes, terms array, device_ms)."""
+        lists: one (docids, freqs[, positions[, payload_lens, payloads]]) per term, as for encode_google.  Returns (index bytes, hits bytes,
+        terms array, device_ms)."""
         lists = list(lists)
         with_pos = len(lists) > 0 and len(lists[0]) > 2 and lists[0][2] is not None
+        with_pay = with_pos and len(lists[0]) > 4 and lists[0][3] is not None
+        pl, pv = _payload_arrays(lists) if with_pay else (None, None)
         tb = np.zeros(len(lists) + 1, np.uint64)
         for i, l in enumerate(lists):
             tb[i + 1] = tb[i] + len(l[0])
@@ -741,11 +758,11 @@ class GpuIndexSource:
         # upper bounds: an int-block is at most 1 + 4 * 166 bytes, so a full document block (two of them) < 11 bytes per document, a tail
         # document <= 10; a full hit block (int-block + 3) < 6 bytes per hit, a tail hit <= 3 (deltas < 2^14)
         icap = 16 + 14 * len(lists) + 11 * int(d.size) + 22 * (int(d.size) // 128)
-        hcap = 16 + 6 * nhits
+        hcap = 16 + 6 * nhits + (9 * nhits if with_pay else 0)  # with payloads: up to a size byte (or its int-block) and 8 bytes per hit
         index, hits = np.empty(icap, np.uint8), np.empty(hcap, np.uint8)
         nb, hb, ms = C.c_uint64(), C.c_uint64(), C.c_float()
-        self._ck(self._L.trn_encode_lucene(self._h, _ptr(tb), len(lists), _ptr(d), _ptr(f), _ptr(p), _ptr(index), icap, C.byref(nb),
-                                           _ptr(hits), hcap, C.byref(hb), _ptr(terms), C.byref(ms)))
+        self._ck(self._L.trn_encode_lucene_payloads(self._h, _ptr(tb), len(lists), _ptr(d), _ptr(f), _ptr(p), _ptr(pl), _ptr(pv), _ptr(index), icap,
+                                                    C.byref(nb), _ptr(hits), hcap, C.byref(hb), _ptr(terms), C.byref(ms)))
         return index[:nb.value].copy(), hits[:hb.value].copy(), terms, float(ms.value)
 
     def percolator_register(self, queries: Sequence[np.ndarray], nterms: int, term_cost=None) -> dict:
@@ -769,13 +786,18 @@ class GpuIndexSource:
         self._ck(self._L.trn_percolate(self._h, _ptr(offs), _ptr(tok) if len(tok) else None, len(docs), C.byref(r)))
         return PercolationResult(r)
 
-    def index_documents(self, codec: int, docids, docs: Sequence[np.ndarray], nterms: int, positions: Optional[Sequence[np.ndarray]] = None) -> "IndexedSegment":
+    def index_documents(self, codec: int, docids, docs: Sequence[np.ndarray], nterms: int, positions: Optional[Sequence[np.ndarray]] = None,
+                        payload_lens: Optional[Sequence[np.ndarray]] = None, payloads: Optional[Sequence[np.ndarray]] = None) -> "IndexedSegment":
         """== SegmentIndexSession begin / insert / commit for a batch: docs are uint32 term-id arrays (every id below nterms), docids their
-        ids (any order, > 0, none twice); positions: per document the position of every token, None = token i at i + 1.  The inversion
-        and the encode run on the device; the result holds the bytes commit() would have written."""
+        ids (any order, > 0, none twice); positions: per document the position of every token, None = token i at i + 1; payload_lens /
+        payloads (both or neither): per document every token's payload size (0..8) and payload (uint64, the payload in its low bytes), as
+        document_proxy::insert(term, pos, payload) takes them.  The inversion and the encode run on the device; the result holds the bytes
+        commit() would have written."""
         d = _u32(docids)
         if len(d) != len(docs) or (positions is not None and len(positions) != len(docs)):
             raise TrinityError("index_documents: one docID (and one positions array) per document")
+        if (payload_lens is None) != (payloads is None) or (payload_lens is not None and (len(payload_lens) != len(docs) or len(payloads) != len(docs))):
+            raise TrinityError("index_documents: payload_lens and payloads come together, one array of each per document")
         offs = np.zeros(len(docs) + 1, np.uint64)
         offs[1:] = np.cumsum([len(x) for x in docs])
         tok = _u32(np.concatenate([np.asarray(x, np.uint32) for x in docs]) if len(docs) else [])
@@ -784,17 +806,35 @@ class GpuIndexSource:
             pos = _u32(np.concatenate([np.asarray(x, np.uint32) for x in positions]) if len(docs) else [])
             if len(pos) != len(tok):
                 raise TrinityError("index_documents: one position per token")
-        return self.index_documents_flat(codec, d, offs, tok, nterms, pos)
+        pl = pv = None
+        if payload_lens is not None:
+            pl = np.ascontiguousarray(np.concatenate([np.asarray(x, np.uint8) for x in payload_lens]) if len(docs) else np.zeros(0, np.uint8), np.uint8)
+            pv = np.ascontiguousarray(np.concatenate([np.asarray(x, np.uint64) for x in payloads]) if len(docs) else np.zeros(0, np.uint64), np.uint64)
+            if len(pl) != len(tok) or len(pv) != len(tok):
+                raise TrinityError("index_documents: one payload length and one payload per token")
+        return self.index_documents_flat(codec, d, offs, tok, nterms, pos, pl, pv)
 
     def index_documents_flat(self, codec: int, docids: np.ndarray, doc_offsets: np.ndarray, tokens: np.ndarray, nterms: int,
-                             positions: Optional[np.ndarray] = None) -> "IndexedSegment":
-        """index_documents over the flat arrays of the C ABI (doc_offsets: uint64, ndocs + 1 entries)"""
+                             positions: Optional[np.ndarray] = None, payload_lens: Optional[np.ndarray] = None,
+                             payloads: Optional[np.ndarray] = None) -> "IndexedSegment":
+        """index_documents over the flat arrays of the C ABI (doc_offsets: uint64, ndocs + 1 entries; payload_lens uint8 and payloads
+        uint64 one per token, both or neither)"""
         d, tok = _u32(docids), _u32(tokens)
         offs = np.ascontiguousarray(doc_offsets, np.uint64)
         pos = None if positions is None else _u32(positions)
+        if (payload_lens is None) != (payloads is None):
+            raise TrinityError("index_documents: payload_lens and payloads come together")
         r = TrnIndexed()
-        self._ck(self._L.trn_index_documents(self._h, codec, _ptr(d), _ptr(offs), _ptr(tok) if len(tok) else None,
-                                             _ptr(pos) if pos is not None and len(pos) else None, len(d), nterms, C.byref(r)))
+        if payload_lens is None:
+            self._ck(self._L.trn_index_documents(self._h, codec, _ptr(d), _ptr(offs), _ptr(tok) if len(tok) else None,
+                                                 _ptr(pos) if pos is not None and len(pos) else None, len(d), nterms, C.byref(r)))
+        else:
+            pl, pv = np.ascontiguousarray(payload_lens, np.uint8), np.ascontiguousarray(payloads, np.uint64)
+            if len(pl) != len(tok) or len(pv) != len(tok):
+                raise TrinityError("index_documents: one payload length and one payload per token")
+            self._ck(self._L.trn_index_documents_payloads(self._h, codec, _ptr(d), _ptr(offs), _ptr(tok) if len(tok) else None,
+                                                          _ptr(pos) if pos is not None and len(pos) else None, _ptr(pl) if len(pl) else None,
+                                                          _ptr(pv) if len(pv) else None, len(d), nterms, C.byref(r)))
         return IndexedSegment(codec, r, d)
 
     def merge_sources(self, out_codec: int, sources: Sequence["MergeSource"], disable_optimizations: bool = False) -> "MergedSegment":

@@ -21,6 +21,7 @@ EXPORTS = [
     "trn_create", "trn_destroy", "trn_last_error", "trn_set_stream", "trn_upload_index", "trn_set_masked_documents", "trn_index_info_get",
     "trn_exec_batch", "trn_exec_batch_device", "trn_last_topk_device", "trn_merge_topk", "trn_fetch_results", "trn_last_timings",
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_encode_lucene", "trn_debug_chunk_plan",
+    "trn_encode_google_payloads", "trn_encode_lucene_payloads", "trn_index_documents_payloads",
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
@@ -197,6 +198,8 @@ def lib() -> C.CDLL:
         P(u32), P(i32))
     sig("trn_encode_google", i32, vp, vp, u32, vp, vp, vp, u32, u32, P(u32), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_encode_lucene", i32, vp, vp, u32, vp, vp, vp, vp, C.c_uint64, P(C.c_uint64), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
+    sig("trn_encode_google_payloads", i32, vp, vp, u32, vp, vp, vp, vp, vp, u32, u32, P(u32), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
+    sig("trn_encode_lucene_payloads", i32, vp, vp, u32, vp, vp, vp, vp, vp, vp, C.c_uint64, P(C.c_uint64), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_debug_last_routes", i32, vp, vp, u32, P(u32))
     sig("trn_exec_matches", i32, vp, vp, u32, P(TrnMatches))
     sig("trn_debug_hits", i32, i32, vp, C.c_uint64, vp, C.c_uint64, vp, vp, u32, vp, vp, vp, C.c_uint64, P(C.c_uint64), C.c_char_p, C.c_size_t)
@@ -211,6 +214,7 @@ def lib() -> C.CDLL:
     sig("trn_percolate", i32, vp, vp, vp, u32, P(TrnPercolation))
     sig("trn_debug_percolator_plan", i32, vp, u32, u32, vp, vp, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     sig("trn_index_documents", i32, vp, i32, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
+    sig("trn_index_documents_payloads", i32, vp, i32, vp, vp, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
     sig("trn_segment_write", i32, C.c_char_p, i32, vp, u64, vp, u64, vp, vp, u32, u64, u32, u64, u32, vp, u64, C.c_char_p, C.c_size_t)
     sig("trn_merge_sources", i32, vp, i32, vp, u32, i32, P(TrnMerged))
     sig("trn_debug_merge_plan", i32, i32, vp, u32, i32, vp, vp, vp, vp, vp, vp, P(u32), P(u64), vp, vp, P(u64), P(u32), C.c_char_p, C.c_size_t)

@@ -212,6 +212,14 @@ struct EncParams {
         uint8_t *                 out;
         uint32_t *                error;     // != 0: an input the reference encoder throws on (docIDs not ascending / 0, positions decreasing or 0)
 };
+// the hits' payloads, beside positions[] (the encoders' payload instantiations only: the parameters of the others keep their layout)
+struct EncPayloads {
+        const uint8_t *           plens;    // per hit: payload bytes 0..8 (null: no payloads)
+        const unsigned long long *payloads; // per hit: the payload in the low plens[] bytes, memory order
+};
+struct EncPayloadParams : EncParams {
+        EncPayloads pay;
+};
 
 // device-side LUCENE encoder (encode_lucene.cuh).  A term's doc units are its full 128-document blocks followed by its tail (the
 // documents % 128 varbyte pairs, possibly none); its hit units are its full 128-hit blocks followed by its hit tail.  Every term has
@@ -233,6 +241,9 @@ struct EncLuceneParams {
         uint8_t *                 index_out;
         uint8_t *                 hits_out;
         uint32_t *                error; // != 0: docIDs not ascending / 0, positions decreasing / 0 / >= Limits::MaxPosition
+};
+struct EncLucenePayloadParams : EncLuceneParams {
+        EncPayloads pay;
 };
 
 // ---- the default exec mode (TRN_MODE_MATCHED_TERMS): which query terms a match holds (collect.cuh; planner.cpp plan_collect)
@@ -400,17 +411,20 @@ __host__ __device__ inline uint32_t index_term_at(uint32_t order, uint32_t nterm
                 ++b;
         return (((order - index_bucket_start(b, nterms)) + (b ? 0u : 1u)) << 5 | b) - 1u;
 }
-enum : uint32_t { IDX_ERR_DOC0, IDX_ERR_DUP, IDX_ERR_TOKEN, IDX_ERR_POS, IDX_ERR_POS0, IDX_ERR_FREQ, IDX_ERR_DOCTERMS, IDX_ERR_KINDS };
+enum : uint32_t { IDX_ERR_DOC0, IDX_ERR_DUP, IDX_ERR_TOKEN, IDX_ERR_POS, IDX_ERR_POS0, IDX_ERR_FREQ, IDX_ERR_DOCTERMS, IDX_ERR_PAYLEN, IDX_ERR_PAYDUP, IDX_ERR_KINDS };
 struct IndexParams {
         // the batch: document d = tokens[doc_off[d] .. doc_off[d + 1]), token i at positions[i] (null: at i - doc_off[d] + 1)
         const unsigned long long *doc_off;
         const uint32_t *          tokens;
         const uint32_t *          positions;
+        const uint8_t *           plens;    // per token: payload bytes 0..8; null: no payloads
+        const unsigned long long *payloads; // per token: the payload in the low plens[] bytes, memory order
         uint32_t                  ndocs, nterms;
         uint64_t                  ntokens;
         const uint32_t *          rank_of;  // per document ordinal: its rank in docID order
         const uint32_t *          docid_of; // per rank: the docID
         unsigned long long *      keys;     // per token: term_order << 40 | doc_rank << 14 | position
+        uint32_t *                ords;     // with payloads: per token its ordinal, the value the sort moves beside the key
         unsigned long long *      errors;   // IDX_ERR_KINDS slots
         // the postings pass over the sorted keys
         const uint32_t *          post_flag, *term_flag; // per token: opens a posting / a term
@@ -419,6 +433,8 @@ struct IndexParams {
         unsigned long long *      term_begin; // per present term + 1: its first posting
         uint32_t *                term_order; // per present term: its place in the encode order
         uint32_t *                out_docids, *out_freqs, *out_positions;
+        uint8_t *                 out_plens;    // with payloads: per hit, gathered through the sorted ordinals
+        unsigned long long *      out_payloads; // ... the payload, bytes past its length cleared
         uint32_t *                doc_terms;  // per rank: distinct terms (zeroed); null when nterms <= 65535 cannot exceed the limit
 };
 

@@ -1576,6 +1576,8 @@ struct DevPostings {
         uint32_t                  nterms;
         const unsigned long long *term_begin;
         const uint32_t *          docids, *freqs, *positions; // positions null: 1..freq
+        const uint8_t *           plens = nullptr;            // per hit: payload bytes (null: no payloads; needs positions)
+        const unsigned long long *payloads = nullptr;         // per hit: the payload in its low plens[] bytes
 };
 struct FreeBufs {
         std::vector<DevBuf *> v;
@@ -1638,7 +1640,7 @@ static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block
         CK(cudaEventRecord(e0, c->stream));
         if (positions)
                 CK(launch_enc_scan(P.freqs, nposts, d_part.as<unsigned long long>(), d_hb.as<unsigned long long>(), c->stream));
-        CK(launch_enc_google_sizes(E, c->stream));
+        CK(launch_enc_google_sizes(E, EncPayloads{P.plens, P.payloads}, c->stream));
         CK(launch_enc_scan(d_bsz.as<uint32_t>(), nblocks, d_part.as<unsigned long long>(), d_boff.as<unsigned long long>(), c->stream));
         CK(launch_enc_term_sizes(E, d_cb.as<unsigned long long>(), c->stream));
         CK(cudaEventRecord(e1, c->stream));
@@ -1650,7 +1652,9 @@ static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block
         CK(cudaMemcpyAsync(&herr, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         if (herr)
-                return fail(c, TRN_ERR_ARG, "google encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 and non-decreasing");
+                return fail(c, TRN_ERR_ARG, P.plens ? "google encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 (0 only with a payload) "
+                                                      "and non-decreasing, payloads of at most 8 bytes"
+                                                    : "google encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 and non-decreasing");
         uint64_t total{0};
         for (uint32_t t = 0; t < nterms; ++t) {
                 toff[t] = total;
@@ -1667,7 +1671,7 @@ static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block
         CK(cudaMemcpyAsync(d_toff.p, toff.data(), (size_t(nterms) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
         CK(cudaEventRecord(e2, c->stream));
         CK(cudaMemsetAsync(d_out.p, 0, std::max<size_t>(4, total), c->stream)); // a term without documents is its zero u16
-        CK(launch_enc_google_write(E, c->stream));
+        CK(launch_enc_google_write(E, EncPayloads{P.plens, P.payloads}, c->stream));
         CK(cudaEventRecord(e3, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         *nblocks_out = nblocks;
@@ -1681,14 +1685,17 @@ static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block
         return TRN_OK;
 }
 
-extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
-                                 uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
-                                 float *device_ms) {
+extern "C" int trn_encode_google_payloads(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs,
+                                          const uint32_t *positions, const uint8_t *payload_lens, const uint64_t *payloads, uint32_t block_docs,
+                                          uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
+                                          float *device_ms) {
         if (!c)
                 return TRN_ERR_ARG;
         if (!term_begin || !nterms || !out_bytes || !terms || block_docs == 0 || block_docs > 128 || skiplist_step == 0 ||
             (countdown && (*countdown == 0 || *countdown > skiplist_step)))
                 return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
+        if (!payload_lens != !payloads || (payload_lens && !positions))
+                return fail(c, TRN_ERR_ARG, "trn_encode_google_payloads: payload_lens and payloads are given together, and with positions");
         const uint64_t nposts = term_begin[nterms];
         if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
                 return fail(c, TRN_ERR_ARG, "trn_encode_google: bad arguments");
@@ -1716,7 +1723,21 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
                 if (nhits)
                         CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
         }
-        const DevPostings     P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), positions ? d_pos.as<uint32_t>() : nullptr};
+        DevBuf   d_pl, d_pv;
+        FreeBufs frp{{&d_pl, &d_pv}};
+        if (payload_lens) {
+                CK(d_pl.ensure(std::max<size_t>(4, nhits)));
+                CK(d_pv.ensure(std::max<size_t>(8, nhits * 8)));
+                if (nhits) {
+                        CK(cudaMemcpyAsync(d_pl.p, payload_lens, nhits, cudaMemcpyHostToDevice, c->stream));
+                        CK(cudaMemcpyAsync(d_pv.p, payloads, nhits * 8, cudaMemcpyHostToDevice, c->stream));
+                }
+        }
+        DevPostings P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), positions ? d_pos.as<uint32_t>() : nullptr};
+        if (payload_lens) {
+                P.plens    = d_pl.as<uint8_t>();
+                P.payloads = d_pv.as<unsigned long long>();
+        }
         std::vector<uint64_t> chunk, toff;
         uint64_t              nblocks{0};
         if (const int r = encode_google_device(c, P, block_docs, skiplist_step, phase0, out != nullptr, cap, out_bytes, d_out, chunk, toff, &nblocks, device_ms))
@@ -1731,6 +1752,13 @@ extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_
         if (countdown)
                 *countdown = skiplist_step - uint32_t((uint64_t(phase0) + nblocks) % skiplist_step);
         return TRN_OK;
+}
+
+extern "C" int trn_encode_google(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                                 uint32_t block_docs, uint32_t skiplist_step, uint32_t *countdown, uint8_t *out, uint64_t cap, uint64_t *out_bytes, trn_term *terms,
+                                 float *device_ms) {
+        return trn_encode_google_payloads(c, term_begin, nterms, docids, freqs, positions, nullptr, nullptr, block_docs, skiplist_step, countdown, out, cap, out_bytes,
+                                          terms, device_ms);
 }
 
 // =================================================================================================== device-side encoder (LUCENE)
@@ -1807,7 +1835,7 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         E.freqs       = P.freqs;
         E.positions   = nhits ? P.positions : nullptr;
         E.hit_begin   = d_hb.as<unsigned long long>();
-        E.dsz       = d_dsz.as<uint32_t>();
+        E.dsz         = d_dsz.as<uint32_t>();
         E.hsz         = d_hsz.as<uint32_t>();
         E.dterm       = d_dterm.as<uint32_t>();
         E.hterm       = d_hterm.as<uint32_t>();
@@ -1815,9 +1843,10 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         E.hoff        = d_hoff.as<unsigned long long>();
         E.term_off    = d_toff.as<unsigned long long>();
         E.error       = d_err.as<uint32_t>();
+        const EncPayloads pay{nhits ? P.plens : nullptr, nhits ? P.payloads : nullptr};
         // (2) sizes of every unit, their scans, the chunk and hits.data offsets of every term
         CK(cudaEventRecord(e0, c->stream));
-        CK(launch_enc_lucene_sizes(E, c->stream));
+        CK(launch_enc_lucene_sizes(E, pay, c->stream));
         CK(launch_enc_scan(d_dsz.as<uint32_t>(), ndunits, d_part.as<unsigned long long>(), d_doff.as<unsigned long long>(), c->stream));
         CK(launch_enc_scan(d_hsz.as<uint32_t>(), nhunits, d_part.as<unsigned long long>(), d_hoff.as<unsigned long long>(), c->stream));
         CK(launch_enc_lucene_terms(E, d_fx.as<unsigned long long>(), d_toff.as<unsigned long long>(), d_hto.as<unsigned long long>(), c->stream));
@@ -1832,7 +1861,9 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         CK(cudaEventElapsedTime(&a, e0, e1));
         ms += a;
         if (herr)
-                return fail(c, TRN_ERR_ARG, "lucene encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 and non-decreasing");
+                return fail(c, TRN_ERR_ARG, pay.plens ? "lucene encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 (0 only with a payload) "
+                                                      "and non-decreasing, payloads of at most 8 bytes"
+                                                    : "lucene encoder: document IDs must be > 0 and strictly ascending, positions in 1..16383 and non-decreasing");
         const uint64_t total = toff[nterms], htotal = hto[nterms];
         *index_bytes         = total;
         *hits_bytes          = htotal;
@@ -1846,7 +1877,7 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         E.hits_out  = d_hout.as<uint8_t>();
         // (3) the bytes: every byte of both outputs is written by exactly one unit's warp
         CK(cudaEventRecord(e0, c->stream));
-        CK(launch_enc_lucene_write(E, c->stream));
+        CK(launch_enc_lucene_write(E, pay, c->stream));
         CK(cudaEventRecord(e1, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         CK(cudaEventElapsedTime(&a, e0, e1));
@@ -1859,13 +1890,15 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         return TRN_OK;
 }
 
-extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
-                                 uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
-                                 trn_term *terms, float *device_ms) {
+extern "C" int trn_encode_lucene_payloads(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs,
+                                          const uint32_t *positions, const uint8_t *payload_lens, const uint64_t *payloads, uint8_t *index_out, uint64_t index_cap,
+                                          uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes, trn_term *terms, float *device_ms) {
         if (!c)
                 return TRN_ERR_ARG;
         if (!term_begin || !nterms || !index_bytes || !hits_bytes || !terms)
                 return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
+        if (!payload_lens != !payloads || (payload_lens && !positions))
+                return fail(c, TRN_ERR_ARG, "trn_encode_lucene_payloads: payload_lens and payloads are given together, and with positions");
         const uint64_t nposts = term_begin[nterms];
         if (term_begin[0] != 0 || (nposts && (!docids || !freqs)))
                 return fail(c, TRN_ERR_ARG, "trn_encode_lucene: bad arguments");
@@ -1892,7 +1925,17 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
                 CK(d_pos.ensure(nhits * 4));
                 CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
         }
-        const DevPostings     P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), nhits ? d_pos.as<uint32_t>() : nullptr};
+        DevBuf   d_pl, d_pv;
+        FreeBufs frp{{&d_pl, &d_pv}};
+        DevPostings P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), nhits ? d_pos.as<uint32_t>() : nullptr};
+        if (payload_lens && nhits) {
+                CK(d_pl.ensure(nhits));
+                CK(d_pv.ensure(nhits * 8));
+                CK(cudaMemcpyAsync(d_pl.p, payload_lens, nhits, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_pv.p, payloads, nhits * 8, cudaMemcpyHostToDevice, c->stream));
+                P.plens    = d_pl.as<uint8_t>();
+                P.payloads = d_pv.as<unsigned long long>();
+        }
         std::vector<uint64_t> toff;
         if (const int r = encode_lucene_device(c, P, index_out != nullptr, index_cap, index_bytes, hits_out != nullptr, hits_cap, hits_bytes, d_iout, d_hout, toff, device_ms))
                 return r;
@@ -1906,6 +1949,13 @@ extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_
                 terms[t].chunk_len = uint32_t(toff[t + 1] - toff[t]);
         }
         return TRN_OK;
+}
+
+extern "C" int trn_encode_lucene(trn_ctx *c, const uint64_t *term_begin, uint32_t nterms, const uint32_t *docids, const uint32_t *freqs, const uint32_t *positions,
+                                 uint8_t *index_out, uint64_t index_cap, uint64_t *index_bytes, uint8_t *hits_out, uint64_t hits_cap, uint64_t *hits_bytes,
+                                 trn_term *terms, float *device_ms) {
+        return trn_encode_lucene_payloads(c, term_begin, nterms, docids, freqs, positions, nullptr, nullptr, index_out, index_cap, index_bytes, hits_out, hits_cap,
+                                          hits_bytes, terms, device_ms);
 }
 
 // =================================================================================================== indexer
@@ -1954,9 +2004,10 @@ uint64_t low_bits_for(uint64_t maxv) { // mask of the bits the values 0 .. maxv 
                 }                                                                                                                                              \
         } while (0)
 
-// sorts n keys by the planned passes; the result is in *sorted (a or b).  No host synchronisation.
+// sorts n keys by the planned passes; the result is in *sorted (a or b).  va / vb (may be null): a u32 per key that moves with it, the
+// result in *vsorted.  No host synchronisation.
 static int index_radix_sort(trn_ctx *c, DevBuf &a, DevBuf &b, uint64_t n, const std::vector<IndexPass> &passes, DevBuf &counts, DevBuf &part, DevBuf &offs,
-                            unsigned long long **sorted) {
+                            unsigned long long **sorted, DevBuf *va = nullptr, DevBuf *vb = nullptr, uint32_t **vsorted = nullptr) {
         const uint64_t ntiles = (n + 4095) / 4096;
         uint32_t       maxbits{1};
         for (const auto &p : passes)
@@ -1966,21 +2017,29 @@ static int index_radix_sort(trn_ctx *c, DevBuf &a, DevBuf &b, uint64_t n, const 
         CKM(offs.ensure((ncounts + 1) * 8));
         CKM(part.ensure((ncounts / 4096 + 4) * 8));
         unsigned long long *in = a.as<unsigned long long>(), *out = b.as<unsigned long long>();
+        uint32_t *          vin = va ? va->as<uint32_t>() : nullptr, *vout = va ? vb->as<uint32_t>() : nullptr;
         for (const auto &p : passes) {
-                CK(launch_radix_pass(in, out, n, p.shift, p.bits, counts.as<uint32_t>(), part.as<unsigned long long>(), offs.as<unsigned long long>(), c->stream));
+                CK(launch_radix_pass(in, out, n, p.shift, p.bits, counts.as<uint32_t>(), part.as<unsigned long long>(), offs.as<unsigned long long>(), c->stream, vin,
+                                     vout));
                 std::swap(in, out);
+                std::swap(vin, vout);
         }
         *sorted = in;
+        if (vsorted)
+                *vsorted = vin;
         return TRN_OK;
 }
 
-extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
-                                   uint32_t ndocs, uint32_t nterms, trn_indexed *out) {
+extern "C" int trn_index_documents_payloads(trn_ctx *c, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens,
+                                            const uint32_t *positions, const uint8_t *payload_lens, const uint64_t *payloads, uint32_t ndocs, uint32_t nterms,
+                                            trn_indexed *out) {
         if (!c)
                 return TRN_ERR_ARG;
         const double t_begin = now_ms();
         if (!docids || !doc_offsets || !out || !ndocs || !nterms || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE) || doc_offsets[0] != 0)
                 return fail(c, TRN_ERR_ARG, "trn_index_documents: bad arguments");
+        if (!payload_lens != !payloads)
+                return fail(c, TRN_ERR_ARG, "trn_index_documents_payloads: payload_lens and payloads are given together");
         if (nterms > kIndexMaxTerms)
                 return fail(c, TRN_ERR_ARG, "trn_index_documents: " + std::to_string(nterms) + " terms: at most 2^24 per call");
         if (ndocs > kIndexMaxDocs)
@@ -2001,6 +2060,9 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         const uint64_t ntok = doc_offsets[ndocs];
         if (ntok && !tokens)
                 return fail(c, TRN_ERR_ARG, "trn_index_documents: bad arguments");
+        const bool with_payloads = payload_lens && ntok;
+        if (with_payloads && ntok > 0xffffffffull) // the ordinal the sort moves beside every key is a u32
+                return fail(c, TRN_ERR_CAPACITY, "trn_index_documents_payloads: " + std::to_string(ntok) + " tokens: at most 2^32 - 1 per call with payloads; split the batch");
         CK(cudaSetDevice(c->device));
         auto &X = c->ix;
         for (auto &e : X.ev)
@@ -2010,9 +2072,9 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         const auto who          = [&](uint32_t d) { return "trn_index_documents: document " + std::to_string(d) + " (docID " + std::to_string(docids[d]) + "): "; };
 
         DevBuf   d_docids, d_doff, d_tok, d_pos, d_ka, d_kb, d_rank, d_docid_of, d_err, d_counts, d_part, d_offs, d_pflag, d_tflag, d_pscan, d_tscan, d_pbegin, d_tb, d_order,
-            d_odoc, d_ofreq, d_opos, d_docterms, d_out, d_hout;
+            d_odoc, d_ofreq, d_opos, d_docterms, d_out, d_hout, d_pl, d_pv, d_va, d_vb, d_opl, d_opv;
         FreeBufs fr{{&d_docids, &d_doff, &d_tok, &d_pos, &d_ka, &d_kb, &d_rank, &d_docid_of, &d_err, &d_counts, &d_part, &d_offs, &d_pflag, &d_tflag, &d_pscan,
-                     &d_tscan, &d_pbegin, &d_tb, &d_order, &d_odoc, &d_ofreq, &d_opos, &d_docterms, &d_out, &d_hout}};
+                     &d_tscan, &d_pbegin, &d_tb, &d_order, &d_odoc, &d_ofreq, &d_opos, &d_docterms, &d_out, &d_hout, &d_pl, &d_pv, &d_va, &d_vb, &d_opl, &d_opv}};
         uint64_t herr[IDX_ERR_KINDS];
         // ---- documents: ranks in docID order, docID 0 and duplicates
         CKM(d_docids.ensure(size_t(ndocs) * 4));
@@ -2025,6 +2087,14 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         CKM(d_tok.ensure(std::max<uint64_t>(1, ntok) * 4));
         if (positions)
                 CKM(d_pos.ensure(std::max<uint64_t>(1, ntok) * 4));
+        if (with_payloads) {
+                CKM(d_pl.ensure(ntok));
+                CKM(d_pv.ensure(ntok * 8));
+                CKM(d_va.ensure(ntok * 4));
+                CKM(d_vb.ensure(ntok * 4));
+                CK(cudaMemcpyAsync(d_pl.p, payload_lens, ntok, cudaMemcpyHostToDevice, c->stream));
+                CK(cudaMemcpyAsync(d_pv.p, payloads, ntok * 8, cudaMemcpyHostToDevice, c->stream));
+        }
         CK(cudaMemcpyAsync(d_docids.p, docids, size_t(ndocs) * 4, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_doff.p, doc_offsets, (size_t(ndocs) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
         if (ntok) {
@@ -2047,6 +2117,9 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         P.doc_off   = d_doff.as<unsigned long long>();
         P.tokens    = d_tok.as<uint32_t>();
         P.positions = positions ? d_pos.as<uint32_t>() : nullptr;
+        P.plens     = with_payloads ? d_pl.as<uint8_t>() : nullptr;
+        P.payloads  = with_payloads ? d_pv.as<unsigned long long>() : nullptr;
+        P.ords      = with_payloads ? d_va.as<uint32_t>() : nullptr;
         P.ndocs     = ndocs;
         P.nterms    = nterms;
         P.ntokens   = ntok;
@@ -2055,7 +2128,9 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         P.keys      = d_ka.as<unsigned long long>();
         P.errors    = d_err.as<unsigned long long>();
         CK(launch_index_keys(P, c->stream));
-        if (const int r = index_radix_sort(c, d_ka, d_kb, ntok, key_passes, d_counts, d_part, d_offs, &sorted))
+        uint32_t *sorted_ords{nullptr};
+        if (const int r = index_radix_sort(c, d_ka, d_kb, ntok, key_passes, d_counts, d_part, d_offs, &sorted, with_payloads ? &d_va : nullptr,
+                                           with_payloads ? &d_vb : nullptr, &sorted_ords))
                 return r;
         CK(cudaEventRecord(X.ev[1], c->stream));
         // ---- postings: flags and their scans
@@ -2087,10 +2162,15 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
                 return fail(c, TRN_ERR_ARG, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) + " has position " +
                                                 std::to_string(positions ? positions[i] : 0u) + ": positions must be below 16384 (Limits::MaxPosition)");
         }
+        if (herr[IDX_ERR_PAYLEN] != ~0ull) {
+                const uint64_t i = herr[IDX_ERR_PAYLEN];
+                return fail(c, TRN_ERR_ARG, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) + " has a payload of " +
+                                                std::to_string(payload_lens[i]) + " bytes: at most 8 (indexer.cpp:26)");
+        }
         if (herr[IDX_ERR_POS0] != ~0ull) {
                 const uint64_t i = herr[IDX_ERR_POS0];
                 return fail(c, TRN_ERR_UNSUPPORTED, who(doc_of_token(i)) + "token " + std::to_string(i - doc_offsets[doc_of_token(i)]) +
-                                                        " has position 0: hits without a position are not indexed");
+                                                        " has position 0 and no payload: hits without a position are not indexed");
         }
         // ---- postings: docids, freqs, positions, term_begin in the layout the encode kernels read
         CKM(d_pbegin.ensure((nposts + 1) * 8));
@@ -2114,8 +2194,14 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         P.out_freqs     = d_ofreq.as<uint32_t>();
         P.out_positions = d_opos.as<uint32_t>();
         P.doc_terms     = nterms > 65535u ? d_docterms.as<uint32_t>() : nullptr;
+        if (with_payloads) {
+                CKM(d_opl.ensure(ntok));
+                CKM(d_opv.ensure(ntok * 8));
+                P.out_plens    = d_opl.as<uint8_t>();
+                P.out_payloads = d_opv.as<unsigned long long>();
+        }
         CK(cudaEventRecord(X.ev[3], c->stream));
-        CK(launch_post_write(P, sorted, c->stream));
+        CK(launch_post_write(P, sorted, sorted_ords, c->stream));
         CK(launch_post_freqs(P, nposts, c->stream));
         CK(cudaEventRecord(X.ev[4], c->stream));
         std::vector<uint64_t> h_tb(npresent + 1);
@@ -2138,12 +2224,21 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
                 CK(cudaMemcpy(&doc, d_docid_of.as<uint32_t>() + herr[IDX_ERR_DOCTERMS], 4, cudaMemcpyDeviceToHost));
                 return fail(c, TRN_ERR_ARG, "trn_index_documents: docID " + std::to_string(doc) + " holds more than 65535 distinct terms (a uint16_t count, indexer.cpp:49,111)");
         }
+        if (herr[IDX_ERR_PAYDUP] != ~0ull) {
+                unsigned long long k{0};
+                uint32_t           doc{0};
+                CK(cudaMemcpy(&k, sorted + herr[IDX_ERR_PAYDUP], 8, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(&doc, d_docid_of.as<uint32_t>() + ((k >> 14) & 0x3ffffffu), 4, cudaMemcpyDeviceToHost));
+                return fail(c, TRN_ERR_UNSUPPORTED, "trn_index_documents: docID " + std::to_string(doc) + " holds term " + std::to_string(index_term_at(uint32_t(k >> 40), nterms)) +
+                                                        " twice at position " + std::to_string(k & 16383u) +
+                                                        " with different payloads: the reference leaves their order undefined (indexer.cpp:55-57)");
+        }
         float sort_ms{0}, a_ms{0}, b_ms{0}, enc_ms{0};
         CK(cudaEventElapsedTime(&sort_ms, X.ev[0], X.ev[1]));
         CK(cudaEventElapsedTime(&a_ms, X.ev[1], X.ev[2]));
         CK(cudaEventElapsedTime(&b_ms, X.ev[3], X.ev[4]));
         for (DevBuf *b : {&d_docids, &d_doff, &d_tok, &d_pos, &d_ka, &d_kb, &d_rank, &d_docid_of, &d_counts, &d_part, &d_offs, &d_pflag, &d_tflag, &d_pscan, &d_tscan,
-                          &d_pbegin, &d_order, &d_docterms})
+                          &d_pbegin, &d_order, &d_docterms, &d_pl, &d_pv, &d_va, &d_vb})
                 b->release();
         // ---- encode the device-resident postings: terms in index order, the reference's geometry, a fresh session
         std::vector<uint8_t>  index, hits;
@@ -2151,8 +2246,12 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         std::vector<uint64_t> chunk, toff;
         uint64_t              index_bytes{0}, hits_bytes{0};
         if (npresent) {
-                const DevPostings DP{h_tb.data(), uint32_t(npresent), d_tb.as<unsigned long long>(), d_odoc.as<uint32_t>(), d_ofreq.as<uint32_t>(), d_opos.as<uint32_t>()};
-                int               r;
+                DevPostings DP{h_tb.data(), uint32_t(npresent), d_tb.as<unsigned long long>(), d_odoc.as<uint32_t>(), d_ofreq.as<uint32_t>(), d_opos.as<uint32_t>()};
+                if (with_payloads) {
+                        DP.plens    = d_opl.as<uint8_t>();
+                        DP.payloads = d_opv.as<unsigned long long>();
+                }
+                int r;
                 if (codec == TRN_CODEC_GOOGLE) {
                         uint64_t nblocks{0};
                         r = encode_google_device(c, DP, 32, 8, 0, true, ~0ull, &index_bytes, d_out, chunk, toff, &nblocks, &enc_ms);
@@ -2200,6 +2299,11 @@ extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids
         out->encode_ms      = enc_ms;
         out->total_ms       = float(now_ms() - t_begin);
         return TRN_OK;
+}
+
+extern "C" int trn_index_documents(trn_ctx *c, int codec, const uint32_t *docids, const uint64_t *doc_offsets, const uint32_t *tokens, const uint32_t *positions,
+                                   uint32_t ndocs, uint32_t nterms, trn_indexed *out) {
+        return trn_index_documents_payloads(c, codec, docids, doc_offsets, tokens, positions, nullptr, nullptr, ndocs, nterms, out);
 }
 
 // =================================================================================================== decode probe

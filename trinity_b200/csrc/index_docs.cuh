@@ -17,6 +17,10 @@
 //               shared memory and copies it out, so neighbouring threads write neighbouring keys of one digit run.
 //   postings    k_post_flags marks the tokens that open a posting / a term; two scans number them; k_post_write emits docids, the first hit
 //               of every posting, positions, term_begin and the terms' orders; k_post_freqs derives the freqs and checks the u16 limits.
+//   payloads    the key has no spare bit, so a call with payloads sorts a u32 token ordinal beside every key (the VALUES instantiation of
+//               k_radix_scatter; the keys-only passes are the ones a call without payloads runs) and k_post_write gathers every hit's
+//               payload size and bytes through it.  Equal keys with different payloads are refused: the reference orders them with an
+//               unstable sort (indexer.cpp:55-57).
 #pragma once
 
 static constexpr uint32_t kRadixTile    = 4096; // keys per CTA of the sort kernels (256 threads x 16)
@@ -66,7 +70,13 @@ __global__ void __launch_bounds__(256) k_index_keys(IndexParams P) {
                 P.keys[i] = 0;
                 return;
         }
-        if (pos == 0)
+        const uint32_t len = P.plens ? P.plens[i] : 0u;
+        if (P.plens) {
+                P.ords[i] = uint32_t(i);
+                if (len > 8u)
+                        atomicMin(P.errors + IDX_ERR_PAYLEN, (unsigned long long)i);
+        }
+        if (pos == 0 && len == 0) // a position-0 hit with a payload is written and counted (google_codec.cpp:42-45)
                 atomicMin(P.errors + IDX_ERR_POS0, (unsigned long long)i);
         else if (pos >= 16384u)
                 atomicMin(P.errors + IDX_ERR_POS, (unsigned long long)i);
@@ -91,8 +101,11 @@ __global__ void __launch_bounds__(kRadixThreads) k_radix_hist(const unsigned lon
                 counts[size_t(threadIdx.x) * ntiles + blockIdx.x] = s_h[threadIdx.x];
 }
 
+// VALUES: vin[] moves with the keys into vout[] (the keys' staging area holds the values once the keys are out)
+template <bool VALUES = false>
 __global__ void __launch_bounds__(kRadixThreads) k_radix_scatter(const unsigned long long *in, unsigned long long *out, uint64_t n, uint32_t shift, uint32_t mask,
-                                                                uint32_t ntiles, const unsigned long long *offsets /* scan of counts */) {
+                                                                uint32_t ntiles, const unsigned long long *offsets /* scan of counts */, const uint32_t *vin,
+                                                                uint32_t *vout) {
         constexpr uint32_t W = kRadixThreads / 32, ROUNDS = kRadixTile / kRadixThreads; // a warp owns ROUNDS x 32 consecutive keys of the tile
         __shared__ unsigned long long s_stage[kRadixTile];
         __shared__ unsigned long long s_gofs[256];
@@ -157,10 +170,41 @@ __global__ void __launch_bounds__(kRadixThreads) k_radix_scatter(const unsigned 
                 }
         }
         __syncthreads();
-        for (uint32_t s = threadIdx.x; s < cnt; s += kRadixThreads) {
-                const unsigned long long k = s_stage[s];
-                const uint32_t           d = uint32_t(k >> shift) & mask;
-                out[s_gofs[d] + (s - s_start[d])] = k;
+        if constexpr (!VALUES) {
+                for (uint32_t s = threadIdx.x; s < cnt; s += kRadixThreads) {
+                        const unsigned long long k = s_stage[s];
+                        const uint32_t           d = uint32_t(k >> shift) & mask;
+                        out[s_gofs[d] + (s - s_start[d])] = k;
+                }
+        } else {
+                uint64_t dst[ROUNDS]; // the place of staged entry threadIdx.x + r * kRadixThreads in out[]
+#pragma unroll
+                for (uint32_t r = 0; r < ROUNDS; ++r) {
+                        const uint32_t s = threadIdx.x + r * kRadixThreads;
+                        if (s < cnt) {
+                                const unsigned long long k = s_stage[s];
+                                const uint32_t           d = uint32_t(k >> shift) & mask;
+                                dst[r]                     = s_gofs[d] + (s - s_start[d]);
+                                out[dst[r]]                = k;
+                        }
+                }
+                __syncthreads();
+                uint32_t *s_val = reinterpret_cast<uint32_t *>(s_stage);
+#pragma unroll
+                for (uint32_t r = 0; r < ROUNDS; ++r) {
+                        const uint32_t j = warp * (ROUNDS * 32u) + r * 32u + lane;
+                        if (j < cnt) {
+                                const uint32_t d                             = uint32_t(key[r] >> shift) & mask;
+                                s_val[s_start[d] + s_wcnt[warp][d] + rnk[r]] = vin[base + j];
+                        }
+                }
+                __syncthreads();
+#pragma unroll
+                for (uint32_t r = 0; r < ROUNDS; ++r) {
+                        const uint32_t s = threadIdx.x + r * kRadixThreads;
+                        if (s < cnt)
+                                vout[dst[r]] = s_val[s];
+                }
         }
 }
 
@@ -174,7 +218,9 @@ __global__ void __launch_bounds__(256) k_post_flags(const unsigned long long *ke
         term_flag[i]     = !i || (k >> 40) != (p >> 40);
 }
 
-__global__ void __launch_bounds__(256) k_post_write(IndexParams P, const unsigned long long *keys) {
+// with payloads (P.out_plens): ords = the sorted token ordinals; errors[IDX_ERR_PAYDUP] = the lowest sorted token whose key equals its
+// predecessor's while its payload differs
+__global__ void __launch_bounds__(256) k_post_write(IndexParams P, const unsigned long long *keys, const uint32_t *ords) {
         const uint64_t i = uint64_t(blockIdx.x) * 256u + threadIdx.x;
         if (i > P.ntokens)
                 return;
@@ -185,6 +231,21 @@ __global__ void __launch_bounds__(256) k_post_write(IndexParams P, const unsigne
         }
         const uint64_t k = keys[i];
         P.out_positions[i] = uint32_t(k) & 16383u;
+        if (P.out_plens) {
+                const auto     payload_of = [&](uint32_t o, uint32_t &len) {
+                        len = P.plens[o];
+                        return len >= 8u ? P.payloads[o] : P.payloads[o] & ((1ull << (8u * len)) - 1ull);
+                };
+                uint32_t                 len;
+                const unsigned long long v = payload_of(ords[i], len);
+                P.out_plens[i]             = uint8_t(len);
+                P.out_payloads[i]          = v;
+                if (i && keys[i - 1] == k) {
+                        uint32_t plen;
+                        if (payload_of(ords[i - 1], plen) != v || plen != len)
+                                atomicMin(P.errors + IDX_ERR_PAYDUP, (unsigned long long)i);
+                }
+        }
         if (P.post_flag[i]) {
                 const uint64_t p    = P.post_scan[i];
                 const uint32_t rank = uint32_t(k >> 14) & 0x3ffffffu;
@@ -233,9 +294,10 @@ cudaError_t launch_index_keys(const IndexParams &P, cudaStream_t stream) {
         k_index_keys<<<unsigned((P.ntokens + 255u) / 256u), 256, 0, stream>>>(P);
         return cudaGetLastError();
 }
-// one pass of the sort: in -> out by the digit (key >> shift) & (2^bits - 1); counts: 2^bits x tiles u32, offsets: one more u64 than that
+// one pass of the sort: in -> out by the digit (key >> shift) & (2^bits - 1); counts: 2^bits x tiles u32, offsets: one more u64 than that.
+// vin / vout (both or neither): a u32 per key that moves with it
 cudaError_t launch_radix_pass(const unsigned long long *in, unsigned long long *out, uint64_t n, uint32_t shift, uint32_t bits, uint32_t *counts,
-                              unsigned long long *partials, unsigned long long *offsets, cudaStream_t stream) {
+                              unsigned long long *partials, unsigned long long *offsets, cudaStream_t stream, const uint32_t *vin, uint32_t *vout) {
         if (!n)
                 return cudaSuccess;
         const uint32_t ntiles = uint32_t((n + kRadixTile - 1) / kRadixTile), mask = (1u << bits) - 1u;
@@ -243,7 +305,10 @@ cudaError_t launch_radix_pass(const unsigned long long *in, unsigned long long *
         cudaError_t e = launch_enc_scan(counts, uint64_t(mask + 1u) * ntiles, partials, offsets, stream);
         if (e != cudaSuccess)
                 return e;
-        k_radix_scatter<<<ntiles, kRadixThreads, 0, stream>>>(in, out, n, shift, mask, ntiles, offsets);
+        if (vin)
+                k_radix_scatter<true><<<ntiles, kRadixThreads, 0, stream>>>(in, out, n, shift, mask, ntiles, offsets, vin, vout);
+        else
+                k_radix_scatter<<<ntiles, kRadixThreads, 0, stream>>>(in, out, n, shift, mask, ntiles, offsets, nullptr, nullptr);
         return cudaGetLastError();
 }
 cudaError_t launch_post_flags(const unsigned long long *keys, uint64_t n, uint32_t *post_flag, uint32_t *term_flag, cudaStream_t stream) {
@@ -252,8 +317,8 @@ cudaError_t launch_post_flags(const unsigned long long *keys, uint64_t n, uint32
         k_post_flags<<<unsigned((n + 255u) / 256u), 256, 0, stream>>>(keys, n, post_flag, term_flag);
         return cudaGetLastError();
 }
-cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *keys, cudaStream_t stream) {
-        k_post_write<<<unsigned((P.ntokens + 256u) / 256u), 256, 0, stream>>>(P, keys);
+cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *keys, const uint32_t *ords, cudaStream_t stream) {
+        k_post_write<<<unsigned((P.ntokens + 256u) / 256u), 256, 0, stream>>>(P, keys, ords);
         return cudaGetLastError();
 }
 cudaError_t launch_post_freqs(const IndexParams &P, uint64_t nposts, cudaStream_t stream) {

@@ -20,6 +20,7 @@
 #include "varbyte.h"
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 namespace trn {

@@ -34,15 +34,15 @@ cudaError_t launch_score_flat(const ScoreParams &S, int threads, int num_sms, cu
 cudaError_t launch_decode_stream(const DevIndex &ix, const DecUnit *units, const uint64_t *out_base, uint32_t total_units, uint32_t *docids, uint32_t *freqs,
                                  unsigned long long *sums, int num_sms, cudaStream_t stream);
 cudaError_t launch_enc_scan(const uint32_t *in, uint64_t n, unsigned long long *partials, unsigned long long *out, cudaStream_t stream);
-cudaError_t launch_enc_google_sizes(const EncParams &E, cudaStream_t stream);
+cudaError_t launch_enc_google_sizes(const EncParams &E, const EncPayloads &pay, cudaStream_t stream);
 cudaError_t launch_enc_term_sizes(const EncParams &E, unsigned long long *chunk_bytes, cudaStream_t stream);
-cudaError_t launch_enc_google_write(const EncParams &E, cudaStream_t stream);
+cudaError_t launch_enc_google_write(const EncParams &E, const EncPayloads &pay, cudaStream_t stream);
 cudaError_t launch_enc_lucene_term_hits(const unsigned long long *term_begin, const unsigned long long *hit_begin, uint32_t nterms, unsigned long long *term_hits,
                                         cudaStream_t stream);
-cudaError_t launch_enc_lucene_sizes(const EncLuceneParams &E, cudaStream_t stream);
+cudaError_t launch_enc_lucene_sizes(const EncLuceneParams &E, const EncPayloads &pay, cudaStream_t stream);
 cudaError_t launch_enc_lucene_terms(const EncLuceneParams &E, const unsigned long long *fixed, unsigned long long *term_off, unsigned long long *hits_off,
                                     cudaStream_t stream);
-cudaError_t launch_enc_lucene_write(const EncLuceneParams &E, cudaStream_t stream);
+cudaError_t launch_enc_lucene_write(const EncLuceneParams &E, const EncPayloads &pay, cudaStream_t stream);
 cudaError_t launch_collect_count(const CollectParams &P, cudaStream_t stream); // the default exec mode's collect pass (collect.cuh)
 cudaError_t launch_collect_write(const CollectParams &P, cudaStream_t stream);
 uint32_t    kernel_max_k();
@@ -61,9 +61,9 @@ cudaError_t launch_index_doc_ranks(const unsigned long long *keys, uint32_t ndoc
                                    cudaStream_t stream);
 cudaError_t launch_index_keys(const IndexParams &P, cudaStream_t stream);
 cudaError_t launch_radix_pass(const unsigned long long *in, unsigned long long *out, uint64_t n, uint32_t shift, uint32_t bits, uint32_t *counts,
-                              unsigned long long *partials, unsigned long long *offsets, cudaStream_t stream);
+                              unsigned long long *partials, unsigned long long *offsets, cudaStream_t stream, const uint32_t *vin = nullptr, uint32_t *vout = nullptr);
 cudaError_t launch_post_flags(const unsigned long long *keys, uint64_t n, uint32_t *post_flag, uint32_t *term_flag, cudaStream_t stream);
-cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *keys, cudaStream_t stream);
+cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *keys, const uint32_t *ords, cudaStream_t stream);
 cudaError_t launch_post_freqs(const IndexParams &P, uint64_t nposts, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
