@@ -41,19 +41,25 @@ QUERIES = ["t1 AND t2", "t1 AND t5", "t2 AND t6", "t1 AND t7", "t3 AND t4", "t4 
 @pytest.fixture
 def cand_cost():
     old = os.environ.get("TRN_CAND_COST")
-    yield lambda v: os.environ.__setitem__("TRN_CAND_COST", str(v))
+    yield lambda v: os.environ.pop("TRN_CAND_COST", None) if v is None else os.environ.__setitem__("TRN_CAND_COST", str(v))
     if old is None:
         os.environ.pop("TRN_CAND_COST", None)
     else:
         os.environ["TRN_CAND_COST"] = old
 
 
-@pytest.mark.parametrize("cost", [1, 450, 0], ids=["forced", "default", "off"])
+@pytest.mark.parametrize("cost", [1, None, 0], ids=["forced", "default", "off"])
 def test_candidate_conjunctions_match_reference(ref, cand_cost, cost):
-    cand_cost(cost)  # read by trn_create
+    cand_cost(cost)  # read by trn_create (unset: the planner's default crossover)
     p = Pair(ref, tb.CODEC_GOOGLE, make_lists(), NDOCS)
     plans = [p.plan(q) for q in QUERIES]
     res = p.gpu.exec_batch(plans, tb.MODE_DOCS_ONLY)
+    routes = list(p.gpu.last_routes())
+    assert routes == list(tb.debug_plan(tb.CODEC_GOOGLE, p.index, p.terms, plans, tb.MODE_DOCS_ONLY, max_docid=NDOCS)[0])
+    if cost == 0:
+        assert tb.ROUTE_CANDIDATE not in routes
+    else:  # every all-term AND of two known terms is candidate-driven when forced; at the default crossover only the sparse leads are
+        assert routes.count(tb.ROUTE_CANDIDATE) >= (17 if cost == 1 else 3), routes
     for i, q in enumerate(QUERIES):
         want, _ = p.ref.exec(q, False, NDOCS + 1)
         assert_same_docs(res.query(i)[0], want, f"[{q}] cost={cost}")
@@ -68,7 +74,7 @@ def test_candidate_conjunctions_match_reference(ref, cand_cost, cost):
         assert_same_docs(res.query(i)[0], want, f"[{q}] masked cost={cost}")
 
 
-@pytest.mark.parametrize("cost", [1, 900], ids=["forced", "default"])
+@pytest.mark.parametrize("cost", [1, None], ids=["forced", "default"])
 def test_candidate_driven_trees_match_reference(ref, cand_cost, cost):
     """every tree with 2..8 distinct terms one of which all matches must hold: lead candidates + membership probes + truth table"""
     cand_cost(cost)
@@ -77,6 +83,7 @@ def test_candidate_driven_trees_match_reference(ref, cand_cost, cost):
     qs = [(q, 0, 0) for q in TEMPLATES + EXTRA] + [(q, 8, 0) for q in OPTIONAL_QUERIES] + [(q, 16, m) for q, m in SOME_QUERIES]
     plans = [tb.parse_query(q, p.tdict, min_match=m or None) for q, _, m in qs]
     res = p.gpu.exec_batch(plans, tb.MODE_DOCS_ONLY)
+    assert (list(p.gpu.last_routes()).count(tb.ROUTE_CANDIDATE) >= 20) == (cost == 1)  # (the closed-form terms are too dense for the default)
     for i, (q, flags, m) in enumerate(qs):
         want, _ = p.ref.exec(q, False, ndocs + 1, parser_flags=flags, min_match=m)
         assert_same_docs(res.query(i)[0], want, f"[{q}] min={m} cost={cost}")
