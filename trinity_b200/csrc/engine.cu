@@ -96,7 +96,7 @@ struct trn_ctx {
         PlanConfig           pc; // the planner's view of the index, its knobs and the kernels' limits (trn_create, trn_upload_index)
         uint32_t             block_docs{32}; // documents per full block of the uploaded index (GOOGLE 32 unless built for the decode sweep; LUCENE 128)
         uint32_t             nterms{0}, ntiles{0}; // ntiles: of pc.tile_shift
-        int                  flat_threads{320}; // TRN_SF_THREADS: CTA size of k_score_flat (256/320/384: two CTAs per SM; 512/640: one)
+        int                  flat_threads{320}; // TRN_SF_THREADS: CTA size of k_score_flat (320: two CTAs per SM; 512: one; any other value runs 320)
         uint64_t             index_bytes{0}, dir_bytes{0}, total_blocks{0}, total_postings{0};
         DevBuf               d_index, d_blk_last, d_blk_off, d_terms, d_tile_first, d_masked;
         bool                 have_masked{false};
@@ -107,7 +107,7 @@ struct trn_ctx {
         std::vector<DevTerm> h_terms;
         // batch scratch (grow-only)
         DevBuf d_queries, d_steps, d_dense_runs, d_mixed_runs, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
-            d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_a, d_dec_b, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
+            d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
         PinBuf h_offsets, h_docids, h_scores, h_counts, h_small, h_chunk, h_item_desc;
         DevBuf d_hits, d_hit_base, d_hblk_off, d_hit_term; // LUCENE positions (trn_upload_hits)
         bool   have_hits{false};
@@ -322,7 +322,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         cudaSetDevice(c->device);
         for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
-                          &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_a, &c->d_dec_b, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
+                          &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores})
                 b->release();
         for (PinBuf *b : {&c->h_offsets, &c->h_docids, &c->h_scores, &c->h_counts, &c->h_small, &c->h_chunk, &c->h_item_desc})
@@ -2316,11 +2316,7 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
         if (!term_ids || !nterms || (materialise && (!docids || !freqs)))
                 return fail(c, TRN_ERR_ARG, "trn_decode_terms: bad arguments");
         CK(cudaSetDevice(c->device));
-        // TRN_DECODE_KERNEL=legacy | single-pass: the round-1 kernels (register-staged span copy / cp.async lane gather), kept for A/B runs;
-        // default: the bulk-copy streaming kernels of decode_stream.cuh
-        static const std::string decodeKernel = getenv("TRN_DECODE_KERNEL") ? getenv("TRN_DECODE_KERNEL") : "";
-        const bool               legacyDecode = (decodeKernel == "legacy" || decodeKernel == "single-pass") && c->block_docs == (c->pc.codec == TRN_CODEC_GOOGLE ? 32u : 128u);
-        std::vector<uint32_t> unit_base(nterms + 1);
+        std::vector<uint32_t> unit_base(nterms);
         std::vector<uint64_t> out_base(nterms + 1), host_base(nterms + 1);
         uint64_t              units{0}, posts{0}, padded{0};
         for (uint32_t i = 0; i < nterms; ++i) {
@@ -2330,16 +2326,15 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                 unit_base[i]  = uint32_t(units);
                 out_base[i]   = padded; // device rows start on a 128-entry boundary (16-byte vector stores)
                 host_base[i]  = posts;
-                units += (legacyDecode && c->pc.codec == TRN_CODEC_LUCENE) ? t.nblocks : (t.nblocks + 31) / 32;
+                units += (t.nblocks + 31) / 32;
                 posts += t.documents;
                 padded += (uint64_t(t.documents) + 127) / 128 * 128;
                 if (units >= (1ull << 32))
                         return fail(c, TRN_ERR_CAPACITY, "too many decode units");
         }
-        unit_base[nterms] = uint32_t(units);
         out_base[nterms]  = padded;
         host_base[nterms] = posts;
-        if (!legacyDecode) { // unit descriptors of the streaming kernels
+        { // unit descriptors of the streaming kernels (decode_stream.cuh)
                 std::vector<DecUnit> du(units);
                 const uint32_t       bd = c->block_docs;
                 for (uint32_t i = 0; i < nterms; ++i) {
@@ -2363,37 +2358,19 @@ extern "C" int trn_decode_terms(trn_ctx *c, const uint32_t *term_ids, uint32_t n
                         CK(cudaMemcpyAsync(c->d_dec_units.p, du.data(), du.size() * sizeof(DecUnit), cudaMemcpyHostToDevice, c->stream));
                 CK(cudaStreamSynchronize(c->stream)); // `du` leaves scope
         }
-        CK(c->d_dec_a.ensure(nterms * 4));
-        CK(c->d_dec_b.ensure((nterms + 1) * 4));
         CK(c->d_dec_c.ensure((nterms + 1) * 8));
         CK(c->d_dec_sums.ensure(size_t(nterms) * 16));
         if (materialise) {
                 CK(c->d_dec_docids.ensure(std::max<size_t>(16, padded * 4)));
                 CK(c->d_dec_freqs.ensure(std::max<size_t>(16, padded * 4)));
         }
-        CK(cudaMemcpyAsync(c->d_dec_a.p, term_ids, nterms * 4, cudaMemcpyHostToDevice, c->stream));
-        CK(cudaMemcpyAsync(c->d_dec_b.p, unit_base.data(), (nterms + 1) * 4, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(c->d_dec_c.p, out_base.data(), (nterms + 1) * 8, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemsetAsync(c->d_dec_sums.p, 0, size_t(nterms) * 16, c->stream));
         CK(cudaEventRecord(c->ev0, c->stream));
-        if (units) {
-                const int grid = int(std::min<uint64_t>(uint64_t(c->num_sms) * 8, (units + 3) / 4));
-                // GOOGLE: the materialising variant uses the single-pass kernel with 16-byte vector stores (k_decode_google); the fused
-                // checksum-only variant is faster with the span-staged kernel (scripts/microbench_decode.py compares the two)
-                const bool forceNew = decodeKernel == "single-pass";
-                if (!legacyDecode)
-                        CK(launch_decode_stream(dev_index(c), c->d_dec_units.as<DecUnit>(), c->d_dec_c.as<uint64_t>(), uint32_t(units),
-                                                materialise ? c->d_dec_docids.as<uint32_t>() : nullptr, materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr,
-                                                c->d_dec_sums.as<unsigned long long>(), c->num_sms, c->stream));
-                else if (c->pc.codec == TRN_CODEC_GOOGLE && (materialise || forceNew))
-                        CK(launch_decode_google(dev_index(c), c->d_dec_a.as<uint32_t>(), c->d_dec_b.as<uint32_t>(), c->d_dec_c.as<uint64_t>(), nterms,
-                                                uint32_t(units), materialise ? c->d_dec_docids.as<uint32_t>() : nullptr,
-                                                materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr, c->d_dec_sums.as<unsigned long long>(), grid, c->stream));
-                else
-                        CK(launch_decode_terms(dev_index(c), c->d_dec_a.as<uint32_t>(), c->d_dec_b.as<uint32_t>(), c->d_dec_c.as<uint64_t>(), nterms,
-                                               uint32_t(units), materialise ? c->d_dec_docids.as<uint32_t>() : nullptr,
-                                               materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr, c->d_dec_sums.as<unsigned long long>(), grid, c->stream));
-        }
+        if (units)
+                CK(launch_decode_stream(dev_index(c), c->d_dec_units.as<DecUnit>(), c->d_dec_c.as<uint64_t>(), uint32_t(units),
+                                        materialise ? c->d_dec_docids.as<uint32_t>() : nullptr, materialise ? c->d_dec_freqs.as<uint32_t>() : nullptr,
+                                        c->d_dec_sums.as<unsigned long long>(), c->num_sms, c->stream));
         CK(cudaEventRecord(c->ev1, c->stream));
         if (materialise && posts) {
                 for (uint32_t i = 0; i < nterms; ++i) {

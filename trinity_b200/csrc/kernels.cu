@@ -12,14 +12,12 @@
 //                  the order in which the reference calls MatchedIndexDocumentsFilter::consider() (exec.cpp:1215-1335).
 //   k_topk_select  per-query exact top-k (score desc, docID asc) over the per-tile candidates.
 //   k_topk_merge   merge of per-shard top-k lists after the all-gather (multi-GPU exchange step, SURVEY.md 8e).
-//   k_decode_terms whole-list decode (microbench + parity probe) == PostingsListIterator::next() over a list.
 #include "device_types.h"
 #include "dirlookup.h"
 #include "hitcursor.h"
 #include "kernels.h"
 #include "varbyte.h"
 #include <algorithm>
-#include <cstdlib>
 #include <type_traits>
 #include <cuda_runtime.h>
 
@@ -940,136 +938,6 @@ __global__ void __launch_bounds__(kThreads) k_topk_merge(const uint32_t *docids,
         }
 }
 
-// ------------------------------------------------------------------------------------------------ whole-list decode
-struct DecodeSink {
-        uint32_t *         docids; // may be null (checksum only)
-        uint32_t *         freqs;
-        unsigned long long sumd, sumf;
-        uint32_t           out_at; // output index of the NEXT visited posting of this lane (google: block base + i)
-        __device__ __forceinline__ void visit(uint32_t doc, uint32_t fr) {
-                if (docids) {
-                        docids[out_at] = doc;
-                        freqs[out_at]  = fr;
-                }
-                ++out_at;
-                sumd += doc;
-                sumf += fr;
-        }
-};
-
-// unit = 32 consecutive blocks (Google) or 1 block (Lucene), one warp per unit
-__global__ void __launch_bounds__(kThreads) k_decode_terms(DevIndex ix, const uint32_t *term_ids, const uint32_t *unit_base /*nterms+1*/, const uint64_t *out_base,
-                                                           uint32_t nterms, uint32_t total_units, uint32_t *docids, uint32_t *freqs, unsigned long long *sums) {
-        extern __shared__ __align__(16) uint8_t smem[];
-        const int                              lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        uint8_t *                              stage = smem + warp * kStageBytes;
-        for (uint32_t unit = blockIdx.x * kWarps + warp; unit < total_units; unit += gridDim.x * kWarps) {
-                uint32_t tlo = 0, thi = nterms;
-                while (thi - tlo > 1) {
-                        const uint32_t mid = (tlo + thi) >> 1;
-                        if (unit_base[mid] <= unit) tlo = mid;
-                        else thi = mid;
-                }
-                const uint32_t ti = tlo;
-                const DevTerm  T  = ix.terms[term_ids[ti]];
-                const uint32_t u  = unit - unit_base[ti];
-                const uint32_t *bl = ix.blk_last + T.dir_begin;
-                const uint32_t *bo = ix.blk_off + T.dir_begin;
-                DecodeSink      sink;
-                sink.docids = docids;
-                sink.freqs  = freqs;
-                sink.sumd = sink.sumf = 0;
-                if (ix.codec == 0) {
-                        const uint32_t g = u * 32u, b = g + lane;
-                        const bool     active = b < T.nblocks;
-                        uint32_t       off = 0, offn = 0, last = 0, prev = 0, n = 0;
-                        if (active) {
-                                off  = bo[b];
-                                offn = bo[b + 1];
-                                last = bl[b];
-                                prev = b ? bl[b - 1] : 0u;
-                                n    = (b + 1 == T.nblocks) ? (T.documents - 32u * (T.nblocks - 1u)) : 32u;
-                        }
-                        const uint32_t cnt       = min(32u, T.nblocks - g);
-                        const uint32_t first_off = __shfl_sync(0xffffffffu, off, 0);
-                        const uint32_t end_off   = __shfl_sync(0xffffffffu, offn, int(cnt) - 1);
-                        const uint32_t span      = end_off - first_off;
-                        sink.out_at              = uint32_t(0); // set below (64-bit base handled via pointer offset)
-                        uint32_t *dd = docids ? docids + out_base[ti] + size_t(b) * 32u : nullptr;
-                        uint32_t *ff = freqs ? freqs + out_base[ti] + size_t(b) * 32u : nullptr;
-                        sink.docids  = dd;
-                        sink.freqs   = ff;
-                        if (span + 32u <= kStageBytes) {
-                                const uint32_t skew = stage_copy(ix.index, first_off, span, stage, lane);
-                                __syncwarp();
-                                if (active)
-                                        google_block<true>(stage + skew + (off - first_off), n, prev, last, 0u, 0xffffffffu, sink);
-                        } else if (active)
-                                google_block<true>(ix.index + off, n, prev, last, 0u, 0xffffffffu, sink);
-                        __syncwarp();
-                } else {
-                        const uint32_t b = u, nfull = T.documents >> 7;
-                        const uint32_t off = bo[b], offn = bo[b + 1], prev = b ? bl[b - 1] : 0u, len = offn - off;
-                        uint32_t *     dd = docids ? docids + out_base[ti] + size_t(b) * 128u : nullptr;
-                        uint32_t *     ff = freqs ? freqs + out_base[ti] + size_t(b) * 128u : nullptr;
-                        if (b < nfull) {
-                                const uint32_t skew = stage_copy(ix.index, off, len, stage, lane);
-                                __syncwarp();
-                                uint32_t d[4], f[4];
-                                const uint32_t o2 = lucene_intblock(stage, skew, lane, d, reinterpret_cast<uint32_t *>(stage + 2560));
-                                (void)lucene_intblock(stage, o2, lane, f, reinterpret_cast<uint32_t *>(stage + 2560));
-                                d[1] += d[0];
-                                d[2] += d[1];
-                                d[3] += d[2];
-                                const uint32_t incl = warp_incl_scan(d[3], lane);
-                                const uint32_t base = prev + incl - d[3];
-#pragma unroll
-                                for (int t = 0; t < 4; ++t) {
-                                        const uint32_t doc = base + d[t];
-                                        if (dd) {
-                                                dd[lane * 4 + t] = doc;
-                                                ff[lane * 4 + t] = f[t];
-                                        }
-                                        sink.sumd += doc;
-                                        sink.sumf += f[t];
-                                }
-                        } else {
-                                const uint32_t tail = T.documents & 127u;
-                                const uint8_t *p;
-                                if (len + 32u <= kStageBytes) {
-                                        const uint32_t skew = stage_copy(ix.index, off, len, stage, lane);
-                                        __syncwarp();
-                                        p = stage + skew;
-                                } else
-                                        p = ix.index + off;
-                                if (lane == 0) {
-                                        sink.docids = dd;
-                                        sink.freqs  = ff;
-                                        sink.out_at = 0;
-                                        uint32_t doc = prev;
-                                        for (uint32_t i = 0; i < tail; ++i) {
-                                                doc += varbyte_get(p);
-                                                const uint32_t fr = varbyte_get(p);
-                                                sink.visit(doc, fr);
-                                        }
-                                }
-                        }
-                        __syncwarp();
-                }
-                // per-term checksums
-                unsigned long long sd = sink.sumd, sf = sink.sumf;
-                for (int d = 16; d > 0; d >>= 1) {
-                        sd += __shfl_xor_sync(0xffffffffu, sd, d);
-                        sf += __shfl_xor_sync(0xffffffffu, sf, d);
-                }
-                if (lane == 0 && sums) {
-                        atomicAdd(&sums[2 * ti], sd);
-                        atomicAdd(&sums[2 * ti + 1], sf);
-                }
-        }
-}
-
-#include "decode_google.cuh"
 #include "decode_stream.cuh"
 #include "encode_google.cuh"
 #include "encode_lucene.cuh"
@@ -1146,13 +1014,6 @@ cudaError_t launch_topk_select(const DevQuery *queries, uint32_t nq, const uint2
 cudaError_t launch_topk_merge(const uint32_t *docids, const float *scores, uint32_t nshards, uint32_t nq, uint32_t k, uint32_t *out_docids, float *out_scores,
                               cudaStream_t stream) {
         k_topk_merge<<<nq, kThreads, 0, stream>>>(docids, scores, nshards, nq, k, out_docids, out_scores);
-        return cudaGetLastError();
-}
-
-cudaError_t launch_decode_terms(const DevIndex &ix, const uint32_t *term_ids, const uint32_t *unit_base, const uint64_t *out_base, uint32_t nterms,
-                                uint32_t total_units, uint32_t *docids, uint32_t *freqs, unsigned long long *sums, int grid, cudaStream_t stream) {
-        const size_t smem = size_t(kWarps) * kStageBytes;
-        k_decode_terms<<<grid, kThreads, smem, stream>>>(ix, term_ids, unit_base, out_base, nterms, total_units, docids, freqs, sums);
         return cudaGetLastError();
 }
 

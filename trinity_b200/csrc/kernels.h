@@ -23,10 +23,6 @@ cudaError_t launch_topk_select(const DevQuery *queries, uint32_t nq, const uint2
                                float *out_scores, uint32_t *out_counts, cudaStream_t stream);
 cudaError_t launch_topk_merge(const uint32_t *docids, const float *scores, uint32_t nshards, uint32_t nq, uint32_t k, uint32_t *out_docids, float *out_scores,
                               cudaStream_t stream);
-cudaError_t launch_decode_terms(const DevIndex &ix, const uint32_t *term_ids, const uint32_t *unit_base, const uint64_t *out_base, uint32_t nterms,
-                                uint32_t total_units, uint32_t *docids, uint32_t *freqs, unsigned long long *sums, int grid, cudaStream_t stream);
-cudaError_t launch_decode_google(const DevIndex &ix, const uint32_t *term_ids, const uint32_t *unit_base, const uint64_t *out_base, uint32_t nterms,
-                                 uint32_t total_units, uint32_t *docids, uint32_t *freqs, unsigned long long *sums, int grid, cudaStream_t stream);
 size_t      score_flat_smem_bytes(uint32_t tile_shift, int threads);
 uint32_t    score_flat_max_leaves();
 cudaError_t launch_build_luts(const FlatLeaf *leaves, uint32_t nleaves, float *luts, cudaStream_t stream);

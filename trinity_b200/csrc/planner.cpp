@@ -937,11 +937,6 @@ extern "C" int trn_debug_compile(int codec, const uint8_t *index, uint64_t nbyte
 // =================================================================================================== batch planner
 PlanConfig trn::plan_config_from_env() {
         PlanConfig pc;
-        if (const char *e = getenv("TRN_TILE_SHIFT")) { // directory granularity == tile of the scored kernel (experiments)
-                const int v = atoi(e);
-                if (v >= 12 && v <= 14)
-                        pc.tile_shift = uint32_t(v);
-        }
         if (const char *e = getenv("TRN_CAND_COST"))
                 pc.cand_cost = std::max(0, atoi(e));
         if (const char *e = getenv("TRN_DOCS_SHIFT")) {

@@ -635,12 +635,11 @@ cudaError_t launch_build_luts(const FlatLeaf *leaves, uint32_t nleaves, float *l
         return cudaGetLastError();
 }
 
-// threads: CTA size (256 / 320: two CTAs per SM on 2^13-document tiles; 512 / 640: one CTA per SM, for 2^14-document tiles)
+// threads: CTA size (320: two CTAs per SM on 2^13-document tiles; 512: one CTA per SM, for 2^14-document tiles; any other value runs 320)
 cudaError_t launch_score_flat(const ScoreParams &S, int threads, int num_sms, cudaStream_t stream) {
-        const void *fn = threads == 320 ? (const void *)k_score_flat<320> : threads == 512 ? (const void *)k_score_flat<512>
-                                                                         : threads == 640 ? (const void *)k_score_flat<640> : (const void *)k_score_flat<256>;
-        if (threads != 320 && threads != 512 && threads != 640)
-                threads = 256;
+        if (threads != 512)
+                threads = 320;
+        const void *fn = threads == 512 ? (const void *)k_score_flat<512> : (const void *)k_score_flat<320>;
         const size_t smem = score_flat_smem_bytes(S.tile_shift, threads);
         cudaError_t  e    = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess)
