@@ -634,7 +634,12 @@ int trn_segment_write(const char *dir, int codec, const uint8_t *index, uint64_t
  * generations, a bad name or order, a tuple outside its source's bytes, a LUCENE source without hits.data, a malformed chunk;
  * TRN_ERR_UNSUPPORTED a hit with a payload, or at a position outside 1..16383, of a posting that is written re-encoded (appended chunks
  * keep their payloads; postings not written are never read); TRN_ERR_CAPACITY an output of 4 GiB or more, or
- * working memory that cannot be allocated.  n = 0: an empty result.  A refused call leaves the context as it was. */
+ * working memory that cannot be allocated.  n = 0: an empty result.  A refused call leaves the context as it was.
+ * trn_merge_sources_payloads: the same call, arguments, result and refusals, except that a re-encoded posting's hits are written with
+ * their payloads (new_hit(pos, {payload, len}), merge.cpp:221-232, 352-361: the low len bytes of the payload) and a hit at position 0
+ * WITH a payload is written and counts in sum_term_hits, as trn_index_documents_payloads writes it.  Its refusals of a written re-encoded
+ * posting: TRN_ERR_UNSUPPORTED a hit at position 0 without a payload, or above 16383; TRN_ERR_FORMAT a stored payload length above 8
+ * (a malformed source).  A merge none of whose written re-encoded hits carries a payload writes what trn_merge_sources writes. */
 #define TRN_MERGE_MAX_SOURCES 128
 typedef struct trn_merge_source {
         int                codec;
@@ -649,7 +654,7 @@ typedef struct trn_merge_source {
         const uint32_t *   updated_docids; /* replaced and erased documents of this generation, any order */
         uint64_t           nupdated;
 } trn_merge_source;
-typedef struct trn_merged { /* owned by the ctx, valid until the next trn_merge_sources */
+typedef struct trn_merged { /* owned by the ctx, valid until the next trn_merge_sources(_payloads) */
         const uint8_t * index;
         uint64_t        index_bytes;
         const uint8_t * hits; /* LUCENE hits.data */
@@ -666,6 +671,7 @@ typedef struct trn_merged { /* owned by the ctx, valid until the next trn_merge_
         float           total_ms;                                    /* host time of the whole call, copies included */
 } trn_merged;
 int trn_merge_sources(trn_ctx *, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out);
+int trn_merge_sources_payloads(trn_ctx *, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out);
 /* Host-only view of the merge planner (csrc/mergeplan.h; no GPU).  Arrays sized by the caller: order[n] = source of candidate i (newest
  * first); per output term k (at most Σ nterms): route[k] (0 append, 1 re-encode), stats[k] (1: its postings count toward sum_terms_docs /
  * sum_term_hits), parts [part_off[k], part_off[k + 1]) (nout + 1 offsets) of part_cand / part_term (candidate, term of that candidate's

@@ -837,13 +837,15 @@ class GpuIndexSource:
                                                           _ptr(pv) if len(pv) else None, len(d), nterms, C.byref(r)))
         return IndexedSegment(codec, r, d)
 
-    def merge_sources(self, out_codec: int, sources: Sequence["MergeSource"], disable_optimizations: bool = False) -> "MergedSegment":
+    def merge_sources(self, out_codec: int, sources: Sequence["MergeSource"], disable_optimizations: bool = False,
+                      payloads: bool = False) -> "MergedSegment":
         """== MergeCandidatesCollection commit() + merge() into a fresh IndexSession of out_codec (trn_merge_sources): the sources fold
-        newest generation first, each masked by the updated documents of the newer ones; the re-encoded terms run on the device"""
+        newest generation first, each masked by the updated documents of the newer ones; the re-encoded terms run on the device.
+        payloads=True (trn_merge_sources_payloads): re-encoded hits keep their payloads; without, such a hit is refused"""
         keep, arr = _merge_sources_c(sources)
         r = TrnMerged()
-        self._ck(self._L.trn_merge_sources(self._h, out_codec, C.cast(arr, C.c_void_p) if len(sources) else None, len(sources),
-                                           int(bool(disable_optimizations)), C.byref(r)))
+        f = self._L.trn_merge_sources_payloads if payloads else self._L.trn_merge_sources
+        self._ck(f(self._h, out_codec, C.cast(arr, C.c_void_p) if len(sources) else None, len(sources), int(bool(disable_optimizations)), C.byref(r)))
         del keep
         return MergedSegment(out_codec, r, sources)
 

@@ -25,7 +25,7 @@ EXPORTS = [
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
-    "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_debug_merge_plan",
+    "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_merge_sources_payloads", "trn_debug_merge_plan",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -217,6 +217,7 @@ def lib() -> C.CDLL:
     sig("trn_index_documents_payloads", i32, vp, i32, vp, vp, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
     sig("trn_segment_write", i32, C.c_char_p, i32, vp, u64, vp, u64, vp, vp, u32, u64, u32, u64, u32, vp, u64, C.c_char_p, C.c_size_t)
     sig("trn_merge_sources", i32, vp, i32, vp, u32, i32, P(TrnMerged))
+    sig("trn_merge_sources_payloads", i32, vp, i32, vp, u32, i32, P(TrnMerged))
     sig("trn_debug_merge_plan", i32, i32, vp, u32, i32, vp, vp, vp, vp, vp, vp, P(u32), P(u64), vp, vp, P(u64), P(u32), C.c_char_p, C.c_size_t)
     _lib = L
     return L

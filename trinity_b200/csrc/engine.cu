@@ -2880,13 +2880,15 @@ extern "C" int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, 
 
 // =================================================================================================== merge
 // == MergeCandidatesCollection::commit() + merge() (merge.cpp): the plan on the host (mergeplan.h), the postings on the device (merge.cuh),
-// the re-encoded terms through the device encoders in one call, the output assembled in output term order by one copy kernel.
+// the re-encoded terms through the device encoders in one call, the output assembled in output term order by one copy kernel.  One
+// implementation behind both entry points: trn_merge_sources refuses a payload hit it has to re-encode, trn_merge_sources_payloads writes
+// it (new_hit(pos, {payload, len}), merge.cpp:221-232, 352-361).
 #define CKMG(call)                                                                                                                                             \
         do {                                                                                                                                                   \
                 cudaError_t e__ = (call);                                                                                                                      \
                 if (e__ == cudaErrorMemoryAllocation) {                                                                                                        \
                         cudaGetLastError();                                                                                                                    \
-                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: working memory cannot be allocated on the device; merge fewer sources");        \
+                        return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": working memory cannot be allocated on the device; merge fewer sources");    \
                 }                                                                                                                                              \
                 if (e__ != cudaSuccess) {                                                                                                                      \
                         c->err = std::string(#call) + ": " + cudaGetErrorString(e__);                                                                          \
@@ -2894,18 +2896,23 @@ extern "C" int trn_debug_percolator_plan(const trn_query *queries, uint32_t nq, 
                 }                                                                                                                                              \
         } while (0)
 
-extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out) {
+static int merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out, bool payloads) {
         if (!c)
                 return TRN_ERR_ARG;
-        const double t_begin = now_ms();
+        const char *const fn      = payloads ? "trn_merge_sources_payloads" : "trn_merge_sources";
+        const double      t_begin = now_ms();
         if (!out)
-                return fail(c, TRN_ERR_ARG, "trn_merge_sources: bad arguments");
+                return fail(c, TRN_ERR_ARG, std::string(fn) + ": bad arguments");
         MergePlan   P;
         std::string perr;
-        if (const int r = plan_merge(out_codec, src, n, disable_optimizations != 0, P, perr))
+        if (const int r = plan_merge(out_codec, src, n, disable_optimizations != 0, P, perr)) {
+                const std::string planner_name = "trn_merge_sources"; // the name the planner's refusals start with
+                if (payloads && perr.rfind(planner_name + ":", 0) == 0)
+                        perr.replace(0, planner_name.size(), fn);
                 return fail(c, r, perr);
+        }
         const uint32_t nout = uint32_t(P.out.size() - 1);
-        const auto     who  = [&](uint32_t s) { return "trn_merge_sources: source " + std::to_string(s) + " (generation " + std::to_string(src[s].generation) + ")"; };
+        const auto     who  = [&](uint32_t s) { return std::string(fn) + ": source " + std::to_string(s) + " (generation " + std::to_string(src[s].generation) + ")"; };
         const auto     name = [&](uint32_t s, uint32_t t) { return who(s) + ", term [" + std::string(src[s].names[t]) + "]"; };
         CK(cudaSetDevice(c->device));
         auto &X = c->mg;
@@ -2973,10 +2980,11 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         re_first.push_back(nposts);
         // ---- upload: every used source's bytes and directories, one view per source
         DevBuf   d_idx, d_hits, d_bl, d_bo, d_tf, d_hb, d_hbo, d_ht, d_views, d_lists, d_lblk, d_lpost, d_ud, d_uf, d_doc, d_fr, d_hc, d_hoff, d_pos, d_keep, d_ks,
-            d_bm, d_part, d_odoc, d_ofr, d_osrc, d_ohoff, d_opos, d_err, d_cnt, d_idx2, d_tb, d_th, d_enc, d_henc, d_segs, d_oi, d_oh;
+            d_bm, d_part, d_odoc, d_ofr, d_osrc, d_ohoff, d_opos, d_err, d_cnt, d_idx2, d_tb, d_th, d_enc, d_henc, d_segs, d_oi, d_oh, d_pl, d_pv, d_opl, d_opv;
         FreeBufs fr{{&d_idx,  &d_hits, &d_bl,   &d_bo,   &d_tf,    &d_hb,   &d_hbo, &d_ht,  &d_views, &d_lists, &d_lblk, &d_lpost, &d_ud,
                      &d_uf,   &d_doc,  &d_fr,   &d_hc,   &d_hoff,  &d_pos,  &d_keep, &d_ks, &d_bm,    &d_part,  &d_odoc, &d_ofr,   &d_osrc,
-                     &d_ohoff, &d_opos, &d_err, &d_cnt, &d_idx2, &d_tb,  &d_th,  &d_enc, &d_henc,  &d_segs,  &d_oi,   &d_oh}};
+                     &d_ohoff, &d_opos, &d_err, &d_cnt, &d_idx2, &d_tb,  &d_th,  &d_enc, &d_henc,  &d_segs,  &d_oi,   &d_oh,  &d_pl,  &d_pv,
+                     &d_opl,   &d_opv}};
         std::vector<uint64_t> ibase(n + 1, 0), hbase(n + 1, 0), dbase(n + 1, 0), tbase(n + 1, 0), hbbase(n + 1, 0), termbase(n + 1, 0);
         for (uint32_t s = 0; s < n; ++s) {
                 const bool u = used[s];
@@ -3045,7 +3053,7 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         CKMG(d_ks.ensure((nposts + 1) * 8));
         CKMG(d_part.ensure((nposts / 4096 + 4) * 8));
         CKMG(d_bm.ensure(nwords * 4));
-        CKMG(d_err.ensure(16));
+        CKMG(d_err.ensure(24));
         CKMG(d_cnt.ensure(8));
         CKMG(d_idx2.ensure((size_t(nre) + 1) * 8));
         CKMG(d_tb.ensure((size_t(nre) + 1) * 8));
@@ -3061,7 +3069,7 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         }
         CK(cudaMemcpyAsync(d_idx2.p, re_first.data(), (size_t(nre) + 1) * 8, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemsetAsync(d_bm.p, 0, nwords * 4, c->stream));
-        CK(cudaMemsetAsync(d_err.p, 0xff, 16, c->stream));
+        CK(cudaMemsetAsync(d_err.p, 0xff, 24, c->stream));
         CK(cudaMemsetAsync(d_cnt.p, 0, 8, c->stream));
         MergeParams M{};
         M.views     = d_views.as<HitsView>();
@@ -3083,8 +3091,8 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         M.kscan     = d_ks.as<unsigned long long>();
         M.error     = d_err.as<unsigned long long>();
         // ---- decode docIDs and freqs of every list; keep (which also drops the hits of every posting that is not written); the hits of
-        // the kept postings
-        uint64_t nhits{0}, nkept{0}, herr2[2]{~0ull, ~0ull}, docs_cnt{0};
+        // the kept postings, and again with their payloads when one of them carries one and the call takes them
+        uint64_t nhits{0}, nkept{0}, herr[3]{~0ull, ~0ull, ~0ull}, docs_cnt{0};
         float    dec_ms{0}, m1{0}, m2{0}, d2{0}, enc_ms{0}, asm_ms{0};
         CK(cudaEventRecord(X.ev[0], c->stream));
         CK(launch_merge_decode(M, c->stream));
@@ -3099,25 +3107,47 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         CK(cudaStreamSynchronize(c->stream));
         CKMG(d_pos.ensure(std::max<uint64_t>(4, nhits * 4)));
         M.positions = d_pos.as<uint32_t>();
-        CK(launch_merge_hits_decode(M, c->stream));
+        CK(launch_merge_hits_decode(M, false, c->stream));
         CK(cudaEventRecord(X.ev[3], c->stream));
         std::vector<uint64_t> h_tb(size_t(nre) + 1), h_th(size_t(nre) + 1);
         CK(cudaMemcpyAsync(h_tb.data(), d_tb.p, (size_t(nre) + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaMemcpyAsync(herr2, d_err.p, 16, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(herr, d_err.p, 24, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaMemcpyAsync(&docs_cnt, d_cnt.p, 8, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         CK(cudaEventElapsedTime(&dec_ms, X.ev[0], X.ev[1]));
         CK(cudaEventElapsedTime(&m1, X.ev[1], X.ev[2]));
         CK(cudaEventElapsedTime(&d2, X.ev[2], X.ev[3]));
         dec_ms += d2;
-        for (int k = 0; k < 2; ++k)
-                if (herr2[k] != ~0ull) {
-                        const uint32_t   l = uint32_t(std::upper_bound(list_post.begin(), list_post.end(), herr2[k]) - list_post.begin()) - 1u;
-                        const MergeList &L = lists[l];
+        const auto posting_name = [&](uint64_t i) {
+                const MergeList &L = lists[uint32_t(std::upper_bound(list_post.begin(), list_post.end(), i) - list_post.begin()) - 1u];
+                return name(L.view, L.term);
+        };
+        if (!payloads) {
+                if (herr[0] != ~0ull)
+                        return fail(c, TRN_ERR_UNSUPPORTED, posting_name(herr[0]) + ": a hit with a payload must be re-encoded; the device encoders write no payloads");
+                if (herr[1] != ~0ull)
                         return fail(c, TRN_ERR_UNSUPPORTED,
-                                    name(L.view, L.term) + (k == 0 ? ": a hit with a payload must be re-encoded; the device encoders write no payloads"
-                                                                   : ": a hit at position 0 or above 16383 must be re-encoded; the device encoders take positions 1..16383"));
-                }
+                                    posting_name(herr[1]) + ": a hit at position 0 or above 16383 must be re-encoded; the device encoders take positions 1..16383");
+        } else {
+                if (herr[2] != ~0ull)
+                        return fail(c, TRN_ERR_FORMAT, posting_name(herr[2]) + ": a hit stores a payload of more than 8 bytes (a payload is a u64)");
+                if (herr[1] != ~0ull)
+                        return fail(c, TRN_ERR_UNSUPPORTED, posting_name(herr[1]) + ": a hit at position 0 without a payload, or above 16383, must be re-encoded; "
+                                                                                     "the device encoders take positions 1..16383 (0 with a payload)");
+        }
+        const bool with_payloads = payloads && herr[0] != ~0ull;
+        if (with_payloads) {
+                CKMG(d_pl.ensure(std::max<uint64_t>(4, nhits)));
+                CKMG(d_pv.ensure(std::max<uint64_t>(8, nhits * 8)));
+                M.plens = d_pl.as<uint8_t>();
+                M.pays  = d_pv.as<unsigned long long>();
+                CK(cudaEventRecord(X.ev[6], c->stream));
+                CK(launch_merge_hits_decode(M, true, c->stream));
+                CK(cudaEventRecord(X.ev[7], c->stream));
+                CK(cudaStreamSynchronize(c->stream));
+                CK(cudaEventElapsedTime(&d2, X.ev[6], X.ev[7]));
+                dec_ms += d2;
+        }
         nkept = h_tb[nre];
         CKMG(d_odoc.ensure(std::max<uint64_t>(4, nkept * 4)));
         CKMG(d_ofr.ensure(std::max<uint64_t>(4, nkept * 4)));
@@ -3136,17 +3166,27 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         CK(cudaStreamSynchronize(c->stream));
         CKMG(d_opos.ensure(std::max<uint64_t>(4, h_th[nre] * 4)));
         M.out_positions = d_opos.as<uint32_t>();
-        CK(launch_merge_out_hits(M, nkept, c->stream));
+        if (with_payloads) {
+                CKMG(d_opl.ensure(std::max<uint64_t>(4, h_th[nre])));
+                CKMG(d_opv.ensure(std::max<uint64_t>(8, h_th[nre] * 8)));
+                M.out_plens = d_opl.as<uint8_t>();
+                M.out_pays  = d_opv.as<unsigned long long>();
+        }
+        CK(launch_merge_out_hits(M, nkept, with_payloads, c->stream));
         CK(cudaEventRecord(X.ev[5], c->stream));
         CK(cudaStreamSynchronize(c->stream));
         CK(cudaEventElapsedTime(&m2, X.ev[4], X.ev[5]));
-        for (DevBuf *b : {&d_fr, &d_hc, &d_hoff, &d_pos, &d_keep, &d_ks, &d_bm, &d_osrc, &d_lists, &d_lblk, &d_lpost, &d_ud, &d_uf})
+        for (DevBuf *b : {&d_fr, &d_hc, &d_hoff, &d_pos, &d_keep, &d_ks, &d_bm, &d_osrc, &d_lists, &d_lblk, &d_lpost, &d_ud, &d_uf, &d_pl, &d_pv})
                 b->release();
         // ---- encode every re-encoded term in one call (orphans included: their headers are part of the output)
         std::vector<uint64_t> chunk, toff, hto;
         uint64_t              enc_bytes{0}, enc_hbytes{0};
         if (nre) {
-                const DevPostings DP{h_tb.data(), nre, d_tb.as<unsigned long long>(), M.out_docids, M.out_freqs, M.out_positions};
+                DevPostings DP{h_tb.data(), nre, d_tb.as<unsigned long long>(), M.out_docids, M.out_freqs, M.out_positions};
+                if (with_payloads) {
+                        DP.plens    = M.out_plens;
+                        DP.payloads = M.out_pays;
+                }
                 int               r;
                 if (out_codec == TRN_CODEC_GOOGLE) {
                         uint64_t nb{0};
@@ -3155,13 +3195,13 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
                 } else
                         r = encode_lucene_device(c, DP, true, ~0ull, &enc_bytes, true, ~0ull, &enc_hbytes, d_enc, d_henc, toff, &enc_ms, &hto);
                 if (r == TRN_ERR_CUDA && c->err.find("out of memory") != std::string::npos)
-                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: working memory cannot be allocated on the device; merge fewer sources");
+                        return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": working memory cannot be allocated on the device; merge fewer sources");
                 if (r == TRN_ERR_ARG || r == TRN_ERR_CAPACITY) { // the encoder's refusal, for the re-encoded terms as a whole: name the first
                         uint32_t k = 0;
                         while (P.out[k].route != MERGE_REENCODE)
                                 ++k;
                         const MergePart &p0 = P.parts[P.out[k].part_begin];
-                        return fail(c, r, "trn_merge_sources: re-encoding the merged terms (the first [" + std::string(src[P.order[p0.cand]].names[p0.term]) +
+                        return fail(c, r, std::string(fn) + ": re-encoding the merged terms (the first [" + std::string(src[P.order[p0.cand]].names[p0.term]) +
                                                   "] of " + who(P.order[p0.cand]) + "): " + c->err);
                 }
                 if (r)
@@ -3215,7 +3255,7 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
                                 ++orphaned;
                 }
                 if (ho >= (1ull << 32))
-                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
+                        return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
                 // a CTA per piece of at most kPiece bytes, so a long chunk is copied by many CTAs
                 constexpr uint64_t kPiece = 1u << 16;
                 for (uint64_t a = 0; a < len || a == 0; a += kPiece)
@@ -3230,16 +3270,16 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
                 io += len;
                 ho += hlen;
                 if (io >= (1ull << 32))
-                        return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged index reaches 4 GiB (range32_t chunk offsets)");
+                        return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": the merged index reaches 4 GiB (range32_t chunk offsets)");
         }
         if (ho >= (1ull << 32))
-                return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
+                return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": the merged hits.data reaches 4 GiB (u32 hitsDataOffset)");
         std::vector<uint8_t> index, hits;
         try {
                 index.resize(io);
                 hits.resize(ho);
         } catch (const std::bad_alloc &) {
-                return fail(c, TRN_ERR_CAPACITY, "trn_merge_sources: the result cannot be allocated on the host");
+                return fail(c, TRN_ERR_CAPACITY, std::string(fn) + ": the result cannot be allocated on the host");
         }
         CKMG(d_segs.ensure(std::max<size_t>(1, segs.size()) * sizeof(MergeCopy)));
         CKMG(d_oi.ensure(std::max<uint64_t>(4, io)));
@@ -3285,6 +3325,14 @@ extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_sour
         out->total_ms         = float(now_ms() - t_begin);
         c->have_kernel_events = false;
         return TRN_OK;
+}
+
+extern "C" int trn_merge_sources_payloads(trn_ctx *c, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out) {
+        return merge_sources(c, out_codec, src, n, disable_optimizations, out, true);
+}
+
+extern "C" int trn_merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, trn_merged *out) {
+        return merge_sources(c, out_codec, src, n, disable_optimizations, out, false);
 }
 
 extern "C" int trn_debug_merge_plan(int out_codec, const trn_merge_source *src, uint32_t n, int disable_optimizations, uint32_t *order, uint8_t *route,

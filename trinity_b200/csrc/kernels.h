@@ -63,7 +63,7 @@ cudaError_t launch_post_write(const IndexParams &P, const unsigned long long *ke
 cudaError_t launch_post_freqs(const IndexParams &P, uint64_t nposts, cudaStream_t stream);
 cudaError_t launch_build_dense(const DevIndex &ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel, uint64_t total_blocks,
                                uint32_t *dense, cudaStream_t stream);
-// merge (merge.cuh): the device half of trn_merge_sources
+// merge (merge.cuh): the device half of trn_merge_sources / trn_merge_sources_payloads
 struct MergeList { // one participant list of an output term (lists of one term are consecutive, newest first)
         DevTerm  t;        // the term in its source's block directory
         uint32_t view;     // its source's entry in MergeParams::views
@@ -82,14 +82,19 @@ struct MergeParams {
         uint32_t *                docids, *freqs, *hcount; // decoded postings; hcount = freq of a re-encoded posting, else 0
         const unsigned long long *hoff;                    // scan of hcount
         uint32_t *                positions;
+        uint8_t *                 plens;  // per decoded hit, only when a kept hit carries a payload and the call takes them: its length
+        unsigned long long *      pays;   // and its payload, masked to the low plens[] bytes
         const uint32_t *          upd_docid, *upd_first;
         unsigned long long        nupd;
         uint32_t *                keep, *bitmap;
         const unsigned long long *kscan;
         uint32_t *                out_docids, *out_freqs, *out_positions;
+        uint8_t *                 out_plens;  // plens / pays in the output order (with them only)
+        unsigned long long *      out_pays;
         unsigned long long *      out_src;
         const unsigned long long *out_hoff;
-        unsigned long long *      error; // first kept posting with [0] a payload hit, [1] a position outside 1..16383 (~0: none)
+        unsigned long long *      error; // first kept posting with [0] a payload hit, [1] a hit at position 0 without a payload or above 16383,
+                                         // [2] a payload length above 8 (~0: none)
 };
 struct MergeCopy {
         const uint8_t *    src;
@@ -97,10 +102,10 @@ struct MergeCopy {
         uint32_t           to_hits, header, hits_off; // header: a LUCENE index chunk whose first u32 becomes hits_off
 };
 cudaError_t launch_merge_decode(const MergeParams &P, cudaStream_t stream);
-cudaError_t launch_merge_hits_decode(const MergeParams &P, cudaStream_t stream);
+cudaError_t launch_merge_hits_decode(const MergeParams &P, bool payloads, cudaStream_t stream); // payloads: also fill plens / pays
 cudaError_t launch_merge_keep(const MergeParams &P, cudaStream_t stream);
 cudaError_t launch_merge_scatter(const MergeParams &P, cudaStream_t stream);
-cudaError_t launch_merge_out_hits(const MergeParams &P, uint64_t nout, cudaStream_t stream);
+cudaError_t launch_merge_out_hits(const MergeParams &P, uint64_t nout, bool payloads, cudaStream_t stream); // payloads: also out_plens / out_pays
 cudaError_t launch_merge_gather(const unsigned long long *a, const unsigned long long *idx, uint32_t n, unsigned long long *out, cudaStream_t stream);
 cudaError_t launch_merge_popcount(const uint32_t *bitmap, uint64_t nwords, unsigned long long *count, cudaStream_t stream);
 cudaError_t launch_merge_assemble(const MergeCopy *segs, uint32_t nsegs, uint8_t *index_out, uint8_t *hits_out, cudaStream_t stream);

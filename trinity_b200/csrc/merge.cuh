@@ -1,13 +1,19 @@
-// trn_merge_sources on the device (included by kernels.cu): the postings of every merged term are decoded from the sources' own bytes,
-// the postings the reference's merge() writes are kept and ranked without a sort, and the survivors are scattered into the term-major
-// layout the device encoders read.  One thread per block (decode), per posting (hits, keep, rank) or per output posting (hits scatter);
-// every list is read through the load-time block / hits directories of its source (MergeParams::views), so a thread starts anywhere.
+// trn_merge_sources / trn_merge_sources_payloads on the device (included by kernels.cu): the postings of every merged term are decoded from
+// the sources' own bytes, the postings the reference's merge() writes are kept and ranked without a sort, and the survivors are scattered
+// into the term-major layout the device encoders read.  One thread per block (decode), per posting (hits, keep, rank) or per output posting
+// (hits scatter); every list is read through the load-time block / hits directories of its source (MergeParams::views), so a thread starts
+// anywhere.
 //
 // Keep and rank (the newest holder of a docID decides, merge.cpp:333-365 / google_codec.cpp IndexSession::merge): posting (p, d) of a
 // re-encoded term is kept iff no newer participant of the term holds d (binary search in its decoded docIDs) and d is not in p's
 // registry (binary search in the sorted updated docIDs; masked iff the newest candidate listing d is newer than p).  With kscan the
 // exclusive scan of the keep flags, its output rank is its kept rank in its own list + the kept postings below d of every other
 // participant: the kept docIDs of one term are distinct, so the ranks are a permutation — a k-way merge without a sort.
+//
+// Payloads (materialize_hits + new_hit(pos, {payload, len}), merge.cpp:221-232, 352-361): the positions pass records whether a kept hit
+// carries one.  Only then, and only when the call takes payloads, a per-hit length and payload array is allocated beside the positions and
+// the PAYLOADS form of the same pass fills all three; k_merge_hits<true> carries them to the output order and the encoders' payload
+// instantiations write them.  A merge without payload hits runs the payload-free forms and allocates nothing more.
 
 __device__ __forceinline__ uint32_t mg_list_of(const unsigned long long *begin, uint32_t n, unsigned long long i) { // last l with begin[l] <= i
         uint32_t lo = 0, hi = n;
@@ -106,8 +112,14 @@ __global__ void __launch_bounds__(kThreads) k_merge_decode_blocks(MergeParams P)
 }
 
 // one thread per KEPT posting of a re-encoded list (k_merge_keep zeroes hcount of the others): its positions (hitcursor.h HitWalker, the
-// reader the exec paths use) at hoff[i]; a hit with a payload (error[0]) or a position outside 1..16383 (error[1]) is recorded: the
-// device encoders write neither.  Postings that are not written are never looked at, as merge() never materialises their hits.
+// reader the exec paths use) at hoff[i].  Recorded, as the first such posting: error[0] a hit with a payload (whether the PAYLOADS pass
+// runs; trn_merge_sources refuses it), error[1] a hit at position 0 without a payload or above 16383 (the encoders take neither),
+// error[2] a stored payload length above 8 (a malformed source: the reference's payload is a u64).  PAYLOADS also writes each hit's
+// length to plens and its payload to pays, masked to the low `len` bytes: a GOOGLE walker keeps the high bytes of an earlier, longer
+// payload of the same document (materialize_hits), and the arrays hold what a reader hands back.  Postings that are not written are never
+// looked at, as merge() never materialises their hits; a LUCENE walker that starts inside a 128-hit block skips the payload bytes of the
+// block's earlier hits by their lengths (HitWalker::lucene_block), so the bytes of a masked or older posting there are never read either.
+template <bool PAYLOADS>
 __global__ void __launch_bounds__(kThreads) k_merge_decode_hits(MergeParams P) {
         const unsigned long long i = blockIdx.x * (unsigned long long)kThreads + threadIdx.x;
         if (i >= P.nposts || !P.hcount[i])
@@ -117,18 +129,25 @@ __global__ void __launch_bounds__(kThreads) k_merge_decode_hits(MergeParams P) {
         w.init(P.views[L.view], mg_term(L), P.docids[i]);
         const uint32_t   f = P.hcount[i];
         uint32_t        *o = P.positions + P.hoff[i];
-        uint32_t any = 0, bad = 0; // flags tested after the loop: an atomic inside it costs a spill
+        uint32_t any = 0, bad = 0, big = 0; // flags tested after the loop: an atomic inside it costs a spill
         for (uint32_t h = 0; h < f; ++h) {
                 uint32_t len;
                 const uint32_t pos = w.next(len);
                 o[h] = pos;
+                if constexpr (PAYLOADS) {
+                        P.plens[P.hoff[i] + h] = uint8_t(len);
+                        P.pays[P.hoff[i] + h]  = len >= 8u ? w.payload : w.payload & ((1ull << (8u * len)) - 1ull);
+                }
                 any |= len;
-                bad |= pos == 0u || pos > 16383u;
+                bad |= (pos == 0u && !len) || pos > 16383u;
+                big |= len > 8u;
         }
         if (any)
                 atomicMin(P.error, i);
         if (bad)
                 atomicMin(P.error + 1, i);
+        if (big)
+                atomicMin(P.error + 2, i);
 }
 
 // one thread per posting (before the hits are decoded): keep flag (re-encoded lists) and the docs_cnt bitmap (every output posting, appended ones included)
@@ -177,7 +196,9 @@ __global__ void __launch_bounds__(kThreads) k_merge_scatter(MergeParams P) {
         P.out_src[r]    = i;
 }
 
-// one thread per output posting: its positions from the decoded hits (out_hoff = the scan of the output freqs)
+// one thread per output posting: its positions (PAYLOADS: and their lengths and payloads) from the decoded hits (out_hoff = the scan of
+// the output freqs)
+template <bool PAYLOADS>
 __global__ void __launch_bounds__(kThreads) k_merge_hits(MergeParams P, unsigned long long nout) {
         const unsigned long long j = blockIdx.x * (unsigned long long)kThreads + threadIdx.x;
         if (j >= nout)
@@ -188,6 +209,11 @@ __global__ void __launch_bounds__(kThreads) k_merge_hits(MergeParams P, unsigned
         uint32_t                *o = P.out_positions + P.out_hoff[j];
         for (uint32_t h = 0; h < f; ++h)
                 o[h] = s[h];
+        if constexpr (PAYLOADS)
+                for (uint32_t h = 0; h < f; ++h) {
+                        P.out_plens[P.out_hoff[j] + h] = P.plens[P.hoff[i] + h];
+                        P.out_pays[P.out_hoff[j] + h]  = P.pays[P.hoff[i] + h];
+                }
 }
 
 __global__ void __launch_bounds__(kThreads) k_merge_gather(const unsigned long long *a, const unsigned long long *idx, uint32_t n, unsigned long long *out) {
@@ -220,9 +246,11 @@ cudaError_t launch_merge_decode(const MergeParams &P, cudaStream_t stream) {
                 k_merge_decode_blocks<<<unsigned((P.nblocks + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P);
         return cudaGetLastError();
 }
-cudaError_t launch_merge_hits_decode(const MergeParams &P, cudaStream_t stream) {
-        if (P.nposts)
-                k_merge_decode_hits<<<unsigned((P.nposts + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P);
+cudaError_t launch_merge_hits_decode(const MergeParams &P, bool payloads, cudaStream_t stream) {
+        if (P.nposts && payloads)
+                k_merge_decode_hits<true><<<unsigned((P.nposts + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P);
+        else if (P.nposts)
+                k_merge_decode_hits<false><<<unsigned((P.nposts + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P);
         return cudaGetLastError();
 }
 cudaError_t launch_merge_keep(const MergeParams &P, cudaStream_t stream) {
@@ -235,9 +263,11 @@ cudaError_t launch_merge_scatter(const MergeParams &P, cudaStream_t stream) {
                 k_merge_scatter<<<unsigned((P.nposts + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P);
         return cudaGetLastError();
 }
-cudaError_t launch_merge_out_hits(const MergeParams &P, uint64_t nout, cudaStream_t stream) {
-        if (nout)
-                k_merge_hits<<<unsigned((nout + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P, nout);
+cudaError_t launch_merge_out_hits(const MergeParams &P, uint64_t nout, bool payloads, cudaStream_t stream) {
+        if (nout && payloads)
+                k_merge_hits<true><<<unsigned((nout + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P, nout);
+        else if (nout)
+                k_merge_hits<false><<<unsigned((nout + kThreads - 1) / kThreads), kThreads, 0, stream>>>(P, nout);
         return cudaGetLastError();
 }
 cudaError_t launch_merge_gather(const unsigned long long *a, const unsigned long long *idx, uint32_t n, unsigned long long *out, cudaStream_t stream) {

@@ -47,13 +47,14 @@ class SegmentCollection:
             if s.masked_documents.size:
                 newer = np.union1d(newer, s.masked_documents).astype(np.uint32)
 
-    def merge(self, out_codec: int, disable_optimizations: bool = False, device: int | None = None) -> MergedSegment:
+    def merge(self, out_codec: int, disable_optimizations: bool = False, device: int | None = None, payloads: bool = False) -> MergedSegment:
         """== MergeCandidatesCollection::merge over the collection's segments as they were opened (newest first, each masked by the
-        updated documents of the newer ones) into one segment of out_codec; MergedSegment.write(path) persists it"""
+        updated documents of the newer ones) into one segment of out_codec; MergedSegment.write(path) persists it.  payloads=True:
+        re-encoded hits keep their payloads (GpuIndexSource.merge_sources)"""
         srcs = [MergeSource.of_segment(s, p, g) for s, p, g in zip(self.segments, self.paths, self.generations)]
         g = GpuIndexSource(self.device if device is None else device)
         try:
-            return g.merge_sources(out_codec, srcs, disable_optimizations)
+            return g.merge_sources(out_codec, srcs, disable_optimizations, payloads)
         finally:
             g.close()
 
