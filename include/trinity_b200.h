@@ -402,6 +402,43 @@ int trn_debug_hits(int codec, const uint8_t *index, uint64_t nbytes, const uint8
 int trn_exec_batch_device(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out_counts_only);
 /* ... device pointers of the last SCORED_TOPK run: nq*k u32 docids, nq*k f32 scores (unused slots: docid 0, score -1.0; real scores are >= 0), nq u32 counts */
 int trn_last_topk_device(trn_ctx *, void **docids, void **scores, void **counts);
+
+/* ------------------------------------------------------------------------------------------------ per-query document filters
+ * == the IndexDocumentsFilter of exec_query (exec.h:50, matches.h:188-201) as docID sets.  A query may name an allow set, a deny set, both
+ * or neither; it ignores document d iff
+ *         masked(d) || (allow && d not in allow) || (deny && d in deny)
+ * which is `documentsFilter->filter(d) || maskedDocumentsRegistry->test(d)` of every exec Handler (exec.cpp:914-932, 1000-1027, 1096-1425).
+ * An ignored document is never emitted in any mode, is not counted in match_counts, never takes a top-k candidate slot or moves the
+ * threshold, and never reaches trn_exec_matches.  A query with no filter gives the documents and counts it gives without one, also beside
+ * filtered queries in one batch; its scores agree to the last-bit spread that k_score_flat's float atomics already have between any two
+ * unfiltered runs (so not bit for bit on that route).  Batches without a filtered query run the kernels they ran before.  A query's tiles (and a candidate-driven query's
+ * lead-block groups) outside its allow set's first..last docID are not evaluated.
+ *
+ * One deliberate difference: in the default mode (no ExecFlags) the reference runs a one-term query with a filter through a Handler that
+ * sets the term's freq once (exec.cpp:991, 1005-1026), so each match reports freq 1 and hits of a later document, and a document of more
+ * than 129 hits overflows its hit buffer.  trn_exec_matches reports the true freq and hits of every match, what the unfiltered run
+ * reports for the same document. */
+
+/* A resident docID set (one bit per docID, laid out and padded like the masked-documents bitmap).  Validation follows
+ * trn_set_masked_documents: docID 0 is TRN_ERR_ARG, docIDs above max_docid are ignored, order and duplicates do not matter; n == 0 makes
+ * the empty set (as an allow set it matches nothing).  Sets live across batches and any number of queries may share one.  A new
+ * trn_upload_index invalidates every handle: a stale handle gives TRN_ERR_STATE, a destroyed or unknown one TRN_ERR_ARG.  The handle
+ * carries the upload count modulo 65536, so a handle kept across 65536 or more uploads may name a live set of the current index again
+ * (never freed memory); callers drop their handles at each upload.
+ * TRN_ERR_CAPACITY when the set cannot be allocated (or the context holds TRN_DOCSET_MAX sets, default 65535); the context, its index,
+ * its sets and its percolator registry stay usable. */
+#define TRN_DOCSET_NONE 0xffffffffu
+int trn_docset_create(trn_ctx *, const uint32_t *docids, uint64_t n, uint32_t *handle);
+int trn_docset_destroy(trn_ctx *, uint32_t handle);
+typedef struct trn_doc_filter {
+        uint32_t allow, deny; /* trn_docset_create handles, or TRN_DOCSET_NONE */
+} trn_doc_filter;
+/* trn_exec_batch / trn_exec_batch_device / trn_exec_matches with filters[0..nq), one per query ({TRN_DOCSET_NONE, TRN_DOCSET_NONE}: no
+ * filter).  filters == NULL is the call without them. */
+int trn_exec_batch_filtered(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, const trn_doc_filter *filters, trn_result *out);
+int trn_exec_batch_device_filtered(trn_ctx *, const trn_query *queries, uint32_t nq, int mode, uint32_t k, const trn_doc_filter *filters,
+                                   trn_result *out_counts_only);
+int trn_exec_matches_filtered(trn_ctx *, const trn_query *queries, uint32_t nq, const trn_doc_filter *filters, trn_matches *out);
 /* merge `nshards` gathered top-k lists (layout [shard][nq][k]) into one; the one exchange step of the multi-GPU path (SURVEY 8e).
  * All pointers are device pointers; docid_base[shard] is added to the docids of that shard (0 if docIDs are already global). */
 int trn_merge_topk(trn_ctx *, const void *docids, const void *scores, uint32_t nshards, uint32_t nq, uint32_t k, void *out_docids, void *out_scores);

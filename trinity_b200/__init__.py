@@ -26,6 +26,7 @@ ROUTE_STEPS, ROUTE_FLAT_AND, ROUTE_FLAT_OR, ROUTE_CANDIDATE, ROUTE_SCORE_FLAT, R
 EMPTY_TERM = 0xFFFFFFFF
 DENSE_NONE = 0xFFFFFFFF  # debug_dense_terms: the term has no resident bitmap
 DOC_IDS_END = 0xFFFFFFFF  # DocIDsEND, common.h:43
+DOCSET_NONE = 0xFFFFFFFF  # trn_doc_filter: no allow / deny set
 
 
 class TrinityError(RuntimeError):
@@ -527,6 +528,48 @@ class IntersectResult:
         return len(self.results)
 
 
+class DocSet:
+    """A resident docID set of one GpuIndexSource (trn_docset_create): the allow or deny side of a query's document filter.  It lives
+    until close() or the source's next upload; any number of queries and batches may use it."""
+
+    def __init__(self, source: "GpuIndexSource", handle: int, size: int):
+        self.source, self.handle, self.size = source, handle, size
+
+    def close(self):
+        if self.handle is not None and self.source._h:
+            self.source._ck(self.source._L.trn_docset_destroy(self.source._h, self.handle))
+        self.handle = None
+
+
+@dataclass(frozen=True)
+class DocFilter:
+    """== an IndexDocumentsFilter over docID sets: a query ignores d iff (allow and d not in allow) or (deny and d in deny), beside the
+    masked documents"""
+    allow: Optional[DocSet] = None
+    deny: Optional[DocSet] = None
+
+
+def _pack_filters(filters: Optional[Sequence[Optional[DocFilter]]], nq: int, source=None) -> Optional[np.ndarray]:
+    """one trn_doc_filter (allow, deny handles) per query; None -> None (the call without filters)"""
+    if filters is None:
+        return None
+    if len(filters) != nq:
+        raise ValueError(f"{len(filters)} filters for {nq} queries")
+    out = np.full((nq, 2), DOCSET_NONE, np.uint32)
+    for q, f in enumerate(filters):
+        if f is None:
+            continue
+        for j, d in enumerate((f.allow, f.deny)):
+            if d is None:
+                continue
+            if d.handle is None:
+                raise ValueError(f"query {q}: a closed DocSet")
+            if source is not None and d.source is not source:
+                raise ValueError(f"query {q}: a DocSet of another index source")
+            out[q, j] = d.handle
+    return out
+
+
 class GpuIndexSource:
     """== one device-resident IndexSource + AccessProxy (index_source.h:18-155, codecs.h:290-317) and the batch form of
     exec_query() (exec.h:50-52) over it."""
@@ -568,6 +611,14 @@ class GpuIndexSource:
         d = _u32([] if docids is None else docids)
         self._ck(self._L.trn_set_masked_documents(self._h, _ptr(d) if len(d) else None, len(d)))
 
+    def docset(self, docids) -> DocSet:
+        """a resident docID set for DocFilter (trn_docset_create): order and duplicates do not matter, docIDs above max_docid are
+        ignored, docID 0 is refused; an empty set is valid (as an allow set it matches nothing)"""
+        d = _u32(docids)
+        h = C.c_uint32()
+        self._ck(self._L.trn_docset_create(self._h, _ptr(d) if len(d) else None, len(d), C.byref(h)))
+        return DocSet(self, int(h.value), len(d))
+
     def info(self) -> dict:
         i = TrnIndexInfo()
         self._ck(self._L.trn_index_info_get(self._h, C.byref(i)))
@@ -584,10 +635,15 @@ class GpuIndexSource:
     def _pack(self, queries: Sequence[np.ndarray]):
         return _pack_queries(queries)
 
-    def exec_batch_device(self, queries: Sequence[np.ndarray], mode: int, k: int = 100, packed=None):
+    def exec_batch_device(self, queries: Sequence[np.ndarray], mode: int, k: int = 100, packed=None, filters=None):
+        """filters: None, or one None / DocFilter per query"""
         arr, keep = packed if packed is not None else self._pack(queries)
         r = TrnResult()
-        self._ck(self._L.trn_exec_batch_device(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, C.byref(r)))
+        f = _pack_filters(filters, len(queries), self)
+        if f is None:
+            self._ck(self._L.trn_exec_batch_device(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, C.byref(r)))
+        else:
+            self._ck(self._L.trn_exec_batch_device_filtered(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, _ptr(f), C.byref(r)))
         self._last = (mode, k, len(queries))
         return r
 
@@ -630,19 +686,29 @@ class GpuIndexSource:
         marshalling out of a timed region"""
         return self._pack(queries)
 
-    def exec_batch(self, queries: Sequence[np.ndarray], mode: int, k: int = 100, copy: bool = True, packed=None) -> BatchResult:
-        """== exec_query() for a batch: plans H2D, fused kernels, results D2H."""
+    def exec_batch(self, queries: Sequence[np.ndarray], mode: int, k: int = 100, copy: bool = True, packed=None, filters=None) -> BatchResult:
+        """== exec_query() for a batch: plans H2D, fused kernels, results D2H.  filters: None, or one None / DocFilter per query (the
+        IndexDocumentsFilter of exec_query)"""
         arr, keep = packed if packed is not None else self._pack(queries)
         r = TrnResult()
-        self._ck(self._L.trn_exec_batch(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, C.byref(r)))
+        f = _pack_filters(filters, len(queries), self)
+        if f is None:
+            self._ck(self._L.trn_exec_batch(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, C.byref(r)))
+        else:
+            self._ck(self._L.trn_exec_batch_filtered(self._h, C.cast(arr, C.c_void_p), len(queries), mode, k, _ptr(f), C.byref(r)))
         self._last = (mode, k, len(queries))
         return self._wrap(r, mode, k, copy)
 
-    def exec_matches(self, queries: Sequence[np.ndarray], packed=None) -> MatchesResult:
-        """== exec_query() with no ExecFlags for a batch: every match with the query terms it holds and their hits (TRN_MODE_MATCHED_TERMS)"""
+    def exec_matches(self, queries: Sequence[np.ndarray], packed=None, filters=None) -> MatchesResult:
+        """== exec_query() with no ExecFlags for a batch: every match with the query terms it holds and their hits (TRN_MODE_MATCHED_TERMS).
+        filters: None, or one None / DocFilter per query"""
         arr, keep = packed if packed is not None else self._pack(queries)
         r = TrnMatches()
-        self._ck(self._L.trn_exec_matches(self._h, C.cast(arr, C.c_void_p), len(queries), C.byref(r)))
+        f = _pack_filters(filters, len(queries), self)
+        if f is None:
+            self._ck(self._L.trn_exec_matches(self._h, C.cast(arr, C.c_void_p), len(queries), C.byref(r)))
+        else:
+            self._ck(self._L.trn_exec_matches_filtered(self._h, C.cast(arr, C.c_void_p), len(queries), _ptr(f), C.byref(r)))
         self._last = (MODE_MATCHED_TERMS, 0, len(queries))
         return MatchesResult(r)
 

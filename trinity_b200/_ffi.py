@@ -26,6 +26,7 @@ EXPORTS = [
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
     "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_merge_sources_payloads", "trn_debug_merge_plan",
+    "trn_docset_create", "trn_docset_destroy", "trn_exec_batch_filtered", "trn_exec_batch_device_filtered", "trn_exec_matches_filtered",
 ]
 
 TERM_DTYPE = np.dtype([("documents", "<u4"), ("chunk_off", "<u4"), ("chunk_len", "<u4")])
@@ -202,6 +203,11 @@ def lib() -> C.CDLL:
     sig("trn_encode_lucene_payloads", i32, vp, vp, u32, vp, vp, vp, vp, vp, vp, C.c_uint64, P(C.c_uint64), vp, C.c_uint64, P(C.c_uint64), vp, P(C.c_float))
     sig("trn_debug_last_routes", i32, vp, vp, u32, P(u32))
     sig("trn_exec_matches", i32, vp, vp, u32, P(TrnMatches))
+    sig("trn_docset_create", i32, vp, vp, u64, P(u32))
+    sig("trn_docset_destroy", i32, vp, u32)
+    sig("trn_exec_batch_filtered", i32, vp, vp, u32, i32, u32, vp, P(TrnResult))
+    sig("trn_exec_batch_device_filtered", i32, vp, vp, u32, i32, u32, vp, P(TrnResult))
+    sig("trn_exec_matches_filtered", i32, vp, vp, u32, vp, P(TrnMatches))
     sig("trn_debug_hits", i32, i32, vp, C.c_uint64, vp, C.c_uint64, vp, vp, u32, vp, vp, vp, C.c_uint64, P(C.c_uint64), C.c_char_p, C.c_size_t)
     sig("trn_debug_plan", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, P(u32), C.c_char_p, C.c_size_t)
     sig("trn_debug_dense_runs", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)

@@ -121,6 +121,15 @@ struct FlatQuery {
         uint32_t item_base;  // scored-all: the query's first (query, tile) item in the batch-wide segment arrays
         uint32_t local_base; // scored-all: the query's first item in this kernel's own ticket space
 };
+// a query's document filter (trn_doc_filter) as the kernels read it: resident docID sets laid out like DevIndex::masked.  A query
+// ignores d iff masked(d) || (allow && d not in allow) || (deny && d in deny).  Only the filtered instantiations (FILT) read it.
+struct DevFilter {
+        const uint32_t *allow; // null: no allow set
+        const uint32_t *deny;  // null: no deny set
+        uint32_t        lo, hi; // the allow set's first and last docID (lo > hi: it is empty); 0, 0xffffffff without one
+};
+static_assert(sizeof(DevFilter) == 24, "DevFilter layout");
+
 struct ScoreParams {
         DevIndex         ix;
         const FlatQuery *fq;
@@ -141,6 +150,7 @@ struct ScoreParams {
         uint64_t *          item_off;
         uint32_t *          item_cnt;
         uint32_t *          overflow;
+        const DevFilter *   filters; // per query of the batch (FlatQuery::qid); null: no query has a filter
 };
 
 // one unit of the whole-list decode kernels (decode_stream.cuh): 32 consecutive blocks of one term, laid out by the host
@@ -192,6 +202,7 @@ struct ExecParams {
         uint32_t *          cand_cursor;  // per query
         uint2 *             cand;         // (score bits, docid)
         uint32_t *          overflow;     // set to 1 if seg_capacity was exceeded
+        const DevFilter *   filters;      // per query; null: no query of the batch has a filter (the unfiltered instantiations run)
 };
 
 // device-side GOOGLE encoder (encode_google.cuh)

@@ -100,6 +100,16 @@ struct trn_ctx {
         uint64_t             index_bytes{0}, dir_bytes{0}, total_blocks{0}, total_postings{0};
         DevBuf               d_index, d_blk_last, d_blk_off, d_terms, d_tile_first, d_masked;
         bool                 have_masked{false};
+        // per-query document filters (trn_docset_create): handle = (epoch & 0xffff) << 16 | slot; a new upload frees every set and bumps the epoch
+        struct DocSet {
+                DevBuf   bits;       // laid out like d_masked
+                uint32_t lo{1}, hi{0}; // first and last docID (lo > hi: empty)
+                bool     live{false};
+        };
+        std::vector<DocSet> docsets;
+        uint32_t            docset_epoch{0};
+        uint32_t            docset_max{0xffffu}; // TRN_DOCSET_MAX: sets a context holds at once (at most 65535)
+        DevBuf              d_filters;           // the batch's DevFilter per query (exec_device_impl, filtered batches only)
         DevBuf               d_dense, d_dense_off; // resident bitmaps of the dense terms (select_dense_terms) and each term's first word in them
         uint32_t             dense_terms{0};       // terms with a bitmap (0: none, d_dense unused)
         uint64_t             dense_bytes{0};
@@ -295,6 +305,11 @@ extern "C" int trn_create(int device, trn_ctx **out) {
                 if (v >= 1)
                         c->match_chunk = uint64_t(v);
         }
+        if (const char *e = getenv("TRN_DOCSET_MAX")) {
+                const long long v = atoll(e);
+                if (v >= 0 && v < 0xffffll)
+                        c->docset_max = uint32_t(v);
+        }
         if (const char *e = getenv("TRN_ISECT_MAX_MASKS")) {
                 const long long v = atoll(e);
                 if (v >= 1 && v < (long long)kIsectMaxMasks)
@@ -323,8 +338,10 @@ extern "C" void trn_destroy(trn_ctx *c) {
         for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
-                          &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores})
+                          &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores, &c->d_filters})
                 b->release();
+        for (auto &d : c->docsets)
+                d.bits.release();
         for (PinBuf *b : {&c->h_offsets, &c->h_docids, &c->h_scores, &c->h_counts, &c->h_small, &c->h_chunk, &c->h_item_desc})
                 b->release();
         for (cudaEvent_t e : {c->ev0, c->ev1, c->evk0, c->evk1, c->ev_done[0], c->ev_done[1], c->ev_d2h[0], c->ev_d2h[1]})
@@ -420,6 +437,14 @@ static int upload_dense(trn_ctx *c) {
         return TRN_OK;
 }
 
+// every docID set of the context is dropped: its handles become stale (trn_upload_index; the sets' sizes follow the old max_docid)
+static void drop_docsets(trn_ctx *c) {
+        for (auto &d : c->docsets)
+                d.bits.release();
+        c->docsets.clear();
+        ++c->docset_epoch;
+}
+
 extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid) {
         if (!c || !index || !terms || (codec != TRN_CODEC_GOOGLE && codec != TRN_CODEC_LUCENE))
                 return c ? fail(c, TRN_ERR_ARG, "trn_upload_index: bad arguments") : TRN_ERR_ARG;
@@ -444,6 +469,7 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         uint32_t min_docid;
         docid_span(ht, min_docid, max_docid);
         c->have_index   = false; // until the new index is completely in place
+        drop_docsets(c);
         c->pc.codec     = codec;
         c->pc.min_docid = min_docid;
         c->pc.max_docid = max_docid;
@@ -502,6 +528,7 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         c->have_masked = false;
         return TRN_OK;
 }
+
 
 // LUCENE positions: hits.data of the uploaded index (lucene_codec.cpp:401-513).  `index` = the bytes trn_upload_index received (they are
 // read again on the host: the freqs give every block's first hit number); without this call phrase plans on a LUCENE source are refused.
@@ -577,6 +604,120 @@ extern "C" int trn_set_masked_documents(trn_ctx *c, const uint32_t *docids, uint
         return TRN_OK;
 }
 
+// ============================================================================================ per-query document filters
+extern "C" int trn_docset_create(trn_ctx *c, const uint32_t *docids, uint64_t n, uint32_t *handle) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (!handle || (n && !docids))
+                return fail(c, TRN_ERR_ARG, "trn_docset_create: null argument");
+        if (!c->have_index)
+                return fail(c, TRN_ERR_STATE, "no index uploaded");
+        CK(cudaSetDevice(c->device));
+        uint32_t slot = 0, nlive = 0;
+        while (slot < c->docsets.size() && c->docsets[slot].live)
+                ++slot;
+        for (const auto &d : c->docsets)
+                nlive += d.live ? 1u : 0u;
+        if (nlive >= c->docset_max)
+                return fail(c, TRN_ERR_CAPACITY, "trn_docset_create: the context holds " + std::to_string(nlive) + " docID sets (TRN_DOCSET_MAX); destroy some");
+        // the layout of trn_set_masked_documents: one bit per docID, padded so that every (largest) tile can read its whole word range
+        const uint64_t        span = ((uint64_t(c->pc.max_docid) >> 17) + 2) << 17;
+        std::vector<uint32_t> words;
+        try {
+                words.assign(span / 32, 0u);
+        } catch (const std::bad_alloc &) {
+                return fail(c, TRN_ERR_CAPACITY, "trn_docset_create: out of host memory");
+        }
+        uint32_t lo = 0xffffffffu, hi = 0;
+        for (uint64_t i = 0; i < n; ++i) {
+                const uint32_t d = docids[i];
+                if (d == 0)
+                        return fail(c, TRN_ERR_ARG, "docID 0 is not a document");
+                if (d > c->pc.max_docid)
+                        continue; // as for the masked documents: a set may name documents this source does not hold
+                words[d >> 5] |= 1u << (d & 31u);
+                lo = std::min(lo, d);
+                hi = std::max(hi, d);
+        }
+        DevBuf            bits;
+        const cudaError_t e = bits.ensure(words.size() * 4);
+        if (e != cudaSuccess) {
+                (void)cudaGetLastError(); // an allocation failure is not sticky: clear it
+                return fail(c, TRN_ERR_CAPACITY, std::string("trn_docset_create: ") + cudaGetErrorString(e));
+        }
+        if (const cudaError_t ce = cudaMemcpyAsync(bits.p, words.data(), words.size() * 4, cudaMemcpyHostToDevice, c->stream); ce != cudaSuccess) {
+                bits.release();
+                CK(ce);
+        }
+        if (const cudaError_t se = cudaStreamSynchronize(c->stream); se != cudaSuccess) {
+                bits.release();
+                CK(se);
+        }
+        if (slot == c->docsets.size())
+                c->docsets.emplace_back();
+        auto &D = c->docsets[slot];
+        D.bits  = bits;
+        D.lo    = lo;
+        D.hi    = hi;
+        D.live  = true;
+        *handle = (c->docset_epoch & 0xffffu) << 16 | slot;
+        return TRN_OK;
+}
+
+// the set behind a handle (TRN_OK), or why there is none
+static int docset_of(trn_ctx *c, uint32_t h, const trn_ctx::DocSet *&out) {
+        if ((h >> 16) != (c->docset_epoch & 0xffffu))
+                return fail(c, TRN_ERR_STATE, "docID set " + std::to_string(h) + " belongs to an index this context no longer holds");
+        const uint32_t slot = h & 0xffffu;
+        if (slot >= c->docsets.size() || !c->docsets[slot].live)
+                return fail(c, TRN_ERR_ARG, "docID set " + std::to_string(h) + " does not exist (destroyed?)");
+        out = &c->docsets[slot];
+        return TRN_OK;
+}
+
+extern "C" int trn_docset_destroy(trn_ctx *c, uint32_t handle) {
+        if (!c)
+                return TRN_ERR_ARG;
+        const trn_ctx::DocSet *d = nullptr;
+        if (const int rc = docset_of(c, handle, d); rc != TRN_OK)
+                return rc;
+        CK(cudaSetDevice(c->device));
+        CK(cudaStreamSynchronize(c->stream)); // a batch in flight may still read it
+        auto &D = c->docsets[handle & 0xffffu];
+        D.bits.release();
+        D.live = false;
+        return TRN_OK;
+}
+
+// the device view of a batch's filters and each query's allow span.  false (nothing written): no query names a set
+static int resolve_filters(trn_ctx *c, const trn_doc_filter *filters, uint32_t nq, std::vector<DevFilter> &dev, std::vector<uint2> &clip, bool &any) {
+        any = false;
+        if (!filters)
+                return TRN_OK;
+        for (uint32_t q = 0; q < nq && !any; ++q)
+                any = filters[q].allow != TRN_DOCSET_NONE || filters[q].deny != TRN_DOCSET_NONE;
+        if (!any)
+                return TRN_OK;
+        dev.assign(nq, DevFilter{nullptr, nullptr, 0u, 0xffffffffu});
+        clip.assign(nq, uint2{0u, 0xffffffffu});
+        for (uint32_t q = 0; q < nq; ++q) {
+                const trn_ctx::DocSet *d = nullptr;
+                if (filters[q].allow != TRN_DOCSET_NONE) {
+                        if (const int rc = docset_of(c, filters[q].allow, d); rc != TRN_OK)
+                                return fail(c, rc, "query " + std::to_string(q) + " allow: " + c->err);
+                        dev[q].allow = d->bits.as<uint32_t>();
+                        dev[q].lo = clip[q].x = d->lo;
+                        dev[q].hi = clip[q].y = d->hi;
+                }
+                if (filters[q].deny != TRN_DOCSET_NONE) {
+                        if (const int rc = docset_of(c, filters[q].deny, d); rc != TRN_OK)
+                                return fail(c, rc, "query " + std::to_string(q) + " deny: " + c->err);
+                        dev[q].deny = d->bits.as<uint32_t>();
+                }
+        }
+        return TRN_OK;
+}
+
 extern "C" int trn_index_info_get(trn_ctx *c, trn_index_info *o) {
         if (!c || !o)
                 return TRN_ERR_ARG;
@@ -625,8 +766,9 @@ static DevIndex dev_index(trn_ctx *c) {
 // routes[0 .. nq): the TRN_ROUTE_* of every query (written on success)
 // collect: non-null = the docs pass of the default exec mode (mode DOCS_ONLY; the plan is made in TRN_MODE_MATCHED_TERMS, and its collect
 // programs are moved to *collect)
+// filters: null, or one per query (trn_doc_filter)
 static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out, int set, cudaEvent_t k0, cudaEvent_t k1,
-                            uint8_t *routes, CollectPlan *collect = nullptr) {
+                            uint8_t *routes, const trn_doc_filter *filters, CollectPlan *collect = nullptr) {
         if (!c)
                 return TRN_ERR_ARG;
         if (!c->have_index)
@@ -644,11 +786,16 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         const bool scored = mode != TRN_MODE_DOCS_ONLY;
 
         const double tCompile0 = now_ms();
+        std::vector<DevFilter> devFilters;
+        std::vector<uint2>     clip;
+        bool                   filtered{false};
+        if (const int rc = resolve_filters(c, filters, nq, devFilters, clip, filtered); rc != TRN_OK)
+                return rc;
         c->pc.allow_phrase     = c->pc.codec == TRN_CODEC_GOOGLE || c->have_hits; // GOOGLE: inline hits; LUCENE: hits.data uploaded (trn_upload_hits)
         BatchPlan   plan;
         std::string perr;
         const int   prc = plan_batch(c->pc, c->h_terms, c->dense_terms ? c->h_dense_off.data() : nullptr, queries, nq, collect ? TRN_MODE_MATCHED_TERMS : mode, k, plan,
-                                     perr);
+                                     perr, filtered ? clip.data() : nullptr);
         if (prc != TRN_OK)
                 return fail(c, prc, perr);
         if (collect)
@@ -723,6 +870,10 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 }
         }
         CK(cudaMemcpyAsync(c->d_queries.p, plan.queries.data(), nq * sizeof(DevQuery), cudaMemcpyHostToDevice, c->stream));
+        if (filtered) {
+                CK(c->d_filters.ensure(nq * sizeof(DevFilter)));
+                CK(cudaMemcpyAsync(c->d_filters.p, devFilters.data(), nq * sizeof(DevFilter), cudaMemcpyHostToDevice, c->stream));
+        }
         if (!steps.empty())
                 CK(cudaMemcpyAsync(c->d_steps.p, steps.data(), steps.size() * sizeof(DevStep), cudaMemcpyHostToDevice, c->stream));
         const uint32_t denseItems = uint32_t(plan.dense_runs.size());
@@ -770,6 +921,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         P.cand_cursor  = cand_cursor;
         P.cand         = c->d_cand.as<uint2>();
         P.overflow     = overflow;
+        P.filters      = filtered ? c->d_filters.as<DevFilter>() : nullptr;
 
         uint32_t launches{0};
         if (totalItems) {
@@ -802,12 +954,14 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         S.item_off     = P.item_off;
                         S.item_cnt     = P.item_cnt;
                         S.overflow     = overflow;
+                        S.filters      = P.filters;
                         CK(launch_build_luts(S.leaves, uint32_t(plan.leaves.size()), c->d_luts.as<float>(), c->stream));
                         CK(launch_score_flat(S, c->flat_threads, c->num_sms, c->stream));
                         launches += 2;
                 }
                 if (ownItems) {
-                        const int perSM = warpKernel ? exec_docs_max_ctas_per_sm(execShift, plan.nslots, exec_docs_stage_bytes(), false, c->pc.codec == TRN_CODEC_LUCENE) : exec_max_ctas_per_sm(execShift, plan.nslots, mode, c->pc.codec);
+                        const int perSM = warpKernel ? exec_docs_max_ctas_per_sm(execShift, plan.nslots, exec_docs_stage_bytes(), false, c->pc.codec == TRN_CODEC_LUCENE, filtered)
+                                                     : exec_max_ctas_per_sm(execShift, plan.nslots, mode, c->pc.codec, filtered);
                         if (perSM <= 0)
                                 return fail(c, TRN_ERR_CUDA, "the exec kernel does not fit on an SM with this many docset slots");
                         const uint64_t workers = warpKernel ? (ownItems + 3) / 4 : ownItems; // 4 warp-workers per CTA
@@ -829,7 +983,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         P2.mixed_runs  = nullptr;
                         P2.mixed_items = 0;
                         P2.ticket     = reinterpret_cast<uint32_t *>(small + 4);
-                        const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true);
+                        const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true, false, filtered);
                         if (perSM <= 0)
                                 return fail(c, TRN_ERR_CUDA, "the flat-tree launch does not fit on an SM with this many docset slots");
                         const int grid = int(std::min<uint64_t>(uint64_t(c->num_sms) * perSM, std::max<uint64_t>(1, (plan.gen_items2 + 3) / 4)));
@@ -877,6 +1031,10 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
 }
 
 extern "C" int trn_exec_batch_device(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out) {
+        return trn_exec_batch_device_filtered(c, queries, nq, mode, k, nullptr, out);
+}
+
+extern "C" int trn_exec_batch_device_filtered(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, const trn_doc_filter *filters, trn_result *out) {
         if (!c)
                 return TRN_ERR_ARG;
         CK(cudaSetDevice(c->device));
@@ -886,7 +1044,7 @@ extern "C" int trn_exec_batch_device(trn_ctx *c, const trn_query *queries, uint3
         const double t0       = now_ms();
         CK(cudaEventRecord(c->ev0, c->stream));
         std::vector<uint8_t> routes(nq);
-        const int            r = exec_device_impl(c, queries, nq, mode, k, out, 0, c->evk0, c->evk1, routes.data());
+        const int            r = exec_device_impl(c, queries, nq, mode, k, out, 0, c->evk0, c->evk1, routes.data(), filters);
         c->tm.total_ms = float(now_ms() - t0);
         if (r != TRN_OK)
                 return r;
@@ -985,8 +1143,19 @@ extern "C" int trn_fetch_results(trn_ctx *c, trn_result *out) {
 // results of chunk i travel to the (pinned) host buffer on a second stream — the e2e time tends to max(kernels, D2H) instead of
 // their sum.  Output-side device buffers are double-buffered (set = chunk parity); everything else is reused in stream order.
 extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, trn_result *out) {
+        return trn_exec_batch_filtered(c, queries, nq, mode, k, nullptr, out);
+}
+
+extern "C" int trn_exec_batch_filtered(trn_ctx *c, const trn_query *queries, uint32_t nq, int mode, uint32_t k, const trn_doc_filter *filters, trn_result *out) {
         if (!c || !out)
                 return TRN_ERR_ARG;
+        if (filters) { // every handle is checked before the first chunk is launched
+                std::vector<DevFilter> dev;
+                std::vector<uint2>     clip;
+                bool                   any{false};
+                if (const int rc = resolve_filters(c, filters, nq, dev, clip, any); rc != TRN_OK)
+                        return rc;
+        }
         // how the batch is split into pipelined launches: chunkplan.h (a pure function of what is known here, pinned on the CPU by
         // tests/test_chunk_plan_cpu.py).
         ChunkPlanIn pin;
@@ -1013,7 +1182,7 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
         const bool      compact     = mode == TRN_MODE_DOCS_COMPACT;
         if (plan.single_call) {
                 const double t0 = now_ms();
-                const int    r  = trn_exec_batch_device(c, queries, nq, mode, k, nullptr);
+                const int    r  = trn_exec_batch_device_filtered(c, queries, nq, mode, k, filters, nullptr);
                 if (r != TRN_OK)
                         return r;
                 const double tw = now_ms();
@@ -1139,7 +1308,8 @@ extern "C" int trn_exec_batch(trn_ctx *c, const trn_query *queries, uint32_t nq,
                 if (i >= 2)
                         CK(cudaStreamWaitEvent(c->stream, c->ev_d2h[set], 0)); // the set's previous results have left the device
                 trn_result part;
-                const int  r = exec_device_impl(c, queries + ch[i].q0, ch[i].n, mode, k, &part, set, c->ev_ck0[i % 16], c->ev_ck1[i % 16], routes.data() + ch[i].q0);
+                const int  r = exec_device_impl(c, queries + ch[i].q0, ch[i].n, mode, k, &part, set, c->ev_ck0[i % 16], c->ev_ck1[i % 16], routes.data() + ch[i].q0,
+                                                filters ? filters + ch[i].q0 : nullptr);
                 if (r == TRN_ERR_CAPACITY && ch[i].n > 1) {
                         // the upper bound of this chunk's matches does not fit the device: halve it and retry (nothing was launched)
                         const Chunk a{ch[i].q0, ch[i].n / 2}, b{ch[i].q0 + ch[i].n / 2, ch[i].n - ch[i].n / 2};
@@ -1230,6 +1400,10 @@ extern "C" int trn_debug_last_routes(trn_ctx *c, uint8_t *out, uint32_t cap, uin
 // plans a batch on the host as exec_device_impl would on a context that holds this index (trn_debug_plan, trn_debug_dense_runs)
 // ============================================================================================ default exec mode
 extern "C" int trn_exec_matches(trn_ctx *c, const trn_query *queries, uint32_t nq, trn_matches *out) {
+        return trn_exec_matches_filtered(c, queries, nq, nullptr, out);
+}
+
+extern "C" int trn_exec_matches_filtered(trn_ctx *c, const trn_query *queries, uint32_t nq, const trn_doc_filter *filters, trn_matches *out) {
         if (!c || !out)
                 return TRN_ERR_ARG;
         CK(cudaSetDevice(c->device));
@@ -1248,7 +1422,7 @@ extern "C" int trn_exec_matches(trn_ctx *c, const trn_query *queries, uint32_t n
         CK(cudaEventRecord(c->ev0, c->stream));
         std::vector<uint8_t> routes(nq);
         CollectPlan          cp;
-        const int            r = exec_device_impl(c, queries, nq, TRN_MODE_DOCS_ONLY, 0, nullptr, 0, c->evk0, c->evk1, routes.data(), &cp);
+        const int            r = exec_device_impl(c, queries, nq, TRN_MODE_DOCS_ONLY, 0, nullptr, 0, c->evk0, c->evk1, routes.data(), filters, &cp);
         c->last_mode         = -1; // trn_fetch_results has nothing to fetch after this call (the docs pass leaves no trn_result)
         if (r != TRN_OK)
                 return r;

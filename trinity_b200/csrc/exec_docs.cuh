@@ -730,9 +730,12 @@ __device__ __forceinline__ unsigned long long run_reserve(const ExecParams &P, u
 // Pass 1 ANDs each tile's words (masked documents removed) row by row in registers and sizes its result; the run's segments take ONE
 // reservation; pass 2 rebuilds each non-empty tile row by row (its words now come from L2) and writes it exactly as the per-tile path
 // would.  No tile passes through shared memory.
-__device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, int lane) {
+template <bool FILT> __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, int lane) {
         const uint32_t q = e.x, t0 = e.y;
         const DevQuery &Q     = P.queries[q];
+        DevFilter       F{};
+        if constexpr (FILT)
+                F = P.filters[q];
         const uint32_t  nt    = dense_run_end(t0, Q.tile_lo, Q.ntiles, P.exec_shift) - t0; // 1 .. 16 tiles
         const uint32_t  item0 = Q.item_base + (t0 - Q.tile_lo);
         const uint32_t  lo0   = t0 << P.exec_shift;
@@ -758,6 +761,10 @@ __device__ void dense_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
                 if (P.ix.masked) {
                         const uint4 m = reinterpret_cast<const uint4 *>(P.ix.masked + ((lo0 >> 5) + j * NW))[i];
                         w             = make_uint4(~m.x, ~m.y, ~m.z, ~m.w);
+                }
+                if constexpr (FILT) { // the query's filter
+                        const uint32_t wi = (lo0 >> 5) + j * NW + i * 4u;
+                        w = make_uint4(w.x & filter_keep(F, wi), w.y & filter_keep(F, wi + 1u), w.z & filter_keep(F, wi + 2u), w.w & filter_keep(F, wi + 3u));
                 }
                 auto leaf = [&](uint32_t k) {
                         const uint4 v = __ldg(reinterpret_cast<const uint4 *>(P.ix.dense + __shfl_sync(0xffffffffu, myw, int(k)) + j * NW) + i);
@@ -826,9 +833,12 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
         return m;
 }
 
-__device__ void mixed_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, uint32_t *smem, int lane) {
+template <bool FILT> __device__ void mixed_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_t NW, uint32_t *smem, int lane) {
         const uint32_t  q    = e.x, t0 = e.y;
         const DevQuery &Q    = P.queries[q];
+        DevFilter       F{};
+        if constexpr (FILT)
+                F = P.filters[q];
         const uint32_t  nt   = dense_run_end(t0, Q.tile_lo, Q.ntiles, P.exec_shift) - t0; // 1 .. 16 tiles
         const uint32_t  lo0  = t0 << P.exec_shift, span = nt << P.exec_shift;         // the run's docIDs [lo0, lo0 + span) (the end may be 2^32)
         uint32_t *const tcnt  = smem + kCandWords; // (the candidate array starts at smem)
@@ -902,6 +912,15 @@ __device__ void mixed_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
 #pragma unroll
                                         for (uint32_t u = 0; u < 4u; ++u)
                                                 rel[u] = (v[u] >> (rel[u] & 31u)) & 1u ? span : rel[u];
+                                }
+                                if constexpr (FILT) { // the query's filter
+                                        uint32_t v[4];
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                v[u] = rel[u] < span ? filter_keep(F, (lo0 >> 5) + (rel[u] >> 5)) : 0u;
+#pragma unroll
+                                        for (uint32_t u = 0; u < 4u; ++u)
+                                                rel[u] = (v[u] >> (rel[u] & 31u)) & 1u ? rel[u] : span;
                                 }
 #pragma unroll
                                 for (uint32_t u = 0; u < 4u; ++u)
@@ -1012,7 +1031,8 @@ __device__ void mixed_run_exec(const ExecParams &P, uint2 e, uint32_t W, uint32_
 // candidate and flat paths it pushed them over the 72-register bound)
 // LUC: the launch runs over a LUCENE index (the codec is a property of the uploaded index, so of the launch): that instantiation carries the
 // bulk-copy block decoder and none of the GOOGLE-only paths (candidate-driven, flat, flat-tree), and the GOOGLE ones do not carry it
-template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsWarps * 32, PH ? 4 : (TREE ? 6 : 7)) k_exec_docs(ExecParams P) { // PH: see k_exec_tiles
+// FILT: the launch holds a query with a document filter (ExecParams::filters); the other instantiations do not read them
+template <bool PH, bool TREE, bool LUC, bool FILT> __global__ void __launch_bounds__(kDocsWarps * 32, PH ? 4 : (TREE ? 6 : 7)) k_exec_docs(ExecParams P) { // PH: see k_exec_tiles
         __shared__ __align__(8) unsigned long long s_lbar[kDocsWarps]; // LUCENE: one mbarrier per warp for its block copies
         uint32_t lseq = 0;                                            // ... and how many copies the warp has consumed (phase parity)
         if constexpr (LUC) {
@@ -1046,12 +1066,12 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                         break;
                 if constexpr (!PH && !TREE && !LUC) {
                         if (gitem < P.dense_items) { // all-bitmap flat AND: the query's tiles of one run
-                                dense_run_exec(P, P.dense_runs[gitem], W, NW, lane);
+                                dense_run_exec<FILT>(P, P.dense_runs[gitem], W, NW, lane);
                                 continue;
                         }
                         if (gitem - P.dense_items < P.mixed_items) { // flat AND with one decoded operand: the query's tiles of one run
                                 __syncwarp();
-                                mixed_run_exec(P, P.mixed_runs[gitem - P.dense_items], W, NW, slots, lane);
+                                mixed_run_exec<FILT>(P, P.mixed_runs[gitem - P.dense_items], W, NW, slots, lane);
                                 continue;
                         }
                 }
@@ -1074,7 +1094,7 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                 if constexpr (!TREE && !LUC) {
                         if (Q.route == TRN_ROUTE_CANDIDATE) { // candidate-driven conjunction: the work item is a 32-block group of the lead term
                                 __syncwarp();
-                                cand_exec_google(P, Q, curq, item, item - Q.item_base, slots, lane);
+                                cand_exec_google<FILT>(P, Q, curq, item, item - Q.item_base, slots, lane);
                                 continue;
                         }
                 }
@@ -1259,6 +1279,16 @@ template <bool PH, bool TREE, bool LUC> __global__ void __launch_bounds__(kDocsW
                                 r[i] &= ~mk[i];
                         __syncwarp();
                 }
+                // ... and neither do the documents the query's filter drops (IndexDocumentsFilter::filter, exec.cpp:1108-1116)
+                if constexpr (FILT) {
+                        if (!dead) {
+                                const DevFilter F = P.filters[curq];
+                                uint32_t *      r = slots + size_t(Q.root_slot) * NW;
+                                for (uint32_t i = lane; i < NW; i += 32)
+                                        r[i] &= filter_keep(F, (lo >> 5) + i);
+                                __syncwarp();
+                        }
+                }
                 // ---- emission: ordered compaction of the root docset
                 const uint32_t *root = slots + size_t(Q.root_slot) * NW;
                 const TileCount tc   = tile_count(root, !dead, P.item_desc != nullptr, W, NW, lane);
@@ -1299,18 +1329,21 @@ size_t exec_docs_smem_bytes(uint32_t exec_shift, uint32_t nslots, uint32_t stage
         return size_t(kDocsWarps) * (size_t(nslots) * NW * 4 + stageBytes);
 }
 
-int exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes, bool tree, bool lucene) {
+// the instantiation of k_exec_docs a launch runs (a flat-tree launch never holds a phrase plan)
+template <bool FILT> static const void *exec_docs_fn(bool phrase, bool tree, bool lucene) {
+        if (lucene)
+                return phrase ? (const void *)k_exec_docs<true, false, true, FILT> : (const void *)k_exec_docs<false, false, true, FILT>;
+        if (tree)
+                return (const void *)k_exec_docs<false, true, false, FILT>;
+        return phrase ? (const void *)k_exec_docs<true, false, false, FILT> : (const void *)k_exec_docs<false, false, false, FILT>;
+}
+static const void *exec_docs_fn(bool phrase, bool tree, bool lucene, bool filt) {
+        return filt ? exec_docs_fn<true>(phrase, tree, lucene) : exec_docs_fn<false>(phrase, tree, lucene);
+}
+
+int exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes, bool tree, bool lucene, bool filt) {
         const size_t smem = exec_docs_smem_bytes(exec_shift, nslots, stageBytes);
-        const void *fns[2];
-        if (lucene) {
-                fns[0] = (const void *)k_exec_docs<false, false, true>;
-                fns[1] = (const void *)k_exec_docs<true, false, true>;
-        } else if (tree) {
-                fns[0] = fns[1] = (const void *)k_exec_docs<false, true, false>;
-        } else {
-                fns[0] = (const void *)k_exec_docs<false, false, false>;
-                fns[1] = (const void *)k_exec_docs<true, false, false>;
-        }
+        const void *fns[2] = {exec_docs_fn(false, tree, lucene, filt), exec_docs_fn(!tree, tree, lucene, filt)};
         int best = 0;
         for (int i = 0; i < 2; ++i) {
                 if (cudaFuncSetAttribute(fns[i], cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess)
@@ -1327,12 +1360,8 @@ int exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t sta
 cudaError_t launch_exec_docs(const ExecParams &P, int grid, cudaStream_t stream) {
         const size_t smem = exec_docs_smem_bytes(P.exec_shift, P.nslots, P.docs_stage_bytes);
         // gen_sel == 1: the flat-tree launch (its ticket space holds flat-tree plans only; phrase plans never take that path; GOOGLE only)
-        const void *fn;
-        if (P.ix.codec != 0)
-                fn = P.has_phrase ? (const void *)k_exec_docs<true, false, true> : (const void *)k_exec_docs<false, false, true>;
-        else
-                fn = P.gen_sel ? (const void *)k_exec_docs<false, true, false>
-                               : (P.has_phrase ? (const void *)k_exec_docs<true, false, false> : (const void *)k_exec_docs<false, false, false>);
+        const bool  lucene = P.ix.codec != 0, tree = !lucene && P.gen_sel;
+        const void *fn     = exec_docs_fn(P.has_phrase && !tree, tree, lucene, P.filters != nullptr);
         cudaError_t  e    = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess)
                 return e;

@@ -120,7 +120,9 @@ __device__ __forceinline__ bool google_block_find(const uint8_t *__restrict__ in
 // The query's program is [OP_LEAF lead, OP_LEAF term 1, ..., OP_TABLE x2]: terms 1 .. Q.root_slot-1 are NECESSARY (a candidate without
 // them is dropped at once); the others only set their bit in the candidate's membership byte, and the truth table (bit m = value of
 // the query when exactly the terms in m are present; bit 0 of m = the lead) decides at the end.
-__device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t curq, uint32_t item, uint32_t group, uint32_t *cand, int lane) {
+// FILT: the query may have a document filter (ExecParams::filters): a group wholly outside its allow set's span is skipped, and the
+// filter drops documents beside the masked ones.
+template <bool FILT> __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_t curq, uint32_t item, uint32_t group, uint32_t *cand, int lane) {
         uint8_t *const stage = reinterpret_cast<uint8_t *>(cand + kCandWords);
         uint8_t *const cmask = stage + kGatherBufBytes;
         // lane j adopts the j-th term; lane w (< 8) keeps word w of the truth table
@@ -157,6 +159,22 @@ __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_
         }
         // ---- 1. the lead's blocks -> candidates
         const uint32_t dir0 = __shfl_sync(0xffffffffu, mydir, 0), nb0 = __shfl_sync(0xffffffffu, mynb, 0), docs0 = __shfl_sync(0xffffffffu, mydocs, 0);
+        DevFilter      F{};
+        if constexpr (FILT) {
+                F = P.filters[curq];
+                // the group's docIDs lie in (last docID of the block before it, last docID of its last block]
+                const uint32_t b0 = group * 32u, b1 = min(nb0, b0 + 32u);
+                const bool     out = b0 >= b1 || F.lo > F.hi || __ldg(P.ix.blk_last + dir0 + b1 - 1u) < F.lo || (b0 && __ldg(P.ix.blk_last + dir0 + b0 - 1u) >= F.hi);
+                if (out) {
+                        if (lane == 0) {
+                                P.item_off[item] = 0;
+                                P.item_cnt[item] = 0;
+                                if (P.item_desc)
+                                        P.item_desc[item] = 0;
+                        }
+                        return;
+                }
+        }
         uint32_t       n = 0;
         {
                 const uint32_t b    = group * 32u + uint32_t(lane);
@@ -261,6 +279,10 @@ __device__ void cand_exec_google(const ExecParams &P, const DevQuery &Q, uint32_
                 }
                 if (ok && P.ix.masked)
                         ok = ((__ldg(P.ix.masked + (c >> 5)) >> (c & 31u)) & 1u) == 0u;
+                if constexpr (FILT) {
+                        if (ok)
+                                ok = (filter_keep(F, c >> 5) >> (c & 31u)) & 1u;
+                }
                 const uint32_t vm = __ballot_sync(0xffffffffu, ok);
                 if (uint32_t(lane) == j)
                         mymask = vm;

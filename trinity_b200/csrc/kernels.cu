@@ -456,9 +456,21 @@ __device__ __forceinline__ unsigned long long make_key(float score, uint32_t doc
 // ------------------------------------------------------------------------------------------------ the fused kernel
 extern __shared__ __align__(16) uint8_t dyn_smem[];
 
+// the documents of word wi (docIDs [32 wi, 32 wi + 32)) that a query's filter keeps: in its allow set (if it has one) and not in its deny
+// set (IndexDocumentsFilter::filter, exec.cpp:1108-1116).  Only the filtered instantiations (FILT) call it.
+__device__ __forceinline__ uint32_t filter_keep(const DevFilter &F, uint32_t wi) {
+        uint32_t k = 0xffffffffu;
+        if (F.allow)
+                k = __ldg(F.allow + wi);
+        if (F.deny)
+                k &= ~__ldg(F.deny + wi);
+        return k;
+}
+
 // PH: the instantiation that also executes OP_PHRASE (position checks, phrase.cuh) — used only for batches that hold phrase nodes, so that
-// the cursor code costs the common instantiation neither registers nor a stack frame
-template <bool PH> __global__ void __launch_bounds__(kThreads) k_exec_tiles(ExecParams P) {
+// the cursor code costs the common instantiation neither registers nor a stack frame.  FILT: likewise for batches that hold a query with a
+// document filter (ExecParams::filters)
+template <bool PH, bool FILT> __global__ void __launch_bounds__(kThreads) k_exec_tiles(ExecParams P) {
         const uint32_t W     = 1u << P.exec_shift;
         const uint32_t NW    = W >> 5; // bitmap words per slot
         const bool     scored = P.mode != 0;
@@ -684,6 +696,16 @@ template <bool PH> __global__ void __launch_bounds__(kThreads) k_exec_tiles(Exec
                         for (uint32_t i = tid; i < NW; i += kThreads)
                                 r[i] &= ~mk[i];
                         __syncthreads();
+                }
+                // ... and neither do the documents the query's filter drops: they take no top-k candidate slot and never move theta
+                if constexpr (FILT) {
+                        if (!dead) {
+                                const DevFilter F = P.filters[q];
+                                uint32_t *      r = slots + size_t(Q.root_slot) * NW;
+                                for (uint32_t i = tid; i < NW; i += kThreads)
+                                        r[i] &= filter_keep(F, (lo >> 5) + i);
+                                __syncthreads();
+                        }
                 }
                 // ---------------------------------------------------------------- emission
                 const uint32_t *root = slots + size_t(Q.root_slot) * NW;
@@ -965,7 +987,8 @@ size_t exec_smem_bytes(uint32_t tile_shift, uint32_t nslots, int mode, int codec
 
 cudaError_t launch_exec_tiles(const ExecParams &P, int grid, cudaStream_t stream) {
         const size_t smem = exec_smem_bytes(P.exec_shift, P.nslots, P.mode, P.ix.codec);
-        const void * fn   = P.has_phrase ? (const void *)k_exec_tiles<true> : (const void *)k_exec_tiles<false>;
+        const void * fn   = P.filters ? (P.has_phrase ? (const void *)k_exec_tiles<true, true> : (const void *)k_exec_tiles<false, true>)
+                                      : (P.has_phrase ? (const void *)k_exec_tiles<true, false> : (const void *)k_exec_tiles<false, false>);
         cudaError_t  e    = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess)
                 return e;
@@ -973,15 +996,17 @@ cudaError_t launch_exec_tiles(const ExecParams &P, int grid, cudaStream_t stream
         return cudaLaunchKernel(fn, dim3(grid), dim3(kThreads), args, smem, stream);
 }
 
-int exec_max_ctas_per_sm(uint32_t tile_shift, uint32_t nslots, int mode, int codec) {
+int exec_max_ctas_per_sm(uint32_t tile_shift, uint32_t nslots, int mode, int codec, bool filt) {
         const size_t smem = exec_smem_bytes(tile_shift, nslots, mode, codec);
         // (the phrase instantiation needs at least as many registers: size the grid for it when in doubt — a smaller grid is still correct)
-        if (cudaFuncSetAttribute(k_exec_tiles<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess ||
-            cudaFuncSetAttribute(k_exec_tiles<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess)
+        const void *a = filt ? (const void *)k_exec_tiles<false, true> : (const void *)k_exec_tiles<false, false>;
+        const void *b = filt ? (const void *)k_exec_tiles<true, true> : (const void *)k_exec_tiles<true, false>;
+        if (cudaFuncSetAttribute(a, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess ||
+            cudaFuncSetAttribute(b, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess)
                 return 0;
         int n = 0, m = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_exec_tiles<false>, kThreads, smem) != cudaSuccess ||
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m, k_exec_tiles<true>, kThreads, smem) != cudaSuccess)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, a, kThreads, smem) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m, b, kThreads, smem) != cudaSuccess)
                 return 0;
         return std::min(n, m);
 }

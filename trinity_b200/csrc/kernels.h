@@ -7,13 +7,13 @@
 namespace trn {
 uint32_t    exec_stage_bytes(int codec);
 size_t      exec_smem_bytes(uint32_t tile_shift, uint32_t nslots, int mode, int codec);
-int         exec_max_ctas_per_sm(uint32_t tile_shift, uint32_t nslots, int mode, int codec);
+int         exec_max_ctas_per_sm(uint32_t tile_shift, uint32_t nslots, int mode, int codec, bool filt = false); // filt: the filtered instantiations
 cudaError_t launch_exec_tiles(const ExecParams &P, int grid, cudaStream_t stream);
 uint32_t    exec_docs_stage_bytes();
 uint32_t    exec_docs_cand_smem_bytes(bool with_membership); // per-warp shared memory of the candidate-driven path (membership bytes: trees with terms that are not necessary)
 uint32_t    exec_docs_mixed_smem_bytes(); // per-warp shared memory of the mixed flat ANDs' run tickets (the candidate array, one gather buffer, counters)
 size_t      exec_docs_smem_bytes(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes);
-int         exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes, bool tree = false, bool lucene = false);
+int         exec_docs_max_ctas_per_sm(uint32_t exec_shift, uint32_t nslots, uint32_t stageBytes, bool tree = false, bool lucene = false, bool filt = false);
 cudaError_t launch_exec_docs(const ExecParams &P, int grid, cudaStream_t stream);
 cudaError_t launch_query_scan(const unsigned long long *match_counts, uint32_t nq, uint64_t *q_offsets, cudaStream_t stream);
 cudaError_t launch_item_scan(const DevQuery *queries, uint32_t nq, const uint32_t *item_cnt, const uint64_t *q_offsets, uint64_t *item_dst, cudaStream_t stream);

@@ -1050,7 +1050,7 @@ static int fail(std::string &err, int code, const std::string &m) {
 }
 
 int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
-                    uint32_t k, BatchPlan &out, std::string &err) {
+                    uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip) {
         out                = BatchPlan{};
         const bool scored  = mode == TRN_MODE_SCORED_ALL || mode == TRN_MODE_SCORED_TOPK;
         if (mode == TRN_MODE_MATCHED_TERMS) { // the DocumentsOnly program, plus what the collect pass runs per match
@@ -1104,7 +1104,11 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                 }
                 out.postings += cc.postings;
                 out.bytes += cc.bytes;
-                const Range r = cc.range(cc.root); // cc.root: the effective root (see apply_reference_root_filter_quirk)
+                Range r = cc.range(cc.root); // cc.root: the effective root (see apply_reference_root_filter_quirk)
+                if (clip) { // no match lies outside the query's allow set: its tiles there are not evaluated
+                        r.lo = std::max(r.lo, clip[q].x);
+                        r.hi = std::min(r.hi, clip[q].y);
+                }
                 // Flat scored disjunction (a k-term OR / a single term, every leaf scoring with a weight >= +0.0) on the LUCENE codec:
                 // k_score_flat (score_flat.cuh) instead of the step program
                 bool flatScored{false};

@@ -81,9 +81,10 @@ int plan_collect(const std::vector<DevTerm> &terms, const trn_query *queries, ui
 // Plans a batch (mode: TRN_MODE_*; k: top-k; TRN_MODE_MATCHED_TERMS: the DocumentsOnly program without the root-filter quirk, plus
 // BatchPlan::collect).  dense_off: per term, the first word of its resident bitmap (DenseSelection::off), or
 // null when the source has none.  Returns TRN_OK, or an error code with its message in err: TRN_ERR_ARG / TRN_ERR_UNSUPPORTED for a
-// plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.
+// plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.  clip (null: none): per query the inclusive docID span its
+// matches can lie in (its allow set's first and last docID; x > y: none), to which its tile range is clipped.
 int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
-               uint32_t k, BatchPlan &out, std::string &err);
+               uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip = nullptr);
 
 // Resident docID bitmaps of dense terms (GOOGLE sources; LUCENE sources get none).  A selected term owns one bitmap over its own docID
 // span, both ends aligned to 2^kDenseAlignShift docIDs — the largest tile of any k_exec_docs launch — so every tile of every launch lies

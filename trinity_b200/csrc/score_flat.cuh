@@ -178,7 +178,8 @@ template <int NT> __device__ __forceinline__ uint32_t sf_prune(unsigned long lon
 static constexpr uint32_t kSfCacheLeaves = 12;                        // leaves that own a cache slot (the others always decode)
 static constexpr uint32_t kSfCacheBytes  = kSfCacheLeaves * 128 * 8;  // per leaf: 128 docIDs + 128 scores of its cached (tile-straddling) block
 
-template <int NT>
+// FILT: the instantiation for batches that hold a query with a document filter (ScoreParams::filters)
+template <int NT, bool FILT>
 __global__ void __launch_bounds__(NT, NT <= 384 ? 2 : 1) k_score_flat(ScoreParams S) {
         constexpr int      NWARPS       = NT / 32;
         constexpr uint32_t kSfListCap   = SfCap<NT>::value;
@@ -456,6 +457,22 @@ __global__ void __launch_bounds__(NT, NT <= 384 ? 2 : 1) k_score_flat(ScoreParam
                         }
                         __syncthreads(); // ---- every posting of the tile has been scored
 
+                        if constexpr (FILT) { // the documents the query's filter drops leave the score tile: not counted, no candidate slot, no theta
+                                const DevFilter F = S.filters[q];
+                                for (uint32_t i4 = tid; i4 < W4; i4 += NT) {
+                                        const uint32_t m = (filter_keep(F, (lo >> 5) + (i4 >> 3)) >> ((i4 & 7u) * 4u)) & 0xfu;
+                                        if (m != 0xfu) {
+                                                float4 v = reinterpret_cast<const float4 *>(acc)[i4];
+                                                if (!(m & 1u)) v.x = sent4.x;
+                                                if (!(m & 2u)) v.y = sent4.y;
+                                                if (!(m & 4u)) v.z = sent4.z;
+                                                if (!(m & 8u)) v.w = sent4.w;
+                                                reinterpret_cast<float4 *>(acc)[i4] = v;
+                                        }
+                                }
+                                __syncthreads();
+                        }
+
                         const uint32_t *mk = S.ix.masked ? S.ix.masked + (lo >> 5) : nullptr;
                         if (S.mode == 2) {
                                 // ---- threshold scan: as signed integers the sentinel is INT_MIN and scores (>= +0.0) order like their bits
@@ -639,7 +656,8 @@ cudaError_t launch_build_luts(const FlatLeaf *leaves, uint32_t nleaves, float *l
 cudaError_t launch_score_flat(const ScoreParams &S, int threads, int num_sms, cudaStream_t stream) {
         if (threads != 512)
                 threads = 320;
-        const void *fn = threads == 512 ? (const void *)k_score_flat<512> : (const void *)k_score_flat<320>;
+        const void *fn = S.filters ? (threads == 512 ? (const void *)k_score_flat<512, true> : (const void *)k_score_flat<320, true>)
+                                   : (threads == 512 ? (const void *)k_score_flat<512, false> : (const void *)k_score_flat<320, false>);
         const size_t smem = score_flat_smem_bytes(S.tile_shift, threads);
         cudaError_t  e    = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess)

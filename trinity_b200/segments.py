@@ -7,12 +7,13 @@ their own engine context; a query batch runs once per segment, exactly like the 
 application."""
 from __future__ import annotations
 
+import hashlib
 import os
-from typing import List, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from . import (EMPTY_TERM, NODE_TERM, GpuIndexSource, MergedSegment, MergeSource, Segment, TermDictionary, bm25_idf, parse_query)
+from . import (EMPTY_TERM, NODE_TERM, DocFilter, DocSet, GpuIndexSource, MergedSegment, MergeSource, Segment, TermDictionary, bm25_idf, parse_query)
 
 
 def generation_of(path: str) -> int:
@@ -36,6 +37,7 @@ class SegmentCollection:
             for n, t in zip(s.names, s.terms):
                 self._df[n] = self._df.get(n, 0) + int(t["documents"])
         self.sources: List[GpuIndexSource] = []
+        self._docsets: Dict[bytes, List[DocSet]] = {}  # the sets exec_batch registered, by content: one per source
         newer = np.zeros(0, np.uint32)
         for s in self.segments:
             g = GpuIndexSource(device)
@@ -82,9 +84,45 @@ class SegmentCollection:
                 acc[m] = acc.get(m, 0) + c
         return sorted(acc.items())
 
-    def exec_batch(self, queries: Sequence[str], mode: int, k: int = 100):
-        """-> [BatchResult per segment], collection order (newest first)"""
+    def docsets(self, docids) -> List[DocSet]:
+        """the docID set of these (global) docIDs in every source, collection order; a set passed again is the one registered before"""
+        d = np.unique(np.asarray(docids, dtype=np.uint32))
+        key = hashlib.sha1(d.tobytes()).digest()
+        if key not in self._docsets:
+            self._docsets[key] = [g.docset(d) for g in self.sources]
+        return self._docsets[key]
+
+    def release_docsets(self):
+        """destroy every set exec_batch / docsets registered (each is a bitmap of the docID space in every source)"""
+        for sets in self._docsets.values():
+            for d in sets:
+                d.close()
+        self._docsets.clear()
+
+    def filters(self, nq: int, allow=None, deny=None) -> Optional[List[List[Optional[DocFilter]]]]:
+        """per source, one DocFilter (or None) per query from per-query allow / deny docID arrays (None: that side is open); None when no
+        query has either"""
+        allow = [None] * nq if allow is None else list(allow)
+        deny = [None] * nq if deny is None else list(deny)
+        if len(allow) != nq or len(deny) != nq:
+            raise ValueError("allow / deny: one entry (or None) per query")
+        if all(a is None for a in allow) and all(d is None for d in deny):
+            return None
+        per = [[None] * nq for _ in self.sources]
+        for q in range(nq):
+            a = self.docsets(allow[q]) if allow[q] is not None else None
+            d = self.docsets(deny[q]) if deny[q] is not None else None
+            if a is None and d is None:
+                continue
+            for i in range(len(self.sources)):
+                per[i][q] = DocFilter(a[i] if a else None, d[i] if d else None)
+        return per
+
+    def exec_batch(self, queries: Sequence[str], mode: int, k: int = 100, allow=None, deny=None):
+        """-> [BatchResult per segment], collection order (newest first).  allow / deny: per query None or an array of global docIDs
+        (docIDs are global across generations: every source registers the same set, and a set passed again is reused)"""
         from . import MODE_DOCS_ONLY
         scored = mode != MODE_DOCS_ONLY
         per_q = [self.plans(q, scored) for q in queries]
-        return [g.exec_batch([pq[i] for pq in per_q], mode, k) for i, g in enumerate(self.sources)]
+        f = self.filters(len(queries), allow, deny)
+        return [g.exec_batch([pq[i] for pq in per_q], mode, k, filters=None if f is None else f[i]) for i, g in enumerate(self.sources)]
