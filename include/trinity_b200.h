@@ -341,6 +341,12 @@ int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const
  * all-bitmap ones (TRN_MIXED_RUNS=0 turns them off).  Same arguments and rows as trn_debug_dense_runs. */
 int trn_debug_mixed_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
                          uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n, char *err, size_t errcap);
+/* The same for the candidate-driven queries (TRN_ROUTE_CANDIDATE): one ticket per 32-block group of the query's lead term, ordered by the
+ * 2^17-docID run of the group's first docID, queries ascending within a run; they follow the flat ANDs' run tickets (TRN_CAND_RUNS=0
+ * turns them off: the groups then take tickets in query order).  qtiles[2q + 1] = the groups of query q; ticket t = tickets[3t .. 3t + 2]:
+ * the query, the group and the group's first docID (the last docID of the block before it plus one; the lead's first docID for group 0). */
+int trn_debug_cand_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid, const trn_query *queries,
+                        uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n, char *err, size_t errcap);
 
 /* Host-only view of the dense-term selection (tests, tooling; no GPU needed): the terms trn_upload_index would keep a resident docID
  * bitmap for on a context that trn_create made with this environment (TRN_DENSE_BITMAPS, TRN_DENSE_BUDGET).  A GOOGLE term qualifies when

@@ -1,17 +1,24 @@
-"""Time the and2 batch of bench.py by route class: with the flat ANDs on their run-major tickets (the default), with TRN_MIXED_RUNS=0 (the
-flat ANDs with one bitmap operand on per-tile tickets) and with TRN_DENSE_RUNS=0 TRN_MIXED_RUNS=0 (every flat AND on per-tile tickets).
+"""Time the and2 batch of bench.py by route class, on sources created with different ticket orders, alternating: the default (every run-major
+ticket space on), TRN_CAND_RUNS=0 (candidate-driven groups in query order), and on request TRN_MIXED_RUNS=0 (the flat ANDs with one
+bitmap operand on per-tile tickets) and TRN_DENSE_RUNS=0 TRN_MIXED_RUNS=0 (every flat AND on per-tile tickets).
 
 Builds bench.py's GOOGLE index and and2 batch, splits the batch into
-  both    flat AND, both operands with a resident bitmap
-  one     flat AND, one operand with a bitmap
-  none    flat AND, no bitmap
-  cand    candidate-driven
-and times each class as its own device-resident batch (exec_batch_device, as bench.py; CUDA events over --steps steps after --warmup) on
-three sources over the same index, created with those settings, alternating.  Per class it prints ms per step, (query, tile) work
-items (candidate-driven: lead-term groups), matches, result words, and the modelled HBM bytes of bitmap reads: per-tile order (every
-item reads its operands' tile words) and run-major order (every bitmap run read once).  Needs a GPU; prints the card and its power limit.
+  both        flat AND, both operands with a resident bitmap
+  one         flat AND, one operand with a bitmap
+  none        flat AND, no bitmap
+  cand_bitmap candidate-driven, every probed operand with a bitmap
+  cand_dir    candidate-driven, at least one operand probed through its block directory
+and times each class as its own device-resident batch (exec_batch_device, as bench.py; CUDA events over --steps steps after --warmup).
+Per class it prints ms per step, (query, tile) work items (candidate-driven: lead-term groups), matches, result words, and a model of
+the HBM traffic of bitmap reads:
+  * flat ANDs: per-tile order (every item reads its operands' tile words) and run-major order (every bitmap run read once);
+  * candidate-driven: the probes issued (an upper bound: every lead document against every other operand) and the 32-byte bitmap
+    sectors they read — in query order (the 16 bitmaps are several times L2, so each query's probes read their own sectors: the
+    expected distinct sectors of its lead documents in each bitmap) and in run-major order (the queries in flight share a docID window,
+    so each bitmap sector is read once per batch: the expected distinct sectors of all the class's probes of that bitmap).
+Directory probes (cand_dir) are counted, not modelled.  Needs a GPU; prints the card and its power limit.
 
-    python scripts/and2_breakdown.py [--ndocs 100000000] [--steps 20] [--warmup 5]
+    python scripts/and2_breakdown.py [--ndocs 100000000] [--steps 20] [--warmup 5] [--settings runs,cand_query_order]
 """
 import argparse
 import json
@@ -28,7 +35,13 @@ import bench  # noqa: E402
 import trinity_b200 as tb  # noqa: E402
 
 
-SETTINGS = {"runs": {}, "mixed_tiles": {"TRN_MIXED_RUNS": "0"}, "tiles": {"TRN_DENSE_RUNS": "0", "TRN_MIXED_RUNS": "0"}}
+SETTINGS = {"runs": {}, "cand_query_order": {"TRN_CAND_RUNS": "0"}, "mixed_tiles": {"TRN_MIXED_RUNS": "0"},
+            "tiles": {"TRN_DENSE_RUNS": "0", "TRN_MIXED_RUNS": "0"}}
+
+
+def distinct_sectors(probes, sectors):
+    """expected distinct sectors hit by `probes` uniformly spread probes over `sectors` sectors"""
+    return sectors * -np.expm1(-probes / sectors) if sectors else 0.0
 
 
 def source(synth, ndocs, env):
@@ -49,14 +62,16 @@ def main():
     ap.add_argument("--nq", type=int, default=1000)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--rounds", type=int, default=3, help="alternations of the two sources per class")
+    ap.add_argument("--rounds", type=int, default=3, help="alternations of the sources per class")
+    ap.add_argument("--settings", default="runs,cand_query_order", help=f"comma-separated sources to time, of {list(SETTINGS)}")
     args = ap.parse_args()
+    settings = {k: SETTINGS[k] for k in args.settings.split(",")}
     import torch
 
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     synth = tb.SynthIndex(tb.CODEC_GOOGLE, args.ndocs, args.nterms, threads=max(1, len(os.sched_getaffinity(0))))
-    srcs = {k: source(synth, args.ndocs, env) for k, env in SETTINGS.items()}
-    g = srcs["runs"]
+    srcs = {k: source(synth, args.ndocs, env) for k, env in settings.items()}
+    g = next(iter(srcs.values()))
     texts, _ = bench.gen_queries("and2", args.nq, args.nterms)
     tdict = tb.TermDictionary(synth.names)
     plans = [tb.parse_query(q, tdict) for q in texts]
@@ -73,12 +88,17 @@ def main():
 
     tile = 1 << 14
     tiles = (args.ndocs >> 14) + 1  # the synthetic terms spread over the whole docID range
-    classes = {"both": [], "one": [], "none": [], "cand": []}
+    classes = {"both": [], "one": [], "none": [], "cand_bitmap": [], "cand_dir": []}
+    docs = lambda t: int(terms["documents"][t])
     for i, p in enumerate(plans):
         ts = [int(x["term"]) for x in p if x["kind"] == tb.NODE_TERM]
         nd = sum(bitmap_bytes(t) > 0 for t in ts)
         if routes[i] == tb.ROUTE_CANDIDATE:
-            classes["cand"].append(i)
+            # a model of the planner's choice, not the planner's own: the rarest term (by blocks) leads (and2: both terms are necessary);
+            # plan_batch breaks a tie in block counts by an unstable sort, so on a tie its lead may be the other term
+            lead = min(ts, key=lambda t: (-(-docs(t) // 32), ts.index(t)))
+            probed = [t for t in ts if t != lead]
+            classes["cand_bitmap" if all(bitmap_bytes(t) for t in probed) else "cand_dir"].append(i)
         elif routes[i] == tb.ROUTE_FLAT_AND:
             classes["both" if nd == len(ts) else "one" if nd else "none"].append(i)
     print(json.dumps({"card": card, "ndocs": args.ndocs, "nq": args.nq, "dense_terms": g.info()["dense_terms"],
@@ -90,11 +110,24 @@ def main():
         sub = [plans[i] for i in qs]
         items = old_b = 0
         used = set()
+        probes = dir_probes = 0
+        sec_query = 0.0
+        per_bitmap = {}  # bitmap term -> probes of the class against it
         for i in qs:
             ts = [int(x["term"]) for x in plans[i] if x["kind"] == tb.NODE_TERM]
-            if name == "cand":  # 32-block groups of the lead (rarest) term
-                lead_blocks = -(-min(int(terms["documents"][t]) for t in ts) // 32)
+            if name.startswith("cand"):  # 32-block groups of the lead (rarest) term
+                lead = min(ts, key=lambda t: (-(-docs(t) // 32), ts.index(t)))  # (the model of the lead above)
+                lead_blocks = -(-docs(lead) // 32)
                 items += -(-lead_blocks // 32)
+                for t in ts:
+                    if t == lead:
+                        continue
+                    probes += docs(lead)
+                    if bitmap_bytes(t):
+                        sec_query += distinct_sectors(docs(lead), bitmap_bytes(t) // 32)
+                        per_bitmap[t] = per_bitmap.get(t, 0) + docs(lead)
+                    else:
+                        dir_probes += docs(lead)
             else:
                 items += tiles
                 nd = [t for t in ts if bitmap_bytes(t)]
@@ -116,10 +149,17 @@ def main():
                 torch.cuda.synchronize()
                 ms[key].append(e0.elapsed_time(e1) / args.steps)
         res = g.exec_batch(sub, tb.MODE_DOCS_COMPACT, copy=False)
-        print(json.dumps({"class": name, "queries": len(qs), "work_items": items, "matches": int(res.match_counts.sum()),
-                          "result_bytes": res.result_bytes(), **{f"ms_per_step_{k}": [round(x, 3) for x in v] for k, v in ms.items()},
-                          "bitmap_bytes_per_tile_order": old_b,
-                          "bitmap_bytes_run_major": new_b}))
+        row = {"class": name, "queries": len(qs), "work_items": items, "matches": int(res.match_counts.sum()),
+               "result_bytes": res.result_bytes(), **{f"ms_per_step_{k}": [round(x, 3) for x in v] for k, v in ms.items()},
+               **{f"ms_median_{k}": round(float(np.median(v)), 3) for k, v in ms.items()}}
+        if name.startswith("cand"):
+            sec_run = sum(distinct_sectors(n, bitmap_bytes(t) // 32) for t, n in per_bitmap.items())
+            row.update({"probes_upper_bound": probes, "directory_probes_upper_bound": dir_probes, "bitmap_sectors_query_order": round(sec_query),
+                        "bitmap_sectors_run_major": round(sec_run), "bitmap_bytes_query_order": round(sec_query) * 32,
+                        "bitmap_bytes_run_major": round(sec_run) * 32})
+        else:
+            row.update({"bitmap_bytes_per_tile_order": old_b, "bitmap_bytes_run_major": new_b})
+        print(json.dumps(row))
     for s in srcs.values():
         s.close()
 

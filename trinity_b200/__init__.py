@@ -322,6 +322,13 @@ def debug_mixed_runs(codec: int, index: np.ndarray, terms: np.ndarray, queries: 
     return _debug_run_tickets(lib().trn_debug_mixed_runs, codec, index, terms, queries, mode, k, max_docid)
 
 
+def debug_cand_runs(codec: int, index: np.ndarray, terms: np.ndarray, queries: Sequence[np.ndarray], mode: int, k: int = 100, max_docid: int = 0):
+    """(qgroups, tickets): the candidate-driven queries' run-major tickets as the planner lays them out (no GPU needed).  qgroups[q, 1] is
+    query q's count of 32-block lead groups; a ticket row is (query, group, the group's first docID), ordered by that docID's 2^17-docID run,
+    queries ascending within a run.  Empty with TRN_CAND_RUNS=0, on LUCENE, in the scored modes and beside a phrase plan."""
+    return _debug_run_tickets(lib().trn_debug_cand_runs, codec, index, terms, queries, mode, k, max_docid)
+
+
 def _debug_run_tickets(fn, codec, index, terms, queries, mode, k, max_docid):
     index = np.ascontiguousarray(index, dtype=np.uint8)
     terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)

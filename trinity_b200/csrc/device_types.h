@@ -176,7 +176,9 @@ struct ExecParams {
         const uint2 *   dense_runs;  // k_exec_docs, step-program launch: tickets [0, dense_items) are the all-bitmap flat ANDs' (query, run) pairs
         uint32_t        dense_items; // (BatchPlan::dense_runs)
         const uint2 *   mixed_runs;  // ... then tickets [dense_items, dense_items + mixed_items): the flat ANDs with one decoded operand
-        uint32_t        mixed_items; // (BatchPlan::mixed_runs); the tickets of gen_items follow them
+        uint32_t        mixed_items; // (BatchPlan::mixed_runs)
+        const uint32_t *cand_order;  // ... then cand_items tickets: ticket i runs gen ticket cand_order[i] (candidate-driven groups, run-major);
+        uint32_t        cand_items;  // the gen tickets follow, and skip those of candidate-driven queries when cand_items != 0
         uint32_t        has_phrase; // some plan of the batch holds OP_PHRASE: launch the instantiation that executes it
         uint32_t        nslots; // bitmap slots per worker (CTA for k_exec_tiles, warp for k_exec_docs)
         uint32_t        stage_bytes; // per-warp staging bytes of k_exec_tiles (codec dependent)

@@ -115,8 +115,9 @@ struct trn_ctx {
         uint64_t             dense_bytes{0};
         std::vector<uint32_t> h_dense_off;          // host copy of d_dense_off (trn_debug_dense_bitmap)
         std::vector<DevTerm> h_terms;
+        GroupStarts          h_groups; // GOOGLE: the first docID of every 32-block group of every term (orders BatchPlan::cand_runs)
         // batch scratch (grow-only)
-        DevBuf d_queries, d_steps, d_dense_runs, d_mixed_runs, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
+        DevBuf d_queries, d_steps, d_dense_runs, d_mixed_runs, d_cand_order, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
             d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
         PinBuf h_offsets, h_docids, h_scores, h_counts, h_small, h_chunk, h_item_desc;
         DevBuf d_hits, d_hit_base, d_hblk_off, d_hit_term; // LUCENE positions (trn_upload_hits)
@@ -335,7 +336,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_small[0], &c->d_small[1], &c->d_item_off,
+        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_cand_order, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores, &c->d_filters})
@@ -461,8 +462,11 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         } catch (const std::exception &e) {
                 return fail(c, TRN_ERR_FORMAT, e.what());
         }
+        GroupStarts gs;
         try {
                 ht = dev_terms(dir, terms, nterms);
+                if (codec == TRN_CODEC_GOOGLE)
+                        gs = group_starts(dir);
         } catch (const std::bad_alloc &) {
                 return fail(c, TRN_ERR_CAPACITY, "trn_upload_index: out of host memory");
         }
@@ -478,6 +482,7 @@ extern "C" int trn_upload_index(trn_ctx *c, int codec, const uint8_t *index, uin
         const uint32_t W = 1u << c->pc.tile_shift;
         c->ntiles       = uint32_t((uint64_t(max_docid) + 1 + W - 1) >> c->pc.tile_shift);
         c->h_terms      = std::move(ht);
+        c->h_groups     = std::move(gs);
         c->total_blocks   = 0;
         c->total_postings = 0;
         for (const auto &d : c->h_terms) {
@@ -795,7 +800,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         BatchPlan   plan;
         std::string perr;
         const int   prc = plan_batch(c->pc, c->h_terms, c->dense_terms ? c->h_dense_off.data() : nullptr, queries, nq, collect ? TRN_MODE_MATCHED_TERMS : mode, k, plan,
-                                     perr, filtered ? clip.data() : nullptr);
+                                     perr, filtered ? clip.data() : nullptr, c->h_groups.base.empty() ? nullptr : &c->h_groups);
         if (prc != TRN_OK)
                 return fail(c, prc, perr);
         if (collect)
@@ -886,6 +891,11 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                 CK(c->d_mixed_runs.ensure(size_t(mixedItems) * sizeof(uint2)));
                 CK(cudaMemcpyAsync(c->d_mixed_runs.p, plan.mixed_runs.data(), size_t(mixedItems) * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
         }
+        const uint32_t candItems = uint32_t(plan.cand_order.size());
+        if (candItems) {
+                CK(c->d_cand_order.ensure(size_t(candItems) * sizeof(uint32_t)));
+                CK(cudaMemcpyAsync(c->d_cand_order.p, plan.cand_order.data(), size_t(candItems) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+        }
         CK(cudaMemsetAsync(small, 0, smallBytes, c->stream));
 
         ExecParams P;
@@ -900,6 +910,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         P.dense_items  = denseItems;
         P.mixed_runs   = mixedItems ? c->d_mixed_runs.as<uint2>() : nullptr;
         P.mixed_items  = mixedItems;
+        P.cand_order   = candItems ? c->d_cand_order.as<uint32_t>() : nullptr;
+        P.cand_items   = candItems;
         P.has_phrase   = plan.any_phrase ? 1u : 0u;
         P.nslots       = plan.nslots;
         P.exec_shift   = execShift;
@@ -926,7 +938,7 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
         uint32_t launches{0};
         if (totalItems) {
                 const bool     warpKernel = !scored;
-                const uint64_t ownItems   = plan.gen_items + denseItems + mixedItems; // tickets of the step-program launch
+                const uint64_t ownItems   = plan.gen_items + denseItems + mixedItems + candItems; // tickets of the step-program launch
                 CK(cudaEventRecord(k0, c->stream));
                 if (nflat && plan.flat_items) {
                         // flat scored disjunctions: per-leaf BM25 tables once per batch, then k_score_flat
@@ -982,6 +994,8 @@ static int exec_device_impl(trn_ctx *c, const trn_query *queries, uint32_t nq, i
                         P2.dense_items = 0;
                         P2.mixed_runs  = nullptr;
                         P2.mixed_items = 0;
+                        P2.cand_order  = nullptr;
+                        P2.cand_items  = 0;
                         P2.ticket     = reinterpret_cast<uint32_t *>(small + 4);
                         const int perSM = exec_docs_max_ctas_per_sm(P2.exec_shift, P2.nslots, exec_docs_stage_bytes(), true, false, filtered);
                         if (perSM <= 0)
@@ -1583,7 +1597,8 @@ extern "C" int trn_exec_matches_filtered(trn_ctx *c, const trn_query *queries, u
 }
 
 static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
-                            const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &plan, char *err, size_t errcap) {
+                            const trn_query *queries, uint32_t nq, int mode, uint32_t k, BatchPlan &plan, char *err, size_t errcap,
+                            GroupStarts *groups = nullptr) {
         auto seterr = [&](const std::string &m, int rc) {
                 if (err && errcap) {
                         std::strncpy(err, m.c_str(), errcap - 1);
@@ -1595,9 +1610,12 @@ static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, co
                 return seterr("bad arguments", TRN_ERR_ARG);
         BlockDirectory       dir;
         std::vector<DevTerm> ht;
+        GroupStarts          gs;
         try {
                 build_directory(codec, index, nbytes, terms, nterms, 1, dir);
                 ht = dev_terms(dir, terms, nterms);
+                if (codec == TRN_CODEC_GOOGLE)
+                        gs = group_starts(dir);
         } catch (const std::exception &e) {
                 return seterr(e.what(), TRN_ERR_FORMAT);
         }
@@ -1608,7 +1626,10 @@ static int debug_plan_batch(int codec, const uint8_t *index, uint64_t nbytes, co
         pc.max_docid            = max_docid;
         const DenseSelection ds = select_dense_terms(pc, ht, nbytes); // what trn_upload_index keeps
         std::string          perr;
-        const int            rc = plan_batch(pc, ht, ds.order.empty() ? nullptr : ds.off.data(), queries, nq, mode, k, plan, perr);
+        const int            rc = plan_batch(pc, ht, ds.order.empty() ? nullptr : ds.off.data(), queries, nq, mode, k, plan, perr, nullptr,
+                                                gs.base.empty() ? nullptr : &gs);
+        if (groups)
+                *groups = std::move(gs);
         return rc == TRN_OK ? TRN_OK : seterr(perr, rc);
 }
 
@@ -1626,20 +1647,22 @@ extern "C" int trn_debug_plan(int codec, const uint8_t *index, uint64_t nbytes, 
         return TRN_OK;
 }
 
-// trn_debug_dense_runs / trn_debug_mixed_runs: the run tickets of BatchPlan::dense_runs (mixed == false) or mixed_runs
-static int debug_run_tickets(bool mixed, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+// trn_debug_dense_runs / trn_debug_mixed_runs / trn_debug_cand_runs: the run tickets of BatchPlan::dense_runs, mixed_runs or cand_runs
+enum class RunTickets { dense, mixed, cand };
+static int debug_run_tickets(RunTickets which, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
                              const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
                              char *err, size_t errcap) {
         if (!qtiles || !n)
                 return TRN_ERR_ARG;
-        BatchPlan plan;
-        if (const int rc = debug_plan_batch(codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, plan, err, errcap); rc != TRN_OK)
+        BatchPlan   plan;
+        GroupStarts gs; // the first docID of every lead group (the third word of a candidate ticket)
+        if (const int rc = debug_plan_batch(codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, plan, err, errcap, &gs); rc != TRN_OK)
                 return rc;
         for (uint32_t q = 0; q < nq; ++q) {
                 qtiles[2 * q]     = plan.queries[q].tile_lo;
                 qtiles[2 * q + 1] = plan.queries[q].ntiles;
         }
-        const std::vector<uint2> &runs = mixed ? plan.mixed_runs : plan.dense_runs;
+        const std::vector<uint2> &runs = which == RunTickets::mixed ? plan.mixed_runs : which == RunTickets::cand ? plan.cand_runs : plan.dense_runs;
         *n                             = runs.size();
         if (cap < *n)
                 return TRN_ERR_CAPACITY;
@@ -1648,7 +1671,8 @@ static int debug_run_tickets(bool mixed, int codec, const uint8_t *index, uint64
                 const DevQuery &dq = plan.queries[e.x];
                 tickets[3 * t]     = e.x;
                 tickets[3 * t + 1] = e.y;
-                tickets[3 * t + 2] = dense_run_end(e.y, dq.tile_lo, dq.ntiles, plan.exec_shift);
+                tickets[3 * t + 2] = which == RunTickets::cand ? gs.first[gs.base[plan.steps[dq.step_begin].term] + e.y]
+                                                               : dense_run_end(e.y, dq.tile_lo, dq.ntiles, plan.exec_shift);
         }
         return TRN_OK;
 }
@@ -1656,13 +1680,19 @@ static int debug_run_tickets(bool mixed, int codec, const uint8_t *index, uint64
 extern "C" int trn_debug_dense_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
                                     const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
                                     char *err, size_t errcap) {
-        return debug_run_tickets(false, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
+        return debug_run_tickets(RunTickets::dense, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
 }
 
 extern "C" int trn_debug_mixed_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
                                     const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
                                     char *err, size_t errcap) {
-        return debug_run_tickets(true, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
+        return debug_run_tickets(RunTickets::mixed, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
+}
+
+extern "C" int trn_debug_cand_runs(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t max_docid,
+                                   const trn_query *queries, uint32_t nq, int mode, uint32_t k, uint32_t *qtiles, uint32_t *tickets, uint64_t cap, uint64_t *n,
+                                   char *err, size_t errcap) {
+        return debug_run_tickets(RunTickets::cand, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
 }
 
 extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,

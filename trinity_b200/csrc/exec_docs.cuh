@@ -1062,7 +1062,7 @@ template <bool PH, bool TREE, bool LUC, bool FILT> __global__ void __launch_boun
                 if (lane == 0)
                         gitem = atomicAdd(P.ticket, 1u);
                 gitem = __shfl_sync(0xffffffffu, gitem, 0);
-                if (gitem >= P.dense_items + P.mixed_items + P.gen_items)
+                if (gitem >= P.dense_items + P.mixed_items + P.cand_items + P.gen_items)
                         break;
                 if constexpr (!PH && !TREE && !LUC) {
                         if (gitem < P.dense_items) { // all-bitmap flat AND: the query's tiles of one run
@@ -1076,6 +1076,14 @@ template <bool PH, bool TREE, bool LUC, bool FILT> __global__ void __launch_boun
                         }
                 }
                 gitem -= P.dense_items + P.mixed_items;
+                // candidate-driven groups, run-major (BatchPlan::cand_order): a run ticket names the group's own step-program ticket, marked in
+                // bit 31; the step-program tickets of those queries follow later and are skipped.  The query lookup below is the same for both.
+                if (!PH && !TREE && !LUC && gitem < P.cand_items)
+                        gitem = P.cand_order[gitem] | 0x80000000u;
+                else
+                        gitem -= P.cand_items;
+                const bool runTicket = gitem >> 31;
+                gitem &= 0x7fffffffu;
                 if (curq == 0xffffffffu || gitem < qgen || gitem - qgen >= Q.ntiles) {
                         uint32_t qlo = 0, qhi = P.nq;
                         while (qhi - qlo > 1) {
@@ -1093,6 +1101,8 @@ template <bool PH, bool TREE, bool LUC, bool FILT> __global__ void __launch_boun
                 const uint32_t item = Q.item_base + (gitem - qgen); // batch-wide (query, tile) item: index of the segment arrays
                 if constexpr (!TREE && !LUC) {
                         if (Q.route == TRN_ROUTE_CANDIDATE) { // candidate-driven conjunction: the work item is a 32-block group of the lead term
+                                if (P.cand_items && !runTicket)
+                                        continue;
                                 __syncwarp();
                                 cand_exec_google<FILT>(P, Q, curq, item, item - Q.item_base, slots, lane);
                                 continue;

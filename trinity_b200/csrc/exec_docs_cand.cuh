@@ -24,6 +24,8 @@ static constexpr uint32_t kCandMaskBytes = kCandWords;            // one members
 static constexpr uint32_t kCandSmem    = kCandBytes + kGatherBufBytes;                  // candidates | one gather buffer
 static constexpr uint32_t kCandSmemMask = kCandSmem + kCandMaskBytes;                   // ... | membership bytes (only queries with terms that are not necessary)
 static constexpr uint32_t kCandInvalid = 0xffffffffu;
+static constexpr uint32_t kCandProbeRounds = 2;                  // bitmap probes: rounds whose word loads are in flight together (at 4, k_exec_docs spills)
+static_assert(32u % kCandProbeRounds == 0, "a group's 32 rounds split into whole batches");
 
 // one lane decodes the doc section of ITS staged block into out[0..n).  Branch-free per code: the 32 lanes of a group hold blocks with
 // different mixes of 1-, 2- and 3-byte codes, and a loop that branches on the code length (with early exits) does not reconverge before
@@ -205,45 +207,10 @@ template <bool FILT> __device__ void cand_exec_google(const ExecParams &P, const
                 const uint32_t  firstt = __shfl_sync(0xffffffffu, myfirst, int(t)), lastt = __shfl_sync(0xffffffffu, mylast, int(t));
                 const uint32_t  tfbt = __shfl_sync(0xffffffffu, mytfb, int(t)), tfbaset = __shfl_sync(0xffffffffu, mytfbase, int(t)), tfst = __shfl_sync(0xffffffffu, mytfs, int(t));
                 const uint32_t *bl = P.ix.blk_last + dirt, *bo = P.ix.blk_off + dirt;
-                // a term with a resident bitmap: the probe is one word load and a bit test
                 const uint32_t  denset = __shfl_sync(0xffffffffu, mydense, int(t));
-                const uint32_t *bmt    = denset != kDenseNone ? P.ix.dense + denset : nullptr;
-                const uint32_t  baset  = (firstt >> kDenseAlignShift) << kDenseAlignShift;
                 uint32_t        alive = 0;
-                for (uint32_t j = 0; j < rounds; ++j) {
-                        const uint32_t nj = __shfl_sync(0xffffffffu, n, int(j));
-                        uint32_t       c  = uint32_t(lane) < nj ? cand[j * kCandStride + lane] : kCandInvalid;
-                        const bool     valid = c != kCandInvalid;
-                        if (!__any_sync(0xffffffffu, valid))
-                                continue;
-                        bool     hit = false, need = false;
-                        uint32_t off = 0, prev = 0, nblk = 0;
-                        if (bmt) {
-                                if (valid && c >= firstt && c <= lastt)
-                                        hit = (__ldg(bmt + ((c - baset) >> 5)) >> (c & 31u)) & 1u;
-                        } else if (valid && nbt) {
-                                // the one block that can hold c: first block whose last document is >= c
-                                const uint32_t lo = first_block_ge(P.ix, dirt, nbt, firstt, lastt, tfbt, tfbaset, tfst, c);
-                                if (lo < nbt) {
-                                        const uint32_t lastv = __ldg(bl + lo);
-                                        if (lastv >= c) {
-                                                hit  = lastv == c;
-                                                need = !hit;
-                                                off  = __ldg(bo + lo);
-                                                prev = lo ? __ldg(bl + lo - 1u) : 0u;
-                                                nblk = (lo + 1u == nbt) ? (docst - 32u * (nbt - 1u)) : 32u;
-                                                if (need && c <= prev) // cannot happen (prev < c by construction); keeps a corrupt directory from looping
-                                                        need = false;
-                                        }
-                                }
-                        }
-                        if (__any_sync(0xffffffffu, need)) {
-                                gather_issue(P.ix.index, off, need, stage, lane);
-                                gather_wait<0>();
-                                if (need)
-                                        hit = google_block_find(P.ix.index, off, stage, lane, nblk, prev, c);
-                                __syncwarp();
-                        }
+                // round j's verdicts: a necessary term drops the candidates it does not hold, another one sets its membership bit
+                auto keep = [&](uint32_t j, bool valid, bool hit) {
                         if (t < nnec) {
                                 if (valid && !hit)
                                         cand[j * kCandStride + lane] = kCandInvalid;
@@ -252,6 +219,66 @@ template <bool FILT> __device__ void cand_exec_google(const ExecParams &P, const
                                 if (valid && hit)
                                         cmask[j * kCandStride + lane] |= uint8_t(1u << t);
                                 alive = 1u;
+                        }
+                };
+                if (denset != kDenseNone) {
+                        // a term with a resident bitmap: the probe is one word load and a bit test.  The words of kR rounds are
+                        // loaded before any of them is tested, so the group waits out one load latency per batch of rounds, not per round.
+                        // (Lanes j >= rounds hold n = 0: the rounds past the group's blocks have no valid candidate.)  The filtered
+                        // instantiation probes one round at a time: two rounds there add to the spills it already has.
+                        const uint32_t *bmt   = P.ix.dense + denset;
+                        const uint32_t  baset = (firstt >> kDenseAlignShift) << kDenseAlignShift;
+                        constexpr uint32_t kR = FILT ? 1u : kCandProbeRounds;
+                        for (uint32_t j0 = 0; j0 < rounds; j0 += kR) {
+                                uint32_t w[kR], meta = 0; // meta bits 6r .. 6r + 5: round r's candidate is valid (bit 5), its bit in w[r]
+#pragma unroll
+                                for (uint32_t r = 0; r < kR; ++r) {
+                                        const uint32_t nj = __shfl_sync(0xffffffffu, n, int(j0 + r));
+                                        const uint32_t c  = uint32_t(lane) < nj ? cand[(j0 + r) * kCandStride + lane] : kCandInvalid;
+                                        w[r]              = c != kCandInvalid && c >= firstt && c <= lastt ? __ldg(bmt + ((c - baset) >> 5)) : 0u;
+                                        meta |= ((c != kCandInvalid ? 32u : 0u) | (c & 31u)) << (6u * r);
+                                }
+#pragma unroll
+                                for (uint32_t r = 0; r < kR; ++r) {
+                                        const uint32_t m     = (meta >> (6u * r)) & 63u;
+                                        const bool     valid = m & 32u;
+                                        if (__any_sync(0xffffffffu, valid))
+                                                keep(j0 + r, valid, (w[r] >> (m & 31u)) & 1u);
+                                }
+                        }
+                } else {
+                        for (uint32_t j = 0; j < rounds; ++j) {
+                                const uint32_t nj = __shfl_sync(0xffffffffu, n, int(j));
+                                uint32_t       c  = uint32_t(lane) < nj ? cand[j * kCandStride + lane] : kCandInvalid;
+                                const bool     valid = c != kCandInvalid;
+                                if (!__any_sync(0xffffffffu, valid))
+                                        continue;
+                                bool     hit = false, need = false;
+                                uint32_t off = 0, prev = 0, nblk = 0;
+                                if (valid && nbt) {
+                                        // the one block that can hold c: first block whose last document is >= c
+                                        const uint32_t lo = first_block_ge(P.ix, dirt, nbt, firstt, lastt, tfbt, tfbaset, tfst, c);
+                                        if (lo < nbt) {
+                                                const uint32_t lastv = __ldg(bl + lo);
+                                                if (lastv >= c) {
+                                                        hit  = lastv == c;
+                                                        need = !hit;
+                                                        off  = __ldg(bo + lo);
+                                                        prev = lo ? __ldg(bl + lo - 1u) : 0u;
+                                                        nblk = (lo + 1u == nbt) ? (docst - 32u * (nbt - 1u)) : 32u;
+                                                        if (need && c <= prev) // cannot happen (prev < c by construction); keeps a corrupt directory from looping
+                                                                need = false;
+                                                }
+                                        }
+                                }
+                                if (__any_sync(0xffffffffu, need)) {
+                                        gather_issue(P.ix.index, off, need, stage, lane);
+                                        gather_wait<0>();
+                                        if (need)
+                                                hit = google_block_find(P.ix.index, off, stage, lane, nblk, prev, c);
+                                        __syncwarp();
+                                }
+                                keep(j, valid, hit);
                         }
                 }
                 __syncwarp();

@@ -972,7 +972,26 @@ PlanConfig trn::plan_config_from_env() {
                 pc.dense_runs = atoi(e) != 0;
         if (const char *e = getenv("TRN_MIXED_RUNS"))
                 pc.mixed_runs = atoi(e) != 0;
+        if (const char *e = getenv("TRN_CAND_RUNS"))
+                pc.cand_runs = atoi(e) != 0;
         return pc;
+}
+
+trn::GroupStarts trn::group_starts(const BlockDirectory &dir) {
+        GroupStarts g;
+        g.base.resize(dir.terms.size());
+        uint64_t n{0};
+        for (size_t t = 0; t < dir.terms.size(); ++t) {
+                g.base[t] = uint32_t(n);
+                n += (dir.terms[t].nblocks + 31u) / 32u;
+        }
+        g.first.resize(n);
+        for (size_t t = 0; t < dir.terms.size(); ++t) {
+                const TermDir &T = dir.terms[t];
+                for (uint32_t gr = 0; gr < (T.nblocks + 31u) / 32u; ++gr)
+                        g.first[g.base[t] + gr] = gr ? dir.blk_last[T.dir_begin + 32u * gr - 1u] + 1u : T.first_doc;
+        }
+        return g;
 }
 
 void trn::dense_span(const DevTerm &T, uint64_t &base, uint64_t &words) {
@@ -1050,7 +1069,7 @@ static int fail(std::string &err, int code, const std::string &m) {
 }
 
 int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
-                    uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip) {
+                    uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip, const GroupStarts *groups) {
         out                = BatchPlan{};
         const bool scored  = mode == TRN_MODE_SCORED_ALL || mode == TRN_MODE_SCORED_TOPK;
         if (mode == TRN_MODE_MATCHED_TERMS) { // the DocumentsOnly program, plus what the collect pass runs per match
@@ -1369,7 +1388,35 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
         };
         run_tickets(group, out.dense_runs);
         run_tickets(mixed, out.mixed_runs);
-        if (!group.empty() || !mixed.empty()) {
+        // Candidate-driven groups, same conditions: {query, group} tickets counting-sorted by the run of the group's first docID (queries
+        // ascending within a run, then groups ascending).  The warps in flight then hold neighbouring docID windows of every lead, so
+        // the bitmap words and directory entries their probes read are shared through L2 instead of each coming from HBM.
+        const bool candRuns = groups && cfg.cand_runs && google && !scored && !out.any_phrase && anyCandidate;
+        if (candRuns) {
+                constexpr uint32_t    kRuns = 1u << (32 - kDenseAlignShift);
+                std::vector<uint32_t> at(kRuns + 1, 0);
+                auto                  lead_groups = [&](const DevQuery &dq) { return groups->first.data() + groups->base[steps[dq.step_begin].term]; };
+                for (uint32_t q = 0; q < nq; ++q) {
+                        const auto &dq = out.queries[q];
+                        if (dq.route != TRN_ROUTE_CANDIDATE)
+                                continue;
+                        const uint32_t *gf = lead_groups(dq);
+                        for (uint32_t gr = 0; gr < dq.ntiles; ++gr)
+                                ++at[(gf[gr] >> kDenseAlignShift) + 1];
+                }
+                for (uint32_t i = 1; i <= kRuns; ++i)
+                        at[i] += at[i - 1];
+                out.cand_runs.resize(at[kRuns]);
+                for (uint32_t q = 0; q < nq; ++q) {
+                        const auto &dq = out.queries[q];
+                        if (dq.route != TRN_ROUTE_CANDIDATE)
+                                continue;
+                        const uint32_t *gf = lead_groups(dq);
+                        for (uint32_t gr = 0; gr < dq.ntiles; ++gr)
+                                out.cand_runs[at[gf[gr] >> kDenseAlignShift]++] = uint2{q, gr};
+                }
+        }
+        if (!group.empty() || !mixed.empty() || candRuns) {
                 // the step-program launch's own tickets without them (the items keep their item_base)
                 out.gen_items = 0;
                 for (uint32_t q = 0, g = 0, m = 0; q < nq; ++q) {
@@ -1382,6 +1429,16 @@ int trn::plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, co
                         else if (dq.route != TRN_ROUTE_FLAT_TREE)
                                 out.gen_items += dq.ntiles;
                 }
+        }
+        // the candidate groups' tickets run the groups' own step-program tickets (gen_base + group), which the launch then skips
+        if (candRuns) {
+                if (out.gen_items >= (1ull << 31)) { // (the kernel marks a run ticket in bit 31 of its ticket number)
+                        out.cand_runs.clear();
+                        return TRN_OK;
+                }
+                out.cand_order.resize(out.cand_runs.size());
+                for (size_t i = 0; i < out.cand_runs.size(); ++i)
+                        out.cand_order[i] = out.queries[out.cand_runs[i].x].gen_base + out.cand_runs[i].y;
         }
         return TRN_OK;
 }

@@ -29,6 +29,7 @@ struct PlanConfig {
         double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
         bool     dense_runs{true};    // TRN_DENSE_RUNS=0: all-bitmap flat ANDs take (query, tile) tickets like the other flat ANDs (BatchPlan::dense_runs)
         bool     mixed_runs{true};    // TRN_MIXED_RUNS=0: flat ANDs with one decoded operand take (query, tile) tickets (BatchPlan::mixed_runs)
+        bool     cand_runs{true};     // TRN_CAND_RUNS=0: candidate-driven groups take tickets in query order (BatchPlan::cand_runs)
         // kernel limits (kernels.h)
         uint32_t score_flat_max_leaves{0};          // leaves of a k_score_flat query
         uint32_t docs_stage_bytes{0};               // per-warp staging bytes of k_exec_docs
@@ -56,6 +57,13 @@ struct BatchPlan {
         // flat ANDs with exactly one operand without a resident bitmap (the lead, decoded; the others probed in their bitmaps), same
         // conditions: the same {query, first tile} tickets over the same runs, run-major, between dense_runs and gen_items
         std::vector<uint2>     mixed_runs;
+        // candidate-driven queries, same conditions: one ticket {query, group} per 32-block group of the lead, counting-sorted by the
+        // 2^kDenseAlignShift-docID run of the group's first docID (ties in query order), between mixed_runs and gen_items.  The queries
+        // that run in flight together then probe the same runs of the resident bitmaps.  A group keeps its item, item_base + group.
+        std::vector<uint2>     cand_runs;
+        // what the launch reads of them: per ticket the group's own step-program ticket, gen_base + group (the launch skips those
+        // tickets where the step-program tickets reach the candidate-driven queries)
+        std::vector<uint32_t>  cand_order;
         uint64_t               seg_cap{0};     // upper bound of the batch's matches (result segments)
         uint64_t               cand_total{0};  // top-k candidate entries
         uint64_t               postings{0}, bytes{0};
@@ -82,9 +90,19 @@ int plan_collect(const std::vector<DevTerm> &terms, const trn_query *queries, ui
 // BatchPlan::collect).  dense_off: per term, the first word of its resident bitmap (DenseSelection::off), or
 // null when the source has none.  Returns TRN_OK, or an error code with its message in err: TRN_ERR_ARG / TRN_ERR_UNSUPPORTED for a
 // plan the compiler refuses, TRN_ERR_CAPACITY when the batch has to be split.  clip (null: none): per query the inclusive docID span its
-// matches can lie in (its allow set's first and last docID; x > y: none), to which its tile range is clipped.
+// matches can lie in (its allow set's first and last docID; x > y: none), to which its tile range is clipped.  groups (null: candidate-driven
+// queries keep query-order tickets): the first docID of every lead group (group_starts), which orders BatchPlan::cand_runs.
+//
+// GroupStarts: the first docID of every 32-block group of every term (GOOGLE directories), where a candidate-driven work item starts.
+// Group g of term t is first[base[t] + g]: the last docID of block 32g - 1 plus one, the term's first docID for g = 0.  1/32 of the
+// directory's entries.
+struct GroupStarts {
+        std::vector<uint32_t> base; // per term: its first entry in `first`
+        std::vector<uint32_t> first;
+};
+GroupStarts group_starts(const BlockDirectory &dir);
 int plan_batch(const PlanConfig &cfg, const std::vector<DevTerm> &terms, const uint32_t *dense_off, const trn_query *queries, uint32_t nq, int mode,
-               uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip = nullptr);
+               uint32_t k, BatchPlan &out, std::string &err, const uint2 *clip = nullptr, const GroupStarts *groups = nullptr);
 
 // Resident docID bitmaps of dense terms (GOOGLE sources; LUCENE sources get none).  A selected term owns one bitmap over its own docID
 // span, both ends aligned to 2^kDenseAlignShift docIDs — the largest tile of any k_exec_docs launch — so every tile of every launch lies
