@@ -225,6 +225,11 @@ typedef struct trn_index_info {
          * counted in directory_bytes.  0 when TRN_DENSE_BITMAPS=0, for LUCENE sources, or when the upload could not allocate them
          * (trn_last_error then says so; the upload itself succeeds). */
         uint64_t dense_terms, dense_bitmap_bytes;
+        /* the probe bitmaps (GOOGLE; trn_debug_probe_terms): the second tier, which only the candidate-driven conjunction probes, for terms
+         * without a dense bitmap.  How many terms have one and their bytes in HBM, beside dense_bitmap_bytes.  0 when TRN_PROBE_BITMAPS=0,
+         * TRN_PROBE_BUDGET=0 or TRN_DENSE_BITMAPS=0, for LUCENE sources, or when the upload could not allocate them (trn_last_error then
+         * says so; the dense tier is kept if it fits alone). */
+        uint64_t probe_terms, probe_bitmap_bytes;
 } trn_index_info;
 int trn_index_info_get(trn_ctx *, trn_index_info *out);
 
@@ -354,6 +359,15 @@ int trn_debug_cand_runs(int codec, const uint8_t *index, uint64_t nbytes, const 
  * taken densest first while the bitmaps fit into the budget (default: 25 % of the index bytes).  offsets[0..nterms) receives every term's
  * first 32-bit word in the bitmap array (0xffffffff: none), *nselected the number of terms with a bitmap, *bitmap_bytes their bytes. */
 int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets, uint32_t *nselected,
+                          uint64_t *bitmap_bytes, char *err, size_t errcap);
+
+/* The same for the probe bitmaps (TRN_PROBE_BITMAPS, TRN_PROBE_RATIO, TRN_PROBE_BUDGET; TRN_DENSE_BITMAPS=0 turns them off too).  A GOOGLE
+ * term without a dense bitmap qualifies when its bitmap is at most TRN_PROBE_RATIO (default 16) times its chunk; qualifying terms are taken
+ * densest first (ties: lower term id) while the tier fits into TRN_PROBE_BUDGET x the index bytes (default 2.0) and both tiers together
+ * into fewer than 2^32 words.  The tier is laid out behind the dense bitmaps.  offsets[0..nterms) receives the word the candidate-driven
+ * conjunction probes each term at: a dense term's dense offset, a probe term's first word, 0xffffffff for a term with neither;
+ * *nselected the number of probe terms, *bitmap_bytes their bytes. */
+int trn_debug_probe_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets, uint32_t *nselected,
                           uint64_t *bitmap_bytes, char *err, size_t errcap);
 
 /* Debug view (tests, tooling): the resident bitmap of `term` as the upload built it.  *nwords = its 32-bit words (0: the term has none),

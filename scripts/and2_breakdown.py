@@ -1,13 +1,15 @@
-"""Time the and2 batch of bench.py by route class, on sources created with different ticket orders, alternating: the default (every run-major
-ticket space on), TRN_CAND_RUNS=0 (candidate-driven groups in query order), and on request TRN_MIXED_RUNS=0 (the flat ANDs with one
+"""Time the and2 batch of bench.py by route class, on sources created with different settings, alternating: the default (every run-major
+ticket space on, both tiers of resident bitmaps), TRN_PROBE_BITMAPS=0 (no probe bitmaps: the candidate-driven conjunction probes every
+term without a dense bitmap through its block directory), TRN_CAND_RUNS=0 (candidate-driven groups in query order), and on request TRN_MIXED_RUNS=0 (the flat ANDs with one
 bitmap operand on per-tile tickets) and TRN_DENSE_RUNS=0 TRN_MIXED_RUNS=0 (every flat AND on per-tile tickets).
 
 Builds bench.py's GOOGLE index and and2 batch, splits the batch into
   both        flat AND, both operands with a resident bitmap
   one         flat AND, one operand with a bitmap
   none        flat AND, no bitmap
-  cand_bitmap candidate-driven, every probed operand with a bitmap
-  cand_dir    candidate-driven, at least one operand probed through its block directory
+  cand_bitmap candidate-driven, every probed operand with a dense bitmap
+  cand_probe  candidate-driven, every probed operand with a bitmap of either tier, at least one of them a probe bitmap
+  cand_dir    candidate-driven, at least one operand probed through its block directory with both tiers on
 and times each class as its own device-resident batch (exec_batch_device, as bench.py; CUDA events over --steps steps after --warmup).
 Per class it prints ms per step, (query, tile) work items (candidate-driven: lead-term groups), matches, result words, and a model of
 the HBM traffic of bitmap reads:
@@ -16,9 +18,9 @@ the HBM traffic of bitmap reads:
     sectors they read — in query order (the 16 bitmaps are several times L2, so each query's probes read their own sectors: the
     expected distinct sectors of its lead documents in each bitmap) and in run-major order (the queries in flight share a docID window,
     so each bitmap sector is read once per batch: the expected distinct sectors of all the class's probes of that bitmap).
-Directory probes (cand_dir) are counted, not modelled.  Needs a GPU; prints the card and its power limit.
+Probes of the probe tier and of the directory are counted, not modelled.  Needs a GPU; prints the card and its power limit.
 
-    python scripts/and2_breakdown.py [--ndocs 100000000] [--steps 20] [--warmup 5] [--settings runs,cand_query_order]
+    python scripts/and2_breakdown.py [--ndocs 100000000] [--steps 20] [--warmup 5] [--settings runs,probe_off,cand_query_order]
 """
 import argparse
 import json
@@ -35,7 +37,7 @@ import bench  # noqa: E402
 import trinity_b200 as tb  # noqa: E402
 
 
-SETTINGS = {"runs": {}, "cand_query_order": {"TRN_CAND_RUNS": "0"}, "mixed_tiles": {"TRN_MIXED_RUNS": "0"},
+SETTINGS = {"runs": {}, "probe_off": {"TRN_PROBE_BITMAPS": "0"}, "cand_query_order": {"TRN_CAND_RUNS": "0"}, "mixed_tiles": {"TRN_MIXED_RUNS": "0"},
             "tiles": {"TRN_DENSE_RUNS": "0", "TRN_MIXED_RUNS": "0"}}
 
 
@@ -63,7 +65,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3, help="alternations of the sources per class")
-    ap.add_argument("--settings", default="runs,cand_query_order", help=f"comma-separated sources to time, of {list(SETTINGS)}")
+    ap.add_argument("--settings", default="runs,probe_off,cand_query_order", help=f"comma-separated sources to time, of {list(SETTINGS)}")
     args = ap.parse_args()
     settings = {k: SETTINGS[k] for k in args.settings.split(",")}
     import torch
@@ -76,6 +78,10 @@ def main():
     tdict = tb.TermDictionary(synth.names)
     plans = [tb.parse_query(q, tdict) for q in texts]
     terms = np.asarray(synth.terms)
+    # the probe tier of the default settings, selected on the host as the upload does (the probed offset of a dense term is its dense one)
+    env = {k: os.environ.pop(k) for k in ("TRN_PROBE_BITMAPS", "TRN_PROBE_RATIO", "TRN_PROBE_BUDGET", "TRN_DENSE_BITMAPS", "TRN_DENSE_BUDGET") if k in os.environ}
+    probe_off, _, _ = tb.debug_probe_terms(tb.CODEC_GOOGLE, np.asarray(synth.index), terms)
+    os.environ.update(env)
     g.exec_batch(plans, tb.MODE_DOCS_COMPACT, copy=False)
     routes = g.last_routes()
     dense = {}  # term -> bitmap bytes
@@ -88,7 +94,8 @@ def main():
 
     tile = 1 << 14
     tiles = (args.ndocs >> 14) + 1  # the synthetic terms spread over the whole docID range
-    classes = {"both": [], "one": [], "none": [], "cand_bitmap": [], "cand_dir": []}
+    classes = {"both": [], "one": [], "none": [], "cand_bitmap": [], "cand_probe": [], "cand_dir": []}
+    in_probe_tier = lambda t: probe_off[t] != tb.DENSE_NONE and not bitmap_bytes(t)
     docs = lambda t: int(terms["documents"][t])
     for i, p in enumerate(plans):
         ts = [int(x["term"]) for x in p if x["kind"] == tb.NODE_TERM]
@@ -98,11 +105,13 @@ def main():
             # plan_batch breaks a tie in block counts by an unstable sort, so on a tie its lead may be the other term
             lead = min(ts, key=lambda t: (-(-docs(t) // 32), ts.index(t)))
             probed = [t for t in ts if t != lead]
-            classes["cand_bitmap" if all(bitmap_bytes(t) for t in probed) else "cand_dir"].append(i)
+            cls = "cand_bitmap" if all(bitmap_bytes(t) for t in probed) else "cand_probe" if all(bitmap_bytes(t) or in_probe_tier(t) for t in probed) else "cand_dir"
+            classes[cls].append(i)
         elif routes[i] == tb.ROUTE_FLAT_AND:
             classes["both" if nd == len(ts) else "one" if nd else "none"].append(i)
     print(json.dumps({"card": card, "ndocs": args.ndocs, "nq": args.nq, "dense_terms": g.info()["dense_terms"],
-                      "dense_bitmap_bytes": g.info()["dense_bitmap_bytes"]}))
+                      "dense_bitmap_bytes": g.info()["dense_bitmap_bytes"],
+                      **{f"probe_{f}_{k}": s.info()[f"probe_{f}"] for k, s in srcs.items() for f in ("terms", "bitmap_bytes")}}))
     stream = torch.cuda.current_stream()
     for name, qs in classes.items():
         if not qs:
@@ -110,7 +119,7 @@ def main():
         sub = [plans[i] for i in qs]
         items = old_b = 0
         used = set()
-        probes = dir_probes = 0
+        probes = dir_probes = tier_probes = 0
         sec_query = 0.0
         per_bitmap = {}  # bitmap term -> probes of the class against it
         for i in qs:
@@ -126,6 +135,8 @@ def main():
                     if bitmap_bytes(t):
                         sec_query += distinct_sectors(docs(lead), bitmap_bytes(t) // 32)
                         per_bitmap[t] = per_bitmap.get(t, 0) + docs(lead)
+                    elif in_probe_tier(t):
+                        tier_probes += docs(lead)
                     else:
                         dir_probes += docs(lead)
             else:
@@ -154,7 +165,7 @@ def main():
                **{f"ms_median_{k}": round(float(np.median(v)), 3) for k, v in ms.items()}}
         if name.startswith("cand"):
             sec_run = sum(distinct_sectors(n, bitmap_bytes(t) // 32) for t, n in per_bitmap.items())
-            row.update({"probes_upper_bound": probes, "directory_probes_upper_bound": dir_probes, "bitmap_sectors_query_order": round(sec_query),
+            row.update({"probes_upper_bound": probes, "probe_tier_probes_upper_bound": tier_probes, "directory_probes_upper_bound": dir_probes, "bitmap_sectors_query_order": round(sec_query),
                         "bitmap_sectors_run_major": round(sec_run), "bitmap_bytes_query_order": round(sec_query) * 32,
                         "bitmap_bytes_run_major": round(sec_run) * 32})
         else:

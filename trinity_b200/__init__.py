@@ -349,17 +349,28 @@ def _debug_run_tickets(fn, codec, index, terms, queries, mode, k, max_docid):
 def debug_dense_terms(codec: int, index: np.ndarray, terms: np.ndarray):
     """(offsets, bitmap_bytes): the first 32-bit word of every term's resident docID bitmap (DENSE_NONE: none) and the bytes of all of them,
     selected on the host as a GpuIndexSource created with this environment would on upload (no GPU needed)"""
+    off, n, nbytes = _debug_bitmap_terms(lib().trn_debug_dense_terms, codec, index, terms)
+    assert int(np.count_nonzero(off != DENSE_NONE)) == n
+    return off, nbytes
+
+
+def debug_probe_terms(codec: int, index: np.ndarray, terms: np.ndarray):
+    """(offsets, nselected, bitmap_bytes) of the probe bitmaps, the second tier that candidate-driven conjunctions probe: per term the word
+    its probes read from (its dense bitmap's, its probe bitmap's, DENSE_NONE: neither), the number of probe-tier terms and their bytes,
+    selected on the host as a GpuIndexSource created with this environment would on upload (no GPU needed)"""
+    return _debug_bitmap_terms(lib().trn_debug_probe_terms, codec, index, terms)
+
+
+def _debug_bitmap_terms(fn, codec, index, terms):
     index = np.ascontiguousarray(index, dtype=np.uint8)
     terms = np.ascontiguousarray(terms, dtype=TERM_DTYPE)
     off = np.zeros(max(len(terms), 1), np.uint32)
     n, nbytes = C.c_uint32(), C.c_uint64()
     err = C.create_string_buffer(256)
-    rc = lib().trn_debug_dense_terms(codec, _ptr(index), index.size, _ptr(terms), len(terms), _ptr(off), C.byref(n), C.byref(nbytes), err, 256)
+    rc = fn(codec, _ptr(index), index.size, _ptr(terms), len(terms), _ptr(off), C.byref(n), C.byref(nbytes), err, 256)
     if rc != 0:
         raise TrinityError(err.value.decode("utf-8", "replace") or f"rc={rc}")
-    off = off[: len(terms)].copy()
-    assert int(np.count_nonzero(off != DENSE_NONE)) == n.value
-    return off, int(nbytes.value)
+    return off[: len(terms)].copy(), n.value, int(nbytes.value)
 
 
 def bm25_idf(doc_freq: int, docs_cnt: int) -> float:

@@ -22,7 +22,7 @@ EXPORTS = [
     "trn_exec_batch", "trn_exec_batch_device", "trn_last_topk_device", "trn_merge_topk", "trn_fetch_results", "trn_last_timings",
     "trn_decode_terms", "trn_result_for_each", "trn_result_decode", "trn_upload_hits", "trn_debug_positions", "trn_encode_google", "trn_encode_lucene", "trn_debug_chunk_plan",
     "trn_encode_google_payloads", "trn_encode_lucene_payloads", "trn_index_documents_payloads",
-    "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_cand_runs", "trn_debug_dense_terms", "trn_debug_dense_bitmap",
+    "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_cand_runs", "trn_debug_dense_terms", "trn_debug_probe_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
     "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
     "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_merge_sources_payloads", "trn_debug_merge_plan",
@@ -46,7 +46,8 @@ class TrnQuery(C.Structure):
 class TrnIndexInfo(C.Structure):
     _fields_ = [("codec", C.c_int), ("nterms", C.c_uint32), ("max_docid", C.c_uint32), ("tile_docs", C.c_uint32),
                 ("ntiles", C.c_uint32), ("block_docs", C.c_uint32), ("index_bytes", C.c_uint64), ("directory_bytes", C.c_uint64),
-                ("total_blocks", C.c_uint64), ("total_postings", C.c_uint64), ("dense_terms", C.c_uint64), ("dense_bitmap_bytes", C.c_uint64)]
+                ("total_blocks", C.c_uint64), ("total_postings", C.c_uint64), ("dense_terms", C.c_uint64), ("dense_bitmap_bytes", C.c_uint64),
+                ("probe_terms", C.c_uint64), ("probe_bitmap_bytes", C.c_uint64)]
 
 
 class TrnResult(C.Structure):
@@ -215,6 +216,7 @@ def lib() -> C.CDLL:
     sig("trn_debug_cand_runs", i32, i32, vp, u64, vp, u32, u32, vp, u32, i32, u32, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
     sig("trn_debug_dense_bitmap", i32, vp, u32, vp, u64, P(u64), P(u64))
     sig("trn_debug_dense_terms", i32, i32, vp, u64, vp, u32, vp, P(u32), P(u64), C.c_char_p, C.c_size_t)
+    sig("trn_debug_probe_terms", i32, i32, vp, u64, vp, u32, vp, P(u32), P(u64), C.c_char_p, C.c_size_t)
     sig("trn_intersect", i32, vp, vp, u32, P(TrnIntersections))
     sig("trn_debug_intersect_plan", i32, vp, vp, u32, u32, vp, vp, vp, vp, u64, P(u32), P(u64), vp, P(u32), C.c_char_p, C.c_size_t)
     sig("trn_percolator_register", i32, vp, vp, u32, u32, vp, P(TrnPercolatorInfo))

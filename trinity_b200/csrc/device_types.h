@@ -55,9 +55,13 @@ struct DevIndex {
         const uint32_t *hblk_off; // per term: byte offsets of its 128-hit blocks in hits.data, then of its varbyte tail, then the end
         const struct HitTerm *hit_term; // per term: {first entry in hblk_off, sumHits} (hitcursor.h)
         // resident docID bitmaps of dense GOOGLE terms (planner.h select_dense_terms; null when the source has none): term t's bitmap starts
-        // at word dense_off[t] of `dense` (kDenseNone: no bitmap) and covers docIDs from first_doc rounded down to 2^kDenseAlignShift
+        // at word dense_off[t] of `dense` (kDenseNone: no bitmap) and covers docIDs from first_doc rounded down to 2^kDenseAlignShift.
+        // probe_off (null, like `dense`, when the source has neither tier): the same for the probe bitmaps (select_probe_terms), laid out
+        // behind the dense ones; it holds dense_off[t] for a term with a dense bitmap.  Only the candidate-driven conjunction probes through
+        // it, and k_build_dense builds both tiers through it.
         const uint32_t *dense;
         const uint32_t *dense_off;
+        const uint32_t *probe_off;
 };
 
 // ---- per-query step program (built on the host from the trn_qnode tree) ----

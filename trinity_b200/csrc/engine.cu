@@ -114,6 +114,9 @@ struct trn_ctx {
         uint32_t             dense_terms{0};       // terms with a bitmap (0: none, d_dense unused)
         uint64_t             dense_bytes{0};
         std::vector<uint32_t> h_dense_off;          // host copy of d_dense_off (trn_debug_dense_bitmap)
+        DevBuf               d_probe_off;          // per term its first word in d_dense for the candidate-driven probes (select_probe_terms)
+        uint32_t             probe_terms{0};       // terms of the probe tier, laid out in d_dense behind the dense bitmaps
+        uint64_t             probe_bytes{0};
         std::vector<DevTerm> h_terms;
         GroupStarts          h_groups; // GOOGLE: the first docID of every 32-block group of every term (orders BatchPlan::cand_runs)
         // batch scratch (grow-only)
@@ -336,7 +339,7 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_cand_order, &c->d_small[0], &c->d_small[1], &c->d_item_off,
+        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_probe_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_cand_order, &c->d_small[0], &c->d_small[1], &c->d_item_off,
                           &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
                           &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
                           &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores, &c->d_filters})
@@ -376,64 +379,106 @@ extern "C" int trn_set_stream(trn_ctx *c, void *s) {
 }
 
 // =================================================================================================== upload
-// The resident docID bitmaps of the dense terms of the index just copied (select_dense_terms), built on the device from the doc-delta
-// sections: exact copies of the terms' docID sets, like the block directory.  Not being able to allocate them does not fail the upload:
-// the source then runs without them, and trn_last_error says why.
+// The resident docID bitmaps of the index just copied, both tiers (select_dense_terms, select_probe_terms) in one array, built on the
+// device from the doc-delta sections: exact copies of the terms' docID sets, like the block directory.  Not being able to allocate them
+// does not fail the upload: the probe tier goes first and the dense tier keeps its bitmaps if they alone fit; without either the source
+// runs without bitmaps.  trn_last_error says why.
 static int upload_dense(trn_ctx *c) {
         c->dense_terms = 0;
         c->dense_bytes = 0;
+        c->probe_terms = 0;
+        c->probe_bytes = 0;
         c->h_dense_off.clear();
-        DenseSelection                  s;
-        std::vector<unsigned long long> prefix;
+        DenseSelection s, p; // p.off: what d_probe_off holds
         try {
                 s = select_dense_terms(c->pc, c->h_terms, c->index_bytes);
-                prefix.assign(s.order.size() + 1, 0ull);
-                for (size_t i = 0; i < s.order.size(); ++i)
-                        prefix[i + 1] = prefix[i] + c->h_terms[s.order[i]].nblocks;
+                p = select_probe_terms(c->pc, c->h_terms, c->index_bytes, s);
         } catch (const std::bad_alloc &) {
-                s = DenseSelection{};
+                s = p = DenseSelection{};
                 c->err = "dense-term bitmaps off for this index: out of host memory";
         }
-        DevBuf sel, pre;
+        // k_build_dense reads blocks of the format's 32 documents; an index built with another block size (decode sweep) gets no
+        // bitmaps, and the exec entry points refuse it
+        if (c->block_docs != Codecs::Google::N)
+                s = p = DenseSelection{};
+        DevBuf      sel, pre;
         cudaError_t e = cudaSuccess;
-        if (!s.order.empty()) {
-                e = c->d_dense.ensure(s.words * 4);
+        auto        allocate = [&] {
+                const size_t nsel = s.order.size() + p.order.size();
+                e                 = c->d_dense.ensure((s.words + p.words) * 4);
                 if (e == cudaSuccess)
                         e = c->d_dense_off.ensure(std::max<size_t>(4, s.off.size() * 4));
                 if (e == cudaSuccess)
-                        e = sel.ensure(s.order.size() * 4);
+                        e = c->d_probe_off.ensure(std::max<size_t>(4, p.off.size() * 4));
                 if (e == cudaSuccess)
-                        e = pre.ensure(prefix.size() * 8);
-        }
-        if (s.order.empty() || e != cudaSuccess) {
+                        e = sel.ensure(nsel * 4);
+                if (e == cudaSuccess)
+                        e = pre.ensure((nsel + 1) * 8);
                 if (e != cudaSuccess) {
                         (void)cudaGetLastError(); // an allocation failure is not sticky: clear it
-                        c->err = std::string("dense-term bitmaps off for this index: ") + cudaGetErrorString(e);
+                        for (DevBuf *b : {&c->d_dense, &c->d_dense_off, &c->d_probe_off, &sel, &pre})
+                                b->release();
                 }
+        };
+        if (!p.order.empty()) {
+                allocate();
+                if (e != cudaSuccess) {
+                        c->err          = std::string("probe bitmaps off for this index: ") + cudaGetErrorString(e);
+                        p.order.clear();
+                        p.words         = 0;
+                        p.off           = s.off;
+                        e               = cudaSuccess;
+                }
+        }
+        if (p.order.empty() && !s.order.empty()) {
+                allocate();
+                if (e != cudaSuccess)
+                        c->err = std::string("dense-term bitmaps off for this index: ") + cudaGetErrorString(e);
+        }
+        std::vector<uint32_t>           order;
+        std::vector<unsigned long long> prefix;
+        if (e == cudaSuccess) {
+                try {
+                        order = s.order;
+                        order.insert(order.end(), p.order.begin(), p.order.end());
+                        prefix.assign(order.size() + 1, 0ull);
+                        for (size_t i = 0; i < order.size(); ++i)
+                                prefix[i + 1] = prefix[i] + c->h_terms[order[i]].nblocks;
+                } catch (const std::bad_alloc &) {
+                        order.clear();
+                        c->err = "dense-term bitmaps off for this index: out of host memory";
+                }
+        }
+        if (order.empty()) {
                 c->d_dense.release();
                 c->d_dense_off.release();
+                c->d_probe_off.release();
                 sel.release();
                 pre.release();
                 return TRN_OK;
         }
-        CK(cudaMemsetAsync(c->d_dense.p, 0, s.words * 4, c->stream));
+        CK(cudaMemsetAsync(c->d_dense.p, 0, (s.words + p.words) * 4, c->stream));
         CK(cudaMemcpyAsync(c->d_dense_off.p, s.off.data(), s.off.size() * 4, cudaMemcpyHostToDevice, c->stream));
-        CK(cudaMemcpyAsync(sel.p, s.order.data(), s.order.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(c->d_probe_off.p, p.off.data(), p.off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(sel.p, order.data(), order.size() * 4, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(pre.p, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, c->stream));
         c->dense_terms = uint32_t(s.order.size()); // dev_index hands the bitmaps out from here on
+        c->probe_terms = uint32_t(p.order.size());
         // the launch check reads the thread's last error: drop one a failed call elsewhere left behind (e.g. trn_destroy's cudaSetDevice
         // of a context created for a device that does not exist)
         (void)cudaGetLastError();
-        const cudaError_t le = launch_build_dense(dev_index(c), sel.as<uint32_t>(), pre.as<unsigned long long>(), uint32_t(s.order.size()), prefix.back(),
+        const cudaError_t le = launch_build_dense(dev_index(c), sel.as<uint32_t>(), pre.as<unsigned long long>(), uint32_t(order.size()), prefix.back(),
                                                   c->d_dense.as<uint32_t>(), c->stream);
         const cudaError_t se = cudaStreamSynchronize(c->stream);
         sel.release();
         pre.release();
         if (le != cudaSuccess || se != cudaSuccess) {
                 c->dense_terms = 0;
+                c->probe_terms = 0;
                 return fail(c, TRN_ERR_CUDA, std::string("building the dense-term bitmaps: ") + cudaGetErrorString(le != cudaSuccess ? le : se));
         }
         c->dense_bytes = s.words * 4;
+        c->probe_bytes = p.words * 4;
         c->h_dense_off = std::move(s.off);
         return TRN_OK;
 }
@@ -740,6 +785,8 @@ extern "C" int trn_index_info_get(trn_ctx *c, trn_index_info *o) {
         o->total_postings  = c->total_postings;
         o->dense_terms        = c->dense_terms;
         o->dense_bitmap_bytes = c->dense_bytes;
+        o->probe_terms        = c->probe_terms;
+        o->probe_bitmap_bytes = c->probe_bytes;
         return TRN_OK;
 }
 
@@ -761,8 +808,10 @@ static DevIndex dev_index(trn_ctx *c) {
         ix.hit_base   = c->have_hits ? c->d_hit_base.as<uint32_t>() : nullptr;
         ix.hblk_off   = c->have_hits ? c->d_hblk_off.as<uint32_t>() : nullptr;
         ix.hit_term   = c->have_hits ? c->d_hit_term.as<HitTerm>() : nullptr;
-        ix.dense      = c->dense_terms ? c->d_dense.as<uint32_t>() : nullptr;
+        const bool bitmaps = c->dense_terms || c->probe_terms;
+        ix.dense      = bitmaps ? c->d_dense.as<uint32_t>() : nullptr;
         ix.dense_off  = c->dense_terms ? c->d_dense_off.as<uint32_t>() : nullptr;
+        ix.probe_off  = bitmaps ? c->d_probe_off.as<uint32_t>() : nullptr;
         return ix;
 }
 
@@ -1695,8 +1744,9 @@ extern "C" int trn_debug_cand_runs(int codec, const uint8_t *index, uint64_t nby
         return debug_run_tickets(RunTickets::cand, codec, index, nbytes, terms, nterms, max_docid, queries, nq, mode, k, qtiles, tickets, cap, n, err, errcap);
 }
 
-extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,
-                                     uint32_t *nselected, uint64_t *bitmap_bytes, char *err, size_t errcap) {
+// trn_debug_dense_terms / trn_debug_probe_terms: the selection of one tier of resident bitmaps
+static int debug_bitmap_terms(bool probe, int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,
+                              uint32_t *nselected, uint64_t *bitmap_bytes, char *err, size_t errcap) {
         auto seterr = [&](const std::string &m, int rc) {
                 if (err && errcap) {
                         std::strncpy(err, m.c_str(), errcap - 1);
@@ -1712,7 +1762,10 @@ extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t n
                 build_directory(codec, index, nbytes, terms, nterms, 1, dir);
                 PlanConfig pc = initial_plan_config();
                 pc.codec      = codec;
-                s             = select_dense_terms(pc, dev_terms(dir, terms, nterms), nbytes);
+                const std::vector<DevTerm> ht = dev_terms(dir, terms, nterms);
+                s                             = select_dense_terms(pc, ht, nbytes);
+                if (probe)
+                        s = select_probe_terms(pc, ht, nbytes, s);
         } catch (const std::exception &e) {
                 return seterr(e.what(), TRN_ERR_FORMAT);
         }
@@ -1721,6 +1774,16 @@ extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t n
         *nselected    = uint32_t(s.order.size());
         *bitmap_bytes = s.words * 4;
         return TRN_OK;
+}
+
+extern "C" int trn_debug_dense_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,
+                                     uint32_t *nselected, uint64_t *bitmap_bytes, char *err, size_t errcap) {
+        return debug_bitmap_terms(false, codec, index, nbytes, terms, nterms, offsets, nselected, bitmap_bytes, err, errcap);
+}
+
+extern "C" int trn_debug_probe_terms(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, uint32_t *offsets,
+                                     uint32_t *nselected, uint64_t *bitmap_bytes, char *err, size_t errcap) {
+        return debug_bitmap_terms(true, codec, index, nbytes, terms, nterms, offsets, nselected, bitmap_bytes, err, errcap);
 }
 
 extern "C" int trn_debug_dense_bitmap(trn_ctx *c, uint32_t term, uint32_t *out, uint64_t cap, uint64_t *base, uint64_t *nwords) {

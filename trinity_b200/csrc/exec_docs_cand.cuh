@@ -148,8 +148,8 @@ template <bool FILT> __device__ void cand_exec_google(const ExecParams &P, const
         uint32_t mydir = 0, mynb = 0, mydocs = 0, myfirst = 0, mylast = 0, mytfb = 0, mytfbase = 0, mytfs = 32, mydense = kDenseNone;
         if (uint32_t(lane) < nleaf && myTerm != kEmptyTerm) {
                 const DevTerm T = P.ix.terms[myTerm];
-                if (P.ix.dense_off)
-                        mydense = __ldg(P.ix.dense_off + myTerm);
+                if (P.ix.probe_off)
+                        mydense = __ldg(P.ix.probe_off + myTerm);
                 mydir           = T.dir_begin;
                 mynb            = T.nblocks;
                 mydocs          = T.documents;

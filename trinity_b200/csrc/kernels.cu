@@ -1042,7 +1042,7 @@ cudaError_t launch_topk_merge(const uint32_t *docids, const float *scores, uint3
         return cudaGetLastError();
 }
 
-// Load time: the bitmaps of the dense terms (DevIndex::dense, zeroed by the caller).  One thread per block of a selected term: it walks the
+// Load time: the bitmaps of the dense and the probe tier (DevIndex::dense at probe_off, zeroed by the caller).  One thread per block of a selected term: it walks the
 // block's doc-delta section (the deltas of documents 2..n, the block's last docID comes from the directory) and ORs one word per 32
 // docIDs it touched.  blk_prefix[s] = blocks of the selected terms before sel[s] (nsel + 1 entries).
 __global__ void __launch_bounds__(kThreads) k_build_dense(DevIndex ix, const uint32_t *sel, const unsigned long long *blk_prefix, uint32_t nsel,
@@ -1060,7 +1060,7 @@ __global__ void __launch_bounds__(kThreads) k_build_dense(DevIndex ix, const uin
         const DevTerm   T = ix.terms[t];
         const uint32_t *bl = ix.blk_last + T.dir_begin;
         const uint32_t  base = (T.first_doc >> kDenseAlignShift) << kDenseAlignShift;
-        uint32_t *      bm   = dense + ix.dense_off[t];
+        uint32_t *      bm   = dense + ix.probe_off[t];
         const uint32_t  n    = (b + 1u == T.nblocks) ? (T.documents - 32u * (T.nblocks - 1u)) : 32u;
         const uint8_t * p    = ix.index + ix.blk_off[T.dir_begin + b];
         uint32_t        doc = b ? bl[b - 1] : 0u, cw = 0xffffffffu, cur = 0;

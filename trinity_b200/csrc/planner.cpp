@@ -968,6 +968,18 @@ PlanConfig trn::plan_config_from_env() {
                 if (v >= 0.0 && v <= 1.0)
                         pc.dense_budget = v;
         }
+        if (const char *e = getenv("TRN_PROBE_BITMAPS"))
+                pc.probe_bitmaps = atoi(e) != 0;
+        if (const char *e = getenv("TRN_PROBE_RATIO")) {
+                const double v = atof(e);
+                if (v > 0.0)
+                        pc.probe_ratio = v;
+        }
+        if (const char *e = getenv("TRN_PROBE_BUDGET")) {
+                const double v = atof(e);
+                if (v >= 0.0)
+                        pc.probe_budget = v;
+        }
         if (const char *e = getenv("TRN_DENSE_RUNS"))
                 pc.dense_runs = atoi(e) != 0;
         if (const char *e = getenv("TRN_MIXED_RUNS"))
@@ -1020,6 +1032,32 @@ trn::DenseSelection trn::select_dense_terms(const PlanConfig &cfg, const std::ve
                 if (double((s.words + words) * 4) > budget)
                         break;
                 s.off[t] = uint32_t(s.words);
+                s.order.push_back(t);
+                s.words += words;
+        }
+        return s;
+}
+
+trn::DenseSelection trn::select_probe_terms(const PlanConfig &cfg, const std::vector<DevTerm> &terms, uint64_t index_bytes, const DenseSelection &dense) {
+        DenseSelection s;
+        s.off = dense.off;
+        if (cfg.codec != TRN_CODEC_GOOGLE || !cfg.dense_bitmaps || !cfg.probe_bitmaps)
+                return s;
+        std::vector<uint32_t> cand;
+        for (uint32_t t = 0; t < terms.size(); ++t) {
+                uint64_t base, words;
+                dense_span(terms[t], base, words);
+                if (terms[t].nblocks && dense.off[t] == kDenseNone && double(words * 4) <= cfg.probe_ratio * double(terms[t].chunk_len))
+                        cand.push_back(t);
+        }
+        std::stable_sort(cand.begin(), cand.end(), [&](uint32_t a, uint32_t b) { return terms[a].documents > terms[b].documents; });
+        const double budget = cfg.probe_budget * double(index_bytes);
+        for (uint32_t t : cand) {
+                uint64_t base, words;
+                dense_span(terms[t], base, words);
+                if (double((s.words + words) * 4) > budget || dense.words + s.words + words >= (1ull << 32))
+                        break;
+                s.off[t] = uint32_t(dense.words + s.words);
                 s.order.push_back(t);
                 s.words += words;
         }

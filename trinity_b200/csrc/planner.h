@@ -27,6 +27,9 @@ struct PlanConfig {
         bool     allow_phrase{false}; // the kernels execute OP_PHRASE (GOOGLE: inline hits; LUCENE: once hits.data is uploaded)
         bool     dense_bitmaps{true}; // TRN_DENSE_BITMAPS=0: no resident docID bitmaps of dense terms (select_dense_terms)
         double   dense_budget{0.25};  // TRN_DENSE_BUDGET: the bitmaps of one source take at most this share of its index bytes (0 .. 1)
+        bool     probe_bitmaps{true}; // TRN_PROBE_BITMAPS=0: no probe bitmaps (select_probe_terms); TRN_DENSE_BITMAPS=0 turns them off too
+        double   probe_ratio{16.0};   // TRN_PROBE_RATIO: a probe bitmap is at most this many times its term's chunk
+        double   probe_budget{2.0};   // TRN_PROBE_BUDGET: the probe bitmaps of one source take at most this multiple of its index bytes (0: none)
         bool     dense_runs{true};    // TRN_DENSE_RUNS=0: all-bitmap flat ANDs take (query, tile) tickets like the other flat ANDs (BatchPlan::dense_runs)
         bool     mixed_runs{true};    // TRN_MIXED_RUNS=0: flat ANDs with one decoded operand take (query, tile) tickets (BatchPlan::mixed_runs)
         bool     cand_runs{true};     // TRN_CAND_RUNS=0: candidate-driven groups take tickets in query order (BatchPlan::cand_runs)
@@ -117,6 +120,14 @@ void dense_span(const DevTerm &T, uint64_t &base, uint64_t &words);
 // A term qualifies when its bitmap is no larger than its chunk (chunk_len); qualifying terms are taken densest first (ties: lower term
 // id) while their bitmaps fit into cfg.dense_budget x index_bytes.  Reads the term records and the config only.
 DenseSelection select_dense_terms(const PlanConfig &cfg, const std::vector<DevTerm> &terms, uint64_t index_bytes);
+
+// The second tier, the probe bitmaps, which only the candidate-driven conjunction reads: a probe there tests one word, so a bitmap pays
+// off far below the density at which the flat paths, which read whole bitmaps, gain from one.  A GOOGLE term without a dense bitmap
+// qualifies when its bitmap is at most cfg.probe_ratio x its chunk; qualifying terms are taken densest first (ties: lower term id) while
+// the tier fits into cfg.probe_budget x index_bytes and both tiers together into fewer than 2^32 words (the offsets are 32-bit word
+// indices).  The tier is laid out behind the dense bitmaps.  off: per term, its dense.off entry when it has a dense bitmap, its first
+// word in the bitmap array when it has a probe bitmap, kDenseNone otherwise; order and words: the probe tier alone.
+DenseSelection select_probe_terms(const PlanConfig &cfg, const std::vector<DevTerm> &terms, uint64_t index_bytes, const DenseSelection &dense);
 
 // the block directory of an index (throws what build_block_directory throws)
 void build_directory(int codec, const uint8_t *index, uint64_t nbytes, const trn_term *terms, uint32_t nterms, int threads, BlockDirectory &dir);
