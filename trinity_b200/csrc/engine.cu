@@ -27,30 +27,67 @@
 #include <string>
 #include <unordered_map>
 #include <thread>
+#include <utility>
 #include <vector>
 
 using namespace trn;
 
 namespace {
-struct DevBuf {
+// Device memory (DevBuf) or pinned host memory (PinBuf) that frees itself when it goes out of scope.  It moves but does not copy, so
+// every allocation has exactly one owner.  release() frees early, where a caller lowers its peak memory.
+template <bool Pinned> struct Buf {
         void * p{nullptr};
         size_t cap{0};
+        Buf() = default;
+        Buf(Buf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {} // (declaring the moves deletes the copies)
+        Buf &operator=(Buf &&o) noexcept {
+                if (this != &o) {
+                        release();
+                        std::swap(p, o.p);
+                        std::swap(cap, o.cap);
+                }
+                return *this;
+        }
+        ~Buf() {
+                release();
+        }
+        // at least `bytes`; the contents are not kept
         cudaError_t ensure(size_t bytes) {
                 if (bytes <= cap)
                         return cudaSuccess;
-                if (p)
-                        cudaFree(p);
-                p   = nullptr;
-                cap = 0;
-                size_t want = bytes + bytes / 8 + 256;
-                cudaError_t e = cudaMalloc(&p, want);
+                release();
+                size_t      want = bytes + bytes / 8 + 256;
+                cudaError_t e    = Pinned ? cudaHostAlloc(&p, want, cudaHostAllocDefault) : cudaMalloc(&p, want);
                 if (e == cudaSuccess)
                         cap = want;
                 return e;
         }
+        // at least `need`, keeping the first `keep` bytes: they are copied once the copies queued on `s` have landed.  On failure the
+        // buffer is unchanged.
+        cudaError_t grow(size_t need, size_t keep, cudaStream_t s) {
+                static_assert(Pinned, "the old contents are copied on the host");
+                if (need <= cap)
+                        return cudaSuccess;
+                void *       np{nullptr};
+                const size_t want = need + need / 4 + 4096;
+                if (const cudaError_t e = cudaHostAlloc(&np, want, cudaHostAllocDefault); e != cudaSuccess)
+                        return e;
+                if (p && keep) {
+                        cudaStreamSynchronize(s);
+                        std::memcpy(np, p, keep);
+                }
+                release();
+                p   = np;
+                cap = want;
+                return cudaSuccess;
+        }
         void release() {
-                if (p)
-                        cudaFree(p);
+                if (p) {
+                        if constexpr (Pinned)
+                                cudaFreeHost(p);
+                        else
+                                cudaFree(p);
+                }
                 p   = nullptr;
                 cap = 0;
         }
@@ -58,32 +95,25 @@ struct DevBuf {
                 return static_cast<T *>(p);
         }
 };
-struct PinBuf {
-        void * p{nullptr};
-        size_t cap{0};
-        cudaError_t ensure(size_t bytes) {
-                if (bytes <= cap)
-                        return cudaSuccess;
-                if (p)
-                        cudaFreeHost(p);
-                p   = nullptr;
-                cap = 0;
-                size_t want = bytes + bytes / 8 + 256;
-                cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
-                if (e == cudaSuccess)
-                        cap = want;
-                return e;
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;
+
+// A CUDA event or stream the context created and destroys (null until created).  It converts to the handle the runtime calls take.
+template <class H, cudaError_t (*Destroy)(H)> struct Owned {
+        H h{nullptr};
+        Owned() = default;
+        Owned(const Owned &)            = delete;
+        Owned &operator=(const Owned &) = delete;
+        ~Owned() {
+                if (h)
+                        Destroy(h);
         }
-        void release() {
-                if (p)
-                        cudaFreeHost(p);
-                p   = nullptr;
-                cap = 0;
-        }
-        template <class T> T *as() const {
-                return static_cast<T *>(p);
+        operator H() const {
+                return h;
         }
 };
+using Event  = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
 } // namespace
 
 struct trn_ctx {
@@ -121,7 +151,7 @@ struct trn_ctx {
         GroupStarts          h_groups; // GOOGLE: the first docID of every 32-block group of every term (orders BatchPlan::cand_runs)
         // batch scratch (grow-only)
         DevBuf d_queries, d_steps, d_dense_runs, d_mixed_runs, d_cand_order, d_small[2], d_item_off, d_item_cnt, d_item_dst, d_seg_docids, d_seg_scores, d_out_docids[2], d_out_scores[2], d_q_offsets[2], d_cand,
-            d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums, d_merge_docids, d_merge_scores;
+            d_topk_docids, d_topk_scores, d_topk_counts, d_fq, d_leaves, d_luts, d_dec_units, d_dec_c, d_dec_docids, d_dec_freqs, d_dec_sums;
         PinBuf h_offsets, h_docids, h_scores, h_counts, h_small, h_chunk, h_item_desc;
         DevBuf d_hits, d_hit_base, d_hblk_off, d_hit_term; // LUCENE positions (trn_upload_hits)
         bool   have_hits{false};
@@ -132,11 +162,11 @@ struct trn_ctx {
         std::vector<trn_qitems> h_qitems;      // ... of the whole batch, item_base rebased (what trn_result::qitems points to)
         std::vector<std::vector<trn_qitems>> qitems_chunk; // pipelined call: per chunk, until its results have been queued for the copy
         uint64_t                last_items_hint{0};
-        cudaEvent_t ev0{nullptr}, ev1{nullptr}, evk0{nullptr}, evk1{nullptr};
-        bool        have_kernel_events{false};
+        Event ev0, ev1, evk0, evk1;
+        bool  have_kernel_events{false};
         // pipelined host-buffer path (trn_exec_batch): kernels of chunk i+1 overlap the D2H of chunk i
-        cudaStream_t copy_stream{nullptr};
-        cudaEvent_t  ev_done[2]{nullptr, nullptr}, ev_d2h[2]{nullptr, nullptr}, ev_ck0[16]{}, ev_ck1[16]{};
+        Stream       copy_stream;
+        Event        ev_done[2], ev_d2h[2], ev_ck0[16], ev_ck1[16];
         uint64_t     chunk_postings{1000000000ull}; // TRN_CHUNK_POSTINGS: referenced postings a pipeline chunk must carry (~1.1 ms of k_exec_docs)
         bool         taper_chunks{true};             // TRN_TAPER_CHUNKS=0: equal chunks only
         bool         chunk_rule_sqrt{true};          // TRN_CHUNK_RULE=postings: chunk count from the referenced postings alone
@@ -153,24 +183,13 @@ struct trn_ctx {
         int      last_mode{-1};
         uint32_t last_nq{0}, last_k{0}, last_launches{0};
         uint64_t last_postings{0}, last_bytes{0};
-        float    last_ms{0};
         std::vector<uint8_t> last_routes; // TRN_ROUTE_* of every query of the last batch (trn_debug_last_routes)
         // the default exec mode (trn_exec_matches): collect programs, per-chunk intermediates and outputs, the pinned result
         struct MatchBufs {
                 DevBuf d_cq, d_cterms, d_cphrases, d_cargs, d_cprog, d_mask, d_nterms, d_nhits, d_tscan, d_hscan, d_part, d_term_off, d_terms, d_freqs,
                     d_hit_off, d_hits, d_error;
-                PinBuf      h_doc_off, h_docids, h_term_off, h_terms, h_freqs, h_hit_off, h_hits, h_small;
-                cudaEvent_t ev_docs{nullptr}, ev_c0{nullptr}, ev_c1{nullptr}, ev_w0{nullptr}, ev_w1{nullptr}, ev_end{nullptr};
-                void release() {
-                        for (DevBuf *b : {&d_cq, &d_cterms, &d_cphrases, &d_cargs, &d_cprog, &d_mask, &d_nterms, &d_nhits, &d_tscan, &d_hscan, &d_part, &d_term_off,
-                                          &d_terms, &d_freqs, &d_hit_off, &d_hits, &d_error})
-                                b->release();
-                        for (PinBuf *b : {&h_doc_off, &h_docids, &h_term_off, &h_terms, &h_freqs, &h_hit_off, &h_hits, &h_small})
-                                b->release();
-                        for (cudaEvent_t e : {ev_docs, ev_c0, ev_c1, ev_w0, ev_w1, ev_end})
-                                if (e)
-                                        cudaEventDestroy(e);
-                }
+                PinBuf h_doc_off, h_docids, h_term_off, h_terms, h_freqs, h_hit_off, h_hits, h_small;
+                Event  ev_docs, ev_c0, ev_c1, ev_w0, ev_w1, ev_end;
         } mt;
         uint64_t match_chunk{1ull << 22}; // TRN_MATCH_CHUNK: matches per chunk of the write pass (halved while its outputs do not fit)
         // query-token intersections (trn_intersect): device scratch of both passes, the result
@@ -178,15 +197,7 @@ struct trn_ctx {
                 DevBuf d_reqs, d_tok, d_small, d_keys, d_first, d_tile_last, d_carry, d_base, d_cmask, d_cfirst, d_estart, d_eoff, d_smask, d_sslot, d_counts;
                 std::vector<uint64_t> offsets, masks;
                 std::vector<uint32_t> counts;
-                cudaEvent_t ev[4]{nullptr, nullptr, nullptr, nullptr};
-                void release() {
-                        for (DevBuf *b : {&d_reqs, &d_tok, &d_small, &d_keys, &d_first, &d_tile_last, &d_carry, &d_base, &d_cmask, &d_cfirst, &d_estart, &d_eoff, &d_smask,
-                                          &d_sslot, &d_counts})
-                                b->release();
-                        for (cudaEvent_t e : ev)
-                                if (e)
-                                        cudaEventDestroy(e);
-                }
+                Event                 ev[4];
         } it;
         uint32_t isect_max_masks{kIsectMaxMasks}; // TRN_ISECT_MAX_MASKS: distinct masks a request may have (lowers the limit only)
         // percolator (trn_percolator_register / trn_percolate): the registry, the batch scratch, the pinned result
@@ -197,40 +208,20 @@ struct trn_ctx {
                 DevBuf d_queries, d_ops, d_pterms, d_covers, d_csr_off, d_csr, d_unanch; // the registry
                 DevBuf d_doc_off, d_tokens, d_docs, d_counts, d_small, d_part, d_out_off, d_out, d_bitmaps, d_dense_slot;
                 PinBuf h_offsets, h_ids;
-                cudaEvent_t ev[4]{nullptr, nullptr, nullptr, nullptr};
-                void release() {
-                        for (DevBuf *b : {&d_queries, &d_ops, &d_pterms, &d_covers, &d_csr_off, &d_csr, &d_unanch, &d_doc_off, &d_tokens, &d_docs, &d_counts, &d_small, &d_part,
-                                          &d_out_off, &d_out, &d_bitmaps, &d_dense_slot})
-                                b->release();
-                        for (PinBuf *b : {&h_offsets, &h_ids})
-                                b->release();
-                        for (cudaEvent_t e : ev)
-                                if (e)
-                                        cudaEventDestroy(e);
-                }
+                Event  ev[4];
         } pq;
         // indexer (trn_index_documents): the last result (its working memory lives for one call only)
         struct IndexBufs {
                 std::vector<uint8_t>  index, hits;
                 std::vector<trn_term> terms;
-                cudaEvent_t           ev[5]{nullptr, nullptr, nullptr, nullptr, nullptr};
-                void release() {
-                        for (cudaEvent_t e : ev)
-                                if (e)
-                                        cudaEventDestroy(e);
-                }
+                Event                 ev[5];
         } ix;
         // merge (trn_merge_sources): the last result
         struct MergeBufs {
                 std::vector<uint8_t>  index, hits;
                 std::vector<trn_term> terms;
                 std::vector<uint32_t> term_source, term_index;
-                cudaEvent_t           ev[8]{};
-                void release() {
-                        for (cudaEvent_t e : ev)
-                                if (e)
-                                        cudaEventDestroy(e);
-                }
+                Event                 ev[8];
         } mg;
 };
 
@@ -319,19 +310,19 @@ extern "C" int trn_create(int device, trn_ctx **out) {
                 if (v >= 1 && v < (long long)kIsectMaxMasks)
                         c->isect_max_masks = uint32_t(v);
         }
-        CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+        CK(cudaStreamCreateWithFlags(&c->copy_stream.h, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
-                CK(cudaEventCreateWithFlags(&c->ev_done[i], cudaEventDisableTiming));
-                CK(cudaEventCreateWithFlags(&c->ev_d2h[i], cudaEventDisableTiming));
+                CK(cudaEventCreateWithFlags(&c->ev_done[i].h, cudaEventDisableTiming));
+                CK(cudaEventCreateWithFlags(&c->ev_d2h[i].h, cudaEventDisableTiming));
         }
         for (int i = 0; i < 16; ++i) {
-                CK(cudaEventCreate(&c->ev_ck0[i]));
-                CK(cudaEventCreate(&c->ev_ck1[i]));
+                CK(cudaEventCreate(&c->ev_ck0[i].h));
+                CK(cudaEventCreate(&c->ev_ck1[i].h));
         }
-        CK(cudaEventCreate(&c->ev0));
-        CK(cudaEventCreate(&c->ev1));
-        CK(cudaEventCreate(&c->evk0));
-        CK(cudaEventCreate(&c->evk1));
+        CK(cudaEventCreate(&c->ev0.h));
+        CK(cudaEventCreate(&c->ev1.h));
+        CK(cudaEventCreate(&c->evk0.h));
+        CK(cudaEventCreate(&c->evk1.h));
         return TRN_OK;
 }
 
@@ -339,31 +330,6 @@ extern "C" void trn_destroy(trn_ctx *c) {
         if (!c)
                 return;
         cudaSetDevice(c->device);
-        for (DevBuf *b : {&c->d_index, &c->d_blk_last, &c->d_blk_off, &c->d_terms, &c->d_tile_first, &c->d_masked, &c->d_dense, &c->d_dense_off, &c->d_probe_off, &c->d_queries, &c->d_steps, &c->d_dense_runs, &c->d_mixed_runs, &c->d_cand_order, &c->d_small[0], &c->d_small[1], &c->d_item_off,
-                          &c->d_item_cnt, &c->d_item_dst, &c->d_seg_docids, &c->d_seg_scores, &c->d_out_docids[0], &c->d_out_docids[1], &c->d_out_scores[0], &c->d_out_scores[1], &c->d_q_offsets[0], &c->d_q_offsets[1], &c->d_cand,
-                          &c->d_topk_docids, &c->d_topk_scores, &c->d_topk_counts, &c->d_fq, &c->d_leaves, &c->d_luts, &c->d_dec_units, &c->d_dec_c, &c->d_dec_docids, &c->d_dec_freqs,
-                          &c->d_dec_sums, &c->d_merge_docids, &c->d_merge_scores, &c->d_filters})
-                b->release();
-        for (auto &d : c->docsets)
-                d.bits.release();
-        for (PinBuf *b : {&c->h_offsets, &c->h_docids, &c->h_scores, &c->h_counts, &c->h_small, &c->h_chunk, &c->h_item_desc})
-                b->release();
-        for (cudaEvent_t e : {c->ev0, c->ev1, c->evk0, c->evk1, c->ev_done[0], c->ev_done[1], c->ev_d2h[0], c->ev_d2h[1]})
-                if (e)
-                        cudaEventDestroy(e);
-        for (int i = 0; i < 16; ++i) {
-                if (c->ev_ck0[i])
-                        cudaEventDestroy(c->ev_ck0[i]);
-                if (c->ev_ck1[i])
-                        cudaEventDestroy(c->ev_ck1[i]);
-        }
-        c->mt.release();
-        c->it.release();
-        c->pq.release();
-        c->ix.release();
-        c->mg.release();
-        if (c->copy_stream)
-                cudaStreamDestroy(c->copy_stream);
         delete c;
 }
 
@@ -453,8 +419,6 @@ static int upload_dense(trn_ctx *c) {
                 c->d_dense.release();
                 c->d_dense_off.release();
                 c->d_probe_off.release();
-                sel.release();
-                pre.release();
                 return TRN_OK;
         }
         CK(cudaMemsetAsync(c->d_dense.p, 0, (s.words + p.words) * 4, c->stream));
@@ -470,8 +434,6 @@ static int upload_dense(trn_ctx *c) {
         const cudaError_t le = launch_build_dense(dev_index(c), sel.as<uint32_t>(), pre.as<unsigned long long>(), uint32_t(order.size()), prefix.back(),
                                                   c->d_dense.as<uint32_t>(), c->stream);
         const cudaError_t se = cudaStreamSynchronize(c->stream);
-        sel.release();
-        pre.release();
         if (le != cudaSuccess || se != cudaSuccess) {
                 c->dense_terms = 0;
                 c->probe_terms = 0;
@@ -485,8 +447,6 @@ static int upload_dense(trn_ctx *c) {
 
 // every docID set of the context is dropped: its handles become stale (trn_upload_index; the sets' sizes follow the old max_docid)
 static void drop_docsets(trn_ctx *c) {
-        for (auto &d : c->docsets)
-                d.bits.release();
         c->docsets.clear();
         ++c->docset_epoch;
 }
@@ -695,18 +655,12 @@ extern "C" int trn_docset_create(trn_ctx *c, const uint32_t *docids, uint64_t n,
                 (void)cudaGetLastError(); // an allocation failure is not sticky: clear it
                 return fail(c, TRN_ERR_CAPACITY, std::string("trn_docset_create: ") + cudaGetErrorString(e));
         }
-        if (const cudaError_t ce = cudaMemcpyAsync(bits.p, words.data(), words.size() * 4, cudaMemcpyHostToDevice, c->stream); ce != cudaSuccess) {
-                bits.release();
-                CK(ce);
-        }
-        if (const cudaError_t se = cudaStreamSynchronize(c->stream); se != cudaSuccess) {
-                bits.release();
-                CK(se);
-        }
+        CK(cudaMemcpyAsync(bits.p, words.data(), words.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
         if (slot == c->docsets.size())
                 c->docsets.emplace_back();
         auto &D = c->docsets[slot];
-        D.bits  = bits;
+        D.bits  = std::move(bits);
         D.lo    = lo;
         D.hi    = hi;
         D.live  = true;
@@ -1198,7 +1152,6 @@ extern "C" int trn_fetch_results(trn_ctx *c, trn_result *out) {
                 out->device_ms = ms;
         if (c->have_kernel_events && cudaEventElapsedTime(&ms, c->evk0, c->evk1) == cudaSuccess)
                 out->exec_kernel_ms = ms;
-        c->last_ms = ms;
         return TRN_OK;
 }
 
@@ -1291,25 +1244,6 @@ extern "C" int trn_exec_batch_filtered(trn_ctx *c, const trn_query *queries, uin
                         q0 += n;
                 }
         }
-        auto grow = [&](PinBuf &b, size_t need, size_t keep) -> cudaError_t {
-                if (need <= b.cap)
-                        return cudaSuccess;
-                void *      np{nullptr};
-                const size_t want = need + need / 4 + 4096;
-                cudaError_t e = cudaHostAlloc(&np, want, cudaHostAllocDefault);
-                if (e != cudaSuccess)
-                        return e;
-                if (b.p && keep) {
-                        // earlier chunks' D2H into the old block must have landed before it is copied
-                        cudaStreamSynchronize(c->copy_stream);
-                        std::memcpy(np, b.p, keep);
-                }
-                if (b.p)
-                        cudaFreeHost(b.p);
-                b.p   = np;
-                b.cap = want;
-                return cudaSuccess;
-        };
         auto finish = [&](uint32_t j) -> int {
                 const int   set = int(j & 1);
                 const auto &C   = ch[j];
@@ -1336,9 +1270,9 @@ extern "C" int trn_exec_batch_filtered(trn_ctx *c, const trn_query *queries, uin
                 const uint64_t total = o[C.n];
                 // grow-only pinned result buffers; after the first batch the previous total is the hint that avoids regrowth
                 const size_t need = std::max<size_t>(4, std::max<uint64_t>(running + total, c->last_total_hint) * 4);
-                CK(grow(c->h_docids, need, running * 4));
+                CK(c->h_docids.grow(need, running * 4, c->copy_stream));
                 if (scored)
-                        CK(grow(c->h_scores, need, running * 4));
+                        CK(c->h_scores.grow(need, running * 4, c->copy_stream));
                 if (total) {
                         CK(cudaMemcpyAsync(c->h_docids.as<uint32_t>() + running, c->d_out_docids[set].p, total * 4, cudaMemcpyDeviceToHost, c->copy_stream));
                         if (scored)
@@ -1346,7 +1280,7 @@ extern "C" int trn_exec_batch_filtered(trn_ctx *c, const trn_query *queries, uin
                 }
                 if (compact) { // the chunk's segment descriptors; its queries' item ranges move behind the earlier chunks' items
                         const uint32_t ni = chunkItems[j];
-                        CK(grow(c->h_item_desc, std::max<size_t>(4, std::max<uint64_t>(runningItems + ni, c->last_items_hint) * 4), runningItems * 4));
+                        CK(c->h_item_desc.grow(std::max<size_t>(4, std::max<uint64_t>(runningItems + ni, c->last_items_hint) * 4), runningItems * 4, c->copy_stream));
                         if (ni)
                                 CK(cudaMemcpyAsync(c->h_item_desc.as<uint32_t>() + runningItems, c->d_item_desc[set].p, size_t(ni) * 4, cudaMemcpyDeviceToHost, c->copy_stream));
                         for (uint32_t i = 0; i < C.n; ++i) {
@@ -1477,8 +1411,8 @@ extern "C" int trn_exec_matches_filtered(trn_ctx *c, const trn_query *queries, u
         c->last_mode = -1;
         auto &M      = c->mt;
         if (!M.ev_docs) {
-                for (cudaEvent_t *e : {&M.ev_docs, &M.ev_c0, &M.ev_c1, &M.ev_w0, &M.ev_w1, &M.ev_end})
-                        CK(cudaEventCreate(e));
+                for (Event *e : {&M.ev_docs, &M.ev_c0, &M.ev_c1, &M.ev_w0, &M.ev_w1, &M.ev_end})
+                        CK(cudaEventCreate(&e->h));
         }
         const double t0 = now_ms();
         // ---- docs pass: the DocumentsOnly routes (root-filter quirk off) into d_out_docids[0] / d_q_offsets[0]
@@ -1846,13 +1780,6 @@ struct DevPostings {
         const uint8_t *           plens = nullptr;            // per hit: payload bytes (null: no payloads; needs positions)
         const unsigned long long *payloads = nullptr;         // per hit: the payload in its low plens[] bytes
 };
-struct FreeBufs {
-        std::vector<DevBuf *> v;
-        ~FreeBufs() {
-                for (auto b : v)
-                        b->release();
-        }
-};
 
 // The encode itself: sizes, scans and the write over device-resident postings; the chunks stay in d_out.  chunk[t] / toff[t] = bytes and
 // offset of term t's chunk, *out_bytes their total (set before the capacity refusals, as trn_encode_google documents), *nblocks the blocks
@@ -1872,7 +1799,6 @@ static int encode_google_device(trn_ctx *c, const DevPostings &P, uint32_t block
         }
         blk_begin[nterms] = nblocks;
         DevBuf   d_bb, d_hb, d_bsz, d_bterm, d_boff, d_part, d_toff, d_cb, d_err;
-        FreeBufs fr{{&d_bb, &d_hb, &d_bsz, &d_bterm, &d_boff, &d_part, &d_toff, &d_cb, &d_err}};
         const size_t parts = size_t(std::max(nposts, nblocks) / 4096 + 4);
         CK(d_bb.ensure((size_t(nterms) + 1) * 8));
         CK(d_bsz.ensure(std::max<size_t>(4, nblocks * 4)));
@@ -1976,7 +1902,6 @@ extern "C" int trn_encode_google_payloads(trn_ctx *c, const uint64_t *term_begin
                         nhits += freqs[i];
         const uint32_t phase0 = countdown ? (skiplist_step - *countdown) % skiplist_step : 0u;
         DevBuf         d_tb, d_doc, d_fr, d_pos, d_out;
-        FreeBufs       fr{{&d_tb, &d_doc, &d_fr, &d_pos, &d_out}};
         CK(d_tb.ensure((size_t(nterms) + 1) * 8));
         CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
         CK(d_fr.ensure(std::max<size_t>(4, nposts * 4)));
@@ -1991,7 +1916,6 @@ extern "C" int trn_encode_google_payloads(trn_ctx *c, const uint64_t *term_begin
                         CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
         }
         DevBuf   d_pl, d_pv;
-        FreeBufs frp{{&d_pl, &d_pv}};
         if (payload_lens) {
                 CK(d_pl.ensure(std::max<size_t>(4, nhits)));
                 CK(d_pv.ensure(std::max<size_t>(8, nhits * 8)));
@@ -2051,7 +1975,6 @@ static int encode_lucene_device(trn_ctx *c, const DevPostings &P, bool have_inde
         dunit[nterms] = ndunits;
         fixed[nterms] = fx;
         DevBuf   d_du, d_hu, d_fx, d_hb, d_th, d_dsz, d_hsz, d_dterm, d_hterm, d_doff, d_hoff, d_part, d_toff, d_hto, d_err;
-        FreeBufs fr{{&d_du, &d_hu, &d_fx, &d_hb, &d_th, &d_dsz, &d_hsz, &d_dterm, &d_hterm, &d_doff, &d_hoff, &d_part, &d_toff, &d_hto, &d_err}};
         const size_t tw = (size_t(nterms) + 1) * 8;
         CK(d_du.ensure(tw));
         CK(d_hu.ensure(tw));
@@ -2178,7 +2101,6 @@ extern "C" int trn_encode_lucene_payloads(trn_ctx *c, const uint64_t *term_begin
                         nhits += freqs[i];
         CK(cudaSetDevice(c->device));
         DevBuf   d_tb, d_doc, d_fr, d_pos, d_iout, d_hout;
-        FreeBufs fr{{&d_tb, &d_doc, &d_fr, &d_pos, &d_iout, &d_hout}};
         const size_t tw = (size_t(nterms) + 1) * 8;
         CK(d_tb.ensure(tw));
         CK(d_doc.ensure(std::max<size_t>(4, nposts * 4)));
@@ -2193,7 +2115,6 @@ extern "C" int trn_encode_lucene_payloads(trn_ctx *c, const uint64_t *term_begin
                 CK(cudaMemcpyAsync(d_pos.p, positions, nhits * 4, cudaMemcpyHostToDevice, c->stream));
         }
         DevBuf   d_pl, d_pv;
-        FreeBufs frp{{&d_pl, &d_pv}};
         DevPostings P{term_begin, nterms, d_tb.as<unsigned long long>(), d_doc.as<uint32_t>(), d_fr.as<uint32_t>(), nhits ? d_pos.as<uint32_t>() : nullptr};
         if (payload_lens && nhits) {
                 CK(d_pl.ensure(nhits));
@@ -2334,14 +2255,12 @@ extern "C" int trn_index_documents_payloads(trn_ctx *c, int codec, const uint32_
         auto &X = c->ix;
         for (auto &e : X.ev)
                 if (!e)
-                        CK(cudaEventCreate(&e));
+                        CK(cudaEventCreate(&e.h));
         const auto doc_of_token = [&](uint64_t i) { return uint32_t(std::upper_bound(doc_offsets, doc_offsets + ndocs + 1, i) - doc_offsets) - 1u; };
         const auto who          = [&](uint32_t d) { return "trn_index_documents: document " + std::to_string(d) + " (docID " + std::to_string(docids[d]) + "): "; };
 
         DevBuf   d_docids, d_doff, d_tok, d_pos, d_ka, d_kb, d_rank, d_docid_of, d_err, d_counts, d_part, d_offs, d_pflag, d_tflag, d_pscan, d_tscan, d_pbegin, d_tb, d_order,
             d_odoc, d_ofreq, d_opos, d_docterms, d_out, d_hout, d_pl, d_pv, d_va, d_vb, d_opl, d_opv;
-        FreeBufs fr{{&d_docids, &d_doff, &d_tok, &d_pos, &d_ka, &d_kb, &d_rank, &d_docid_of, &d_err, &d_counts, &d_part, &d_offs, &d_pflag, &d_tflag, &d_pscan,
-                     &d_tscan, &d_pbegin, &d_tb, &d_order, &d_odoc, &d_ofreq, &d_opos, &d_docterms, &d_out, &d_hout, &d_pl, &d_pv, &d_va, &d_vb, &d_opl, &d_opv}};
         uint64_t herr[IDX_ERR_KINDS];
         // ---- documents: ranks in docID order, docID 0 and duplicates
         CKM(d_docids.ensure(size_t(ndocs) * 4));
@@ -2676,8 +2595,8 @@ extern "C" int trn_intersect(trn_ctx *c, const trn_isect_req *reqs, uint32_t n, 
         const double t0 = now_ms();
         auto &       B  = c->it;
         if (!B.ev[0])
-                for (cudaEvent_t &e : B.ev)
-                        CK(cudaEventCreate(&e));
+                for (Event &e : B.ev)
+                        CK(cudaEventCreate(&e.h));
 
         // ---- the requests: known tokens (deduplicated per group), tile geometry, mask tables
         std::vector<IsectReq> rq(n);
@@ -2983,8 +2902,8 @@ extern "C" int trn_percolate(trn_ctx *c, const uint64_t *doc_offsets, const uint
         std::memset(out, 0, sizeof(*out));
         const double t0 = now_ms();
         if (!B.ev[0])
-                for (cudaEvent_t &e : B.ev)
-                        CK(cudaEventCreate(&e));
+                for (Event &e : B.ev)
+                        CK(cudaEventCreate(&e.h));
 
         // ---- the documents: lengths, tokens, the short and the long launch
         const uint64_t base = ndocs ? doc_offsets[0] : 0, ntok = ndocs ? doc_offsets[ndocs] - base : 0;
@@ -3185,7 +3104,7 @@ static int merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src,
         auto &X = c->mg;
         for (auto &e : X.ev)
                 if (!e)
-                        CK(cudaEventCreate(&e));
+                        CK(cudaEventCreate(&e.h));
         // ---- the sources' directories (host, as trn_upload_index / trn_upload_hits build them)
         std::vector<uint8_t>              used(n, 0);
         std::vector<BlockDirectory>       dirs(n);
@@ -3248,10 +3167,6 @@ static int merge_sources(trn_ctx *c, int out_codec, const trn_merge_source *src,
         // ---- upload: every used source's bytes and directories, one view per source
         DevBuf   d_idx, d_hits, d_bl, d_bo, d_tf, d_hb, d_hbo, d_ht, d_views, d_lists, d_lblk, d_lpost, d_ud, d_uf, d_doc, d_fr, d_hc, d_hoff, d_pos, d_keep, d_ks,
             d_bm, d_part, d_odoc, d_ofr, d_osrc, d_ohoff, d_opos, d_err, d_cnt, d_idx2, d_tb, d_th, d_enc, d_henc, d_segs, d_oi, d_oh, d_pl, d_pv, d_opl, d_opv;
-        FreeBufs fr{{&d_idx,  &d_hits, &d_bl,   &d_bo,   &d_tf,    &d_hb,   &d_hbo, &d_ht,  &d_views, &d_lists, &d_lblk, &d_lpost, &d_ud,
-                     &d_uf,   &d_doc,  &d_fr,   &d_hc,   &d_hoff,  &d_pos,  &d_keep, &d_ks, &d_bm,    &d_part,  &d_odoc, &d_ofr,   &d_osrc,
-                     &d_ohoff, &d_opos, &d_err, &d_cnt, &d_idx2, &d_tb,  &d_th,  &d_enc, &d_henc,  &d_segs,  &d_oi,   &d_oh,  &d_pl,  &d_pv,
-                     &d_opl,   &d_opv}};
         std::vector<uint64_t> ibase(n + 1, 0), hbase(n + 1, 0), dbase(n + 1, 0), tbase(n + 1, 0), hbbase(n + 1, 0), termbase(n + 1, 0);
         for (uint32_t s = 0; s < n; ++s) {
                 const bool u = used[s];
