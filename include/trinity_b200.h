@@ -574,6 +574,7 @@ int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *firsts, uint
  *   Registry   trn_percolator_register: the same trn_qnode trees trn_exec_batch takes; query ids are indices into `queries`; registering
  *              again replaces the set.  Term ids index a percolator vocabulary of `nterms` terms; TRN_EMPTY_TERM is a query term outside it.
  *              term_cost (optional, nterms entries; NULL: all equal), e.g. each term's document frequency, only chooses the anchors.
+ *              trn_percolator_add / trn_percolator_remove change the registered set in place (below).
  *   Documents  trn_percolate: document d is tokens[doc_offsets[d] .. doc_offsets[d + 1]) and token i sits at position i + 1; a token
  *              outside the vocabulary is TRN_EMPTY_TERM: it takes up a position and equals no query term, not even TRN_EMPTY_TERM.
  *   Meaning    query q matches document d exactly when percolator_query(q).match(proxy) returns true for the proxy whose match_term(t) says
@@ -586,16 +587,45 @@ int trn_debug_intersect_plan(const uint64_t *masks, const uint32_t *firsts, uint
  *              phrase of more than 16 terms (Limits::MaxPhraseSize), a term id >= nterms other than TRN_EMPTY_TERM, a document token >= nterms
  *              other than TRN_EMPTY_TERM, a document of more than 16383 tokens (positions below Limits::MaxPosition).  TRN_ERR_UNSUPPORTED:
  *              a query whose post-order program needs more than 64 pending operands (an operator with more than 64 operands).
- *              TRN_ERR_STATE: trn_percolate without a registry.  TRN_ERR_CAPACITY: the batch's matches cannot be staged (split the batch). */
+ *              TRN_ERR_STATE: trn_percolate without a registry.  TRN_ERR_CAPACITY: the batch's matches cannot be staged (split the batch).
+ *              TRN_PERC_MAX_IDS / TRN_PERC_MAX_ENTRIES lower the id and anchor-entry limits (tests). */
 typedef struct trn_percolator_info {
         uint32_t nqueries;
         uint32_t unanchored;     /* queries a match may hold none of the terms of (evaluated for every document) */
         uint32_t never;          /* queries no document can match (never evaluated) */
-        uint32_t pad;
+        uint32_t next_id;        /* the id the next added query gets (nqueries right after a registration) */
         uint64_t anchor_entries; /* (term, query) entries of the term -> anchored-queries index */
-        uint64_t device_bytes;   /* the registry in HBM */
+        uint64_t device_bytes;   /* the registry in HBM: the bytes uploaded after a registration, the buffers' capacity after an add or remove */
 } trn_percolator_info;
+/* nqueries / unanchored / never / anchor_entries describe the live queries (issued and not removed). */
 int trn_percolator_register(trn_ctx *, const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, trn_percolator_info *out);
+/* In-place changes of the registered set.  After any sequence of register / add / remove, trn_percolate returns exactly what registering
+ * the live queries fresh returns, with ids mapped through the live ids: the same matches per document, ascending id, and the same
+ * `candidates`.  The anchor index and the unanchored list are rebuilt on the device into what a fresh registration of every issued query
+ * would hold minus the removed ones; k_perc reads them as it reads a registration's.
+ *   trn_percolator_add     appends nq queries with the ids *first_id .. *first_id + nq - 1 (ids are never reused until the next
+ *                          trn_percolator_register, which starts again at 0).  Same trees, vocabulary (nterms) and term_cost as the
+ *                          registration: growing the vocabulary or changing the costs means registering again.
+ *   trn_percolator_remove  removes live queries: no later trn_percolate returns them.
+ * Refusals, atomic: a refused call leaves the registry, and the last trn_percolate result, exactly as they were.  trn_percolator_add returns
+ * the codes trn_percolator_register returns for the same input, naming the query by its index in the batch; TRN_ERR_CAPACITY when ids
+ * would reach 0xFFFFFFFF (it pads the sort in k_perc, so it is never an id) or anchor entries 2^32.  trn_percolator_remove: TRN_ERR_ARG,
+ * naming the id, for an id never issued, already removed or given twice.  Either: TRN_ERR_STATE without a registry; TRN_ERR_CAPACITY /
+ * TRN_ERR_CUDA when device memory cannot be allocated (the new index is built in new buffers and replaces the old one only on success).
+ * nq == 0 / n == 0: a no-op.
+ * Memory: the programs of added queries are appended (a full buffer is replaced by one twice its size); when the program words of removed
+ * queries outnumber the live ones, the program storage is compacted on the device.  The per-id query table (16 B per id ever issued) and
+ * the bitmap width of a document with more than 4096 matches (next_id / 32 words) grow with next_id until the next registration. */
+int trn_percolator_add(trn_ctx *, const trn_query *queries, uint32_t nq, uint32_t *first_id, trn_percolator_info *out);
+int trn_percolator_remove(trn_ctx *, const uint32_t *ids, uint32_t n, trn_percolator_info *out);
+/* CUDA-event time of the device work of the last successful trn_percolator_add / trn_percolator_remove (its uploads, program copies and
+ * rebuild kernels) and its host time, ms. */
+int trn_percolator_last_update(trn_ctx *, float *device_ms, float *host_ms);
+/* Debug view (tests, tooling): copies the resident index and unanchored list to the host.  csr_off: *nterms + 1 entries; csr: 2 words per
+ * entry (query id, anchor ordinal), entry e of term t at csr_off[t] <= e < csr_off[t + 1]; unanchored: ascending ids.  Any output may be
+ * NULL (then *nterms, *nentries and *nunanchored still report the sizes); cap / ucap entries at most, TRN_ERR_CAPACITY beyond. */
+int trn_debug_percolator_registry(trn_ctx *, uint32_t *csr_off, uint32_t *csr, uint64_t cap, uint32_t *unanchored, uint64_t ucap, uint32_t *nterms,
+                                  uint64_t *nentries, uint64_t *nunanchored);
 /* owned by the ctx, valid until the next trn_percolate: document d owns [offsets[d], offsets[d + 1]) of queries (ascending, no duplicates) */
 typedef struct trn_percolation {
         uint32_t        ndocs;

@@ -859,7 +859,40 @@ class GpuIndexSource:
         i = TrnPercolatorInfo()
         self._ck(self._L.trn_percolator_register(self._h, C.cast(arr, C.c_void_p), len(queries), nterms, _ptr(cost) if cost is not None else None,
                                                  C.byref(i)))
-        return {f: int(getattr(i, f)) for f, _ in TrnPercolatorInfo._fields_ if f != "pad"}
+        self.percolator_info = {f: int(getattr(i, f)) for f, _ in TrnPercolatorInfo._fields_}
+        return dict(self.percolator_info)
+
+    def percolator_add(self, queries: Sequence[np.ndarray]) -> np.ndarray:
+        """appends queries (trn_qnode trees over the registration's vocabulary) to the registered set; returns their ids (uint32, ascending
+        from the info's next_id).  A refused call adds none of them."""
+        arr, keep = _pack_queries(queries)
+        i, first = TrnPercolatorInfo(), C.c_uint32()
+        self._ck(self._L.trn_percolator_add(self._h, C.cast(arr, C.c_void_p) if len(queries) else None, len(queries), C.byref(first), C.byref(i)))
+        self.percolator_info = {f: int(getattr(i, f)) for f, _ in TrnPercolatorInfo._fields_}
+        return np.arange(first.value, first.value + len(queries), dtype=np.uint32)
+
+    def percolator_remove(self, ids) -> dict:
+        """removes live queries by id: no later percolate() returns them.  A refused call removes none of them."""
+        a = _u32(ids).ravel()
+        i = TrnPercolatorInfo()
+        self._ck(self._L.trn_percolator_remove(self._h, _ptr(a) if len(a) else None, len(a), C.byref(i)))
+        self.percolator_info = {f: int(getattr(i, f)) for f, _ in TrnPercolatorInfo._fields_}
+        return dict(self.percolator_info)
+
+    def percolator_last_update(self) -> dict:
+        """device time (CUDA events around its uploads, copies and rebuild kernels) and host time of the last add / remove, ms"""
+        dev, host = C.c_float(), C.c_float()
+        self._ck(self._L.trn_percolator_last_update(self._h, C.byref(dev), C.byref(host)))
+        return {"device_ms": float(dev.value), "host_ms": float(host.value)}
+
+    def debug_percolator_registry(self):
+        """the resident anchor index and unanchored list: (csr_off[nterms + 1], csr[entries, 2] of (query id, anchor ordinal), unanchored)"""
+        nt, ne, nu = C.c_uint32(), C.c_uint64(), C.c_uint64()
+        self._ck(self._L.trn_debug_percolator_registry(self._h, None, None, 0, None, 0, C.byref(nt), C.byref(ne), C.byref(nu)))
+        off, csr, un = np.zeros(nt.value + 1, np.uint32), np.zeros((ne.value, 2), np.uint32), np.zeros(nu.value, np.uint32)
+        self._ck(self._L.trn_debug_percolator_registry(self._h, _ptr(off), _ptr(csr), ne.value, _ptr(un), nu.value, C.byref(nt), C.byref(ne),
+                                                       C.byref(nu)))
+        return off, csr, un
 
     def percolate(self, docs: Sequence[np.ndarray]) -> "PercolationResult":
         """every registered query each document matches: docs are uint32 token arrays (EMPTY_TERM: a token outside the vocabulary)"""
@@ -972,12 +1005,24 @@ class Percolator:
     """== Trinity's percolator_query::match (percolator.h) for a whole registered query set at once: which stored queries each incoming
     document matches.  queries: trn_qnode trees (parse_query); nterms: the size of the vocabulary their term ids index; term_cost: optional
     per-term cost (e.g. document frequency) that picks each query's anchors; source: a GpuIndexSource whose context to share (its index and
-    exec_batch stay as they are), else a context of its own on `device`."""
+    exec_batch stay as they are), else a context of its own on `device`.  add() / remove() change the set in place: it then answers what
+    registering the live queries fresh would, under the ids add() returned."""
 
     def __init__(self, queries: Sequence[np.ndarray], device: int = 0, nterms: int = 0, term_cost=None, source: Optional["GpuIndexSource"] = None):
         self.source = source if source is not None else GpuIndexSource(device)
         self._info = self.source.percolator_register(queries, nterms, term_cost)
         self._last = None
+
+    def add(self, queries: Sequence[np.ndarray]) -> np.ndarray:
+        """adds queries (parse_query trees over the registration's vocabulary) to the set; returns their new ids (uint32).  Ids are never
+        reused; the vocabulary and term_cost stay the registration's."""
+        ids = self.source.percolator_add(queries)
+        self._info = dict(self.source.percolator_info)
+        return ids
+
+    def remove(self, ids) -> None:
+        """removes queries by id; an id never issued, already removed or given twice is refused, and then none is removed"""
+        self._info = self.source.percolator_remove(ids)
 
     def percolate(self, docs: Sequence[np.ndarray]) -> PercolationResult:
         self._last = self.source.percolate(docs)
@@ -994,6 +1039,10 @@ class Percolator:
         """device times (ms) of the count and write passes of the last percolate() call and its host time"""
         r = self._last
         return {} if r is None else {"count_ms": r.count_ms, "write_ms": r.write_ms, "total_ms": r.total_ms}
+
+    def last_update_timings(self) -> dict:
+        """device time (ms, CUDA events) and host time of the last add() / remove()"""
+        return self.source.percolator_last_update()
 
 
 def debug_percolator_plan(queries: Sequence[np.ndarray], nterms: int, term_cost=None):

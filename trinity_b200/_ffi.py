@@ -24,7 +24,8 @@ EXPORTS = [
     "trn_encode_google_payloads", "trn_encode_lucene_payloads", "trn_index_documents_payloads",
     "trn_debug_last_routes", "trn_debug_plan", "trn_debug_dense_runs", "trn_debug_mixed_runs", "trn_debug_cand_runs", "trn_debug_dense_terms", "trn_debug_probe_terms", "trn_debug_dense_bitmap",
     "trn_exec_matches", "trn_debug_hits", "trn_intersect", "trn_debug_intersect_plan",
-    "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan",
+    "trn_percolator_register", "trn_percolate", "trn_debug_percolator_plan", "trn_percolator_add", "trn_percolator_remove",
+    "trn_percolator_last_update", "trn_debug_percolator_registry",
     "trn_index_documents", "trn_segment_write", "trn_merge_sources", "trn_merge_sources_payloads", "trn_debug_merge_plan",
     "trn_docset_create", "trn_docset_destroy", "trn_exec_batch_filtered", "trn_exec_batch_device_filtered", "trn_exec_matches_filtered",
 ]
@@ -79,7 +80,7 @@ class TrnIntersections(C.Structure):
 
 
 class TrnPercolatorInfo(C.Structure):
-    _fields_ = [("nqueries", C.c_uint32), ("unanchored", C.c_uint32), ("never", C.c_uint32), ("pad", C.c_uint32), ("anchor_entries", C.c_uint64),
+    _fields_ = [("nqueries", C.c_uint32), ("unanchored", C.c_uint32), ("never", C.c_uint32), ("next_id", C.c_uint32), ("anchor_entries", C.c_uint64),
                 ("device_bytes", C.c_uint64)]
 
 
@@ -222,6 +223,10 @@ def lib() -> C.CDLL:
     sig("trn_percolator_register", i32, vp, vp, u32, u32, vp, P(TrnPercolatorInfo))
     sig("trn_percolate", i32, vp, vp, vp, u32, P(TrnPercolation))
     sig("trn_debug_percolator_plan", i32, vp, u32, u32, vp, vp, vp, vp, u64, P(u64), C.c_char_p, C.c_size_t)
+    sig("trn_percolator_add", i32, vp, vp, u32, P(u32), P(TrnPercolatorInfo))
+    sig("trn_percolator_remove", i32, vp, vp, u32, P(TrnPercolatorInfo))
+    sig("trn_percolator_last_update", i32, vp, P(C.c_float), P(C.c_float))
+    sig("trn_debug_percolator_registry", i32, vp, vp, vp, u64, vp, u64, P(u32), P(u64), P(u64))
     sig("trn_index_documents", i32, vp, i32, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
     sig("trn_index_documents_payloads", i32, vp, i32, vp, vp, vp, vp, vp, vp, u32, u32, P(TrnIndexed))
     sig("trn_segment_write", i32, C.c_char_p, i32, vp, u64, vp, u64, vp, vp, u32, u64, u32, u64, u32, vp, u64, C.c_char_p, C.c_size_t)

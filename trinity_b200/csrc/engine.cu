@@ -200,12 +200,29 @@ struct trn_ctx {
                 Event                 ev[4];
         } it;
         uint32_t isect_max_masks{kIsectMaxMasks}; // TRN_ISECT_MAX_MASKS: distinct masks a request may have (lowers the limit only)
+        uint64_t perc_max_ids{0xFFFFFFFFull};      // TRN_PERC_MAX_IDS: ids a registry may issue (lowers the limit only)
+        uint64_t perc_max_entries{1ull << 32};     // TRN_PERC_MAX_ENTRIES: anchor entries a registry may hold (lowers the limit only)
         // percolator (trn_percolator_register / trn_percolate): the registry, the batch scratch, the pinned result
         struct PercBufs {
                 bool                have{false};
-                uint32_t            nq{0}, nterms{0}, nunanchored{0};
+                uint32_t            next_id{0}, nterms{0}, nunanchored{0}; // next_id: ids issued since the registration (removed ones included)
                 trn_percolator_info info{};
                 DevBuf d_queries, d_ops, d_pterms, d_covers, d_csr_off, d_csr, d_unanch; // the registry
+                // the host's view of the registry for trn_percolator_add / trn_percolator_remove
+                struct Sizes {
+                        uint32_t nops, npt, ncover;
+                        uint8_t  status;
+                };
+                std::vector<Sizes>    sizes;     // per issued id
+                std::vector<uint32_t> removed;   // bitmap over the issued ids
+                std::vector<uint32_t> term_cost; // the registration's (empty: all equal)
+                uint32_t              nlive{0}, nnever{0};
+                uint64_t              nentries{0};                              // entries of d_csr
+                uint64_t              ops_used{0}, pt_used{0}, cov_used{0};     // entries of d_ops / d_pterms / d_covers in use ...
+                uint64_t              dead_words{0};                            // ... and the words of removed queries among them
+                DevBuf d_removed, d_keep, d_kscan, d_upart, d_cnt, d_toff, d_new, d_new_terms, d_new_unanch; // update scratch (grow-only)
+                Event  uev[2];
+                float  update_ms{0}, update_host_ms{0}; // the last add / remove: CUDA-event time of its device work, host time
                 DevBuf d_doc_off, d_tokens, d_docs, d_counts, d_small, d_part, d_out_off, d_out, d_bitmaps, d_dense_slot;
                 PinBuf h_offsets, h_ids;
                 Event  ev[4];
@@ -309,6 +326,16 @@ extern "C" int trn_create(int device, trn_ctx **out) {
                 const long long v = atoll(e);
                 if (v >= 1 && v < (long long)kIsectMaxMasks)
                         c->isect_max_masks = uint32_t(v);
+        }
+        if (const char *e = getenv("TRN_PERC_MAX_IDS")) {
+                const long long v = atoll(e);
+                if (v >= 1 && uint64_t(v) < c->perc_max_ids)
+                        c->perc_max_ids = uint64_t(v);
+        }
+        if (const char *e = getenv("TRN_PERC_MAX_ENTRIES")) {
+                const long long v = atoll(e);
+                if (v >= 1 && uint64_t(v) < c->perc_max_entries)
+                        c->perc_max_entries = uint64_t(v);
         }
         CK(cudaStreamCreateWithFlags(&c->copy_stream.h, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
@@ -2863,6 +2890,9 @@ extern "C" int trn_percolator_register(trn_ctx *c, const trn_query *queries, uin
         std::string err;
         if (const int rc = perc_plan(queries, nq, nterms, term_cost, P, err))
                 return fail(c, rc, "trn_percolator_register: " + err);
+        if (nq > c->perc_max_ids || P.csr.size() >= c->perc_max_entries)
+                return fail(c, TRN_ERR_CAPACITY, "trn_percolator_register: " + std::to_string(nq) + " queries with " + std::to_string(P.csr.size()) +
+                                                     " anchor entries exceed the registry's limits");
         auto &B = c->pq;
         B.have  = false;
         uint64_t bytes{0};
@@ -2880,10 +2910,22 @@ extern "C" int trn_percolator_register(trn_ctx *c, const trn_query *queries, uin
         CK(upload(B.d_csr, P.csr.data(), P.csr.size() * sizeof(PercEntry)));
         CK(upload(B.d_unanch, P.unanchored.data(), P.unanchored.size() * 4));
         CK(cudaStreamSynchronize(c->stream));
-        B.nq          = nq;
+        B.next_id     = nq;
         B.nterms      = nterms;
         B.nunanchored = uint32_t(P.unanchored.size());
-        B.info        = trn_percolator_info{nq, B.nunanchored, P.never, 0, P.csr.size(), bytes};
+        B.sizes.resize(nq);
+        for (uint32_t q = 0; q < nq; ++q)
+                B.sizes[q] = {P.queries[q].nops, P.npt[q], P.queries[q].ncover, P.status[q]};
+        B.removed.assign((size_t(nq) + 31u) / 32u, 0u);
+        B.term_cost.assign(term_cost, term_cost ? term_cost + nterms : term_cost);
+        B.nlive       = nq;
+        B.nnever      = P.never;
+        B.nentries    = P.csr.size();
+        B.ops_used    = P.ops.size();
+        B.pt_used     = P.phrase_terms.size();
+        B.cov_used    = P.covers.size();
+        B.dead_words  = 0;
+        B.info        = trn_percolator_info{nq, B.nunanchored, P.never, nq, P.csr.size(), bytes};
         B.have        = true;
         if (out)
                 *out = B.info;
@@ -2990,7 +3032,7 @@ extern "C" int trn_percolate(trn_ctx *c, const uint64_t *doc_offsets, const uint
         for (uint32_t d = 0; d < ndocs; ++d)
                 if (hoff[d + 1] - hoff[d] > kPercSortCap)
                         slot[d] = ndense++;
-        const uint32_t words = (B.nq + 31u) / 32u;
+        const uint32_t words = (B.next_id + 31u) / 32u;
         auto capacity = [&](cudaError_t e, const char *what) {
                 (void)cudaGetLastError();
                 return fail(c, e == cudaErrorMemoryAllocation ? TRN_ERR_CAPACITY : TRN_ERR_CUDA,
@@ -3031,6 +3073,297 @@ extern "C" int trn_percolate(trn_ctx *c, const uint64_t *doc_offsets, const uint
         out->count_ms   = countMs;
         out->write_ms   = writeMs;
         out->total_ms   = float(now_ms() - t0);
+        return TRN_OK;
+}
+
+// ---- trn_percolator_add / trn_percolator_remove (DESIGN.md §4): the added queries are planned on the host (perc_plan_queries on the slice)
+// and their programs appended; the anchor index and the unanchored list are rebuilt on the device (percolate_update.cuh) into new buffers,
+// and program storage that grows or is compacted goes to new buffers too.  They replace the old ones only once every step has succeeded, so
+// a refused or failed call leaves the registry, and the last trn_percolate result, as they were.
+#define CKPU(call)                                                                                                                                             \
+        do {                                                                                                                                                   \
+                cudaError_t e__ = (call);                                                                                                                      \
+                if (e__ != cudaSuccess) {                                                                                                                      \
+                        (void)cudaGetLastError();                                                                                                              \
+                        return fail(c, e__ == cudaErrorMemoryAllocation ? TRN_ERR_CAPACITY : TRN_ERR_CUDA,                                                    \
+                                    std::string(fn) + ": " + #call + ": " + cudaGetErrorString(e__) + " (the registry is unchanged)");                        \
+                }                                                                                                                                              \
+        } while (0)
+
+static uint64_t perc_registry_bytes(const trn_ctx::PercBufs &B) {
+        return B.d_queries.cap + B.d_ops.cap + B.d_pterms.cap + B.d_covers.cap + B.d_csr_off.cap + B.d_csr.cap + B.d_unanch.cap;
+}
+
+static void perc_refresh_info(trn_ctx::PercBufs &B) {
+        B.info = trn_percolator_info{B.nlive, B.nunanchored, B.nnever, B.next_id, B.nentries, perc_registry_bytes(B)};
+}
+
+// The device half of an add (S: the added queries' plan, rebased onto the used program storage; their ids start at B.next_id) or a remove
+// (removed: the bitmap of every removed id after the call; compact: rewrite the program storage without the removed queries).  nentries /
+// nunanchored: the index's entries and the unanchored ids after the call (the host knows them from the per-id sizes).
+static int perc_update(trn_ctx *c, const char *fn, const PercPlan *S, const std::vector<uint32_t> *removed, bool compact, uint64_t nentries,
+                       uint32_t nunanchored) {
+        auto &         B  = c->pq;
+        const double   t0 = now_ms();
+        const uint32_t nt = B.nterms, nq = B.next_id, nadd = S ? uint32_t(S->queries.size()) : 0u;
+        // the added queries' anchor entries, by (term, id)
+        std::vector<PercEntry> ne;
+        std::vector<uint32_t>  nterm;
+        if (S) {
+                std::vector<std::pair<uint32_t, PercEntry>> e;
+                e.reserve(S->covers.size());
+                for (uint32_t q = 0; q < nadd; ++q)
+                        for (uint32_t j = 0; j < S->queries[q].ncover; ++j)
+                                e.push_back({S->covers[S->queries[q].cover_begin - B.cov_used + j], PercEntry{nq + q, j}});
+                std::stable_sort(e.begin(), e.end(), [](const auto &a, const auto &b) { return a.first < b.first; });
+                for (const auto &x : e) {
+                        nterm.push_back(x.first);
+                        ne.push_back(x.second);
+                }
+        }
+        const uint64_t nold = B.nentries, nold_u = B.nunanchored, nnew = ne.size();
+        const uint32_t nadd_u = S ? uint32_t(S->unanchored.size()) : 0u;
+        if (!B.uev[0])
+                for (Event &e : B.uev)
+                        CKPU(cudaEventCreate(&e.h));
+        cudaStream_t st = c->stream;
+        auto         up = [&](DevBuf &b, const void *src, size_t n) -> cudaError_t {
+                if (const cudaError_t e = b.ensure(std::max<size_t>(16, n)); e != cudaSuccess)
+                        return e;
+                return n ? cudaMemcpyAsync(b.p, src, n, cudaMemcpyHostToDevice, st) : cudaSuccess;
+        };
+        const uint64_t nmax = std::max<uint64_t>({nold, nold_u, nt, nq});
+        CKPU(B.d_keep.ensure(std::max<size_t>(16, nmax * 4)));
+        CKPU(B.d_kscan.ensure((nmax + 1) * 8));
+        CKPU(B.d_upart.ensure((nmax / 4096 + 2) * 8));
+        CKPU(B.d_cnt.ensure(std::max<size_t>(16, size_t(nt) * 4)));
+        CKPU(B.d_toff.ensure((size_t(nt) + 1) * 8));
+        DevBuf n_off, n_csr, n_un; // the rebuilt index and unanchored list
+        CKPU(n_off.ensure((size_t(nt) + 1) * 4));
+        CKPU(n_csr.ensure(std::max<size_t>(16, nentries * sizeof(PercEntry))));
+        CKPU(n_un.ensure(std::max<size_t>(16, size_t(nunanchored) * 4)));
+        const uint32_t *rm = nullptr;
+        if (removed) {
+                CKPU(up(B.d_removed, removed->data(), removed->size() * 4));
+                rm = B.d_removed.as<uint32_t>();
+        }
+        CKPU(cudaEventRecord(B.uev[0], st));
+
+        // ---- program storage: the added queries' programs behind the used ones (a full buffer is replaced by one twice its size), or the
+        // live queries' programs compacted into buffers of their size
+        DevBuf g_q, g_ops, g_pt, g_cov;
+        uint64_t ops_used = B.ops_used, pt_used = B.pt_used, cov_used = B.cov_used;
+        auto     append   = [&](DevBuf &cur, DevBuf &grown, size_t used, const void *src, size_t n) -> cudaError_t {
+                DevBuf *dst = &cur;
+                if (used + n > cur.cap) {
+                        if (const cudaError_t e = grown.ensure(std::max(used + n, 2 * cur.cap)); e != cudaSuccess)
+                                return e;
+                        if (used)
+                                if (const cudaError_t e = cudaMemcpyAsync(grown.p, cur.p, used, cudaMemcpyDeviceToDevice, st); e != cudaSuccess)
+                                        return e;
+                        dst = &grown;
+                }
+                return n ? cudaMemcpyAsync(static_cast<char *>(dst->p) + used, src, n, cudaMemcpyHostToDevice, st) : cudaSuccess;
+        };
+        if (S) {
+                CKPU(append(B.d_queries, g_q, size_t(nq) * sizeof(PercQuery), S->queries.data(), S->queries.size() * sizeof(PercQuery)));
+                CKPU(append(B.d_ops, g_ops, B.ops_used * sizeof(PercOp), S->ops.data(), S->ops.size() * sizeof(PercOp)));
+                CKPU(append(B.d_pterms, g_pt, B.pt_used * 4, S->phrase_terms.data(), S->phrase_terms.size() * 4));
+                CKPU(append(B.d_covers, g_cov, B.cov_used * 4, S->covers.data(), S->covers.size() * 4));
+                ops_used += S->ops.size();
+                pt_used += S->phrase_terms.size();
+                cov_used += S->covers.size();
+        } else if (compact) {
+                ops_used = pt_used = cov_used = 0;
+                for (uint32_t q = 0; q < nq; ++q)
+                        if (!((*removed)[q >> 5] >> (q & 31u) & 1u)) {
+                                ops_used += B.sizes[q].nops;
+                                pt_used += B.sizes[q].npt;
+                                cov_used += B.sizes[q].ncover;
+                        }
+                DevBuf c_n, c_s; // per id: its ops / phrase terms / cover terms, and their scans
+                CKPU(c_n.ensure(std::max<size_t>(16, size_t(nq) * 12)));
+                CKPU(c_s.ensure((size_t(nq) + 1) * 24));
+                CKPU(g_q.ensure(std::max<size_t>(16, size_t(nq) * sizeof(PercQuery))));
+                CKPU(g_ops.ensure(std::max<size_t>(16, ops_used * sizeof(PercOp))));
+                CKPU(g_pt.ensure(std::max<size_t>(16, pt_used * 4)));
+                CKPU(g_cov.ensure(std::max<size_t>(16, cov_used * 4)));
+                uint32_t *          cn = c_n.as<uint32_t>();
+                unsigned long long *cs = c_s.as<unsigned long long>();
+                CKPU(launch_perc_upd_prog_sizes(B.d_queries.as<PercQuery>(), B.d_ops.as<PercOp>(), nq, rm, cn, cn + nq, cn + 2 * size_t(nq), st));
+                for (int k = 0; k < 3; ++k)
+                        CKPU(launch_enc_scan(cn + k * size_t(nq), nq, B.d_upart.as<unsigned long long>(), cs + k * (size_t(nq) + 1), st));
+                CKPU(launch_perc_upd_prog_scatter(B.d_queries.as<PercQuery>(), B.d_ops.as<PercOp>(), B.d_pterms.as<uint32_t>(), B.d_covers.as<uint32_t>(), nq, rm,
+                                                  cs, cs + (size_t(nq) + 1), cs + 2 * (size_t(nq) + 1), g_q.as<PercQuery>(), g_ops.as<PercOp>(),
+                                                  g_pt.as<uint32_t>(), g_cov.as<uint32_t>(), st));
+                CKPU(cudaStreamSynchronize(st)); // c_n / c_s are freed on return
+        }
+
+        // ---- the anchor index: surviving old entries of every term, then its new ones
+        uint32_t *          keep  = B.d_keep.as<uint32_t>();
+        unsigned long long *kscan = B.d_kscan.as<unsigned long long>(), *part = B.d_upart.as<unsigned long long>();
+        CKPU(up(B.d_new, ne.data(), ne.size() * sizeof(PercEntry)));
+        CKPU(up(B.d_new_terms, nterm.data(), nterm.size() * 4));
+        CKPU(launch_perc_upd_keep(B.d_csr.as<PercEntry>(), nold, rm, keep, st));
+        CKPU(launch_enc_scan(keep, nold, part, kscan, st));
+        CKPU(launch_perc_upd_csr(B.d_csr.as<PercEntry>(), B.d_csr_off.as<uint32_t>(), nt, nold, keep, kscan, B.d_new.as<PercEntry>(),
+                                 B.d_new_terms.as<uint32_t>(), uint32_t(nnew), B.d_cnt.as<uint32_t>(), part, B.d_toff.as<unsigned long long>(),
+                                 n_csr.as<PercEntry>(), n_off.as<uint32_t>(), st));
+        // ---- the unanchored list: its surviving ids, then the added ones
+        CKPU(up(B.d_new_unanch, S ? S->unanchored.data() : nullptr, size_t(nadd_u) * 4));
+        CKPU(launch_perc_upd_keep(B.d_unanch.as<uint32_t>(), nold_u, rm, keep, st));
+        CKPU(launch_enc_scan(keep, nold_u, part, kscan, st));
+        CKPU(launch_perc_upd_unanch(B.d_unanch.as<uint32_t>(), nold_u, keep, kscan, B.d_new_unanch.as<uint32_t>(), nadd_u, n_un.as<uint32_t>(), st));
+        CKPU(cudaEventRecord(B.uev[1], st));
+        CKPU(cudaStreamSynchronize(st));
+
+        // ---- every step succeeded: the new buffers replace the old ones
+        B.d_csr_off = std::move(n_off);
+        B.d_csr     = std::move(n_csr);
+        B.d_unanch  = std::move(n_un);
+        const std::pair<DevBuf *, DevBuf *> grown[] = {{&g_q, &B.d_queries}, {&g_ops, &B.d_ops}, {&g_pt, &B.d_pterms}, {&g_cov, &B.d_covers}};
+        for (const auto &[g, b] : grown)
+                if (g->p)
+                        *b = std::move(*g);
+        B.nentries    = nentries;
+        B.nunanchored = nunanchored;
+        B.ops_used    = ops_used;
+        B.pt_used     = pt_used;
+        B.cov_used    = cov_used;
+        (void)cudaEventElapsedTime(&B.update_ms, B.uev[0], B.uev[1]);
+        B.update_host_ms = float(now_ms() - t0);
+        return TRN_OK;
+}
+
+extern "C" int trn_percolator_add(trn_ctx *c, const trn_query *queries, uint32_t nq, uint32_t *first_id, trn_percolator_info *out) {
+        static const char *fn = "trn_percolator_add";
+        if (!c)
+                return TRN_ERR_ARG;
+        if (nq && !queries)
+                return fail(c, TRN_ERR_ARG, "trn_percolator_add: bad arguments");
+        auto &B = c->pq;
+        if (!B.have)
+                return fail(c, TRN_ERR_STATE, "trn_percolator_add: no query set registered (trn_percolator_register)");
+        CK(cudaSetDevice(c->device));
+        const uint32_t first = B.next_id;
+        if (nq) {
+                if (uint64_t(B.next_id) + nq > c->perc_max_ids)
+                        return fail(c, TRN_ERR_CAPACITY, "trn_percolator_add: ids would reach " + std::to_string(c->perc_max_ids) + " (" +
+                                                             std::to_string(B.next_id) + " issued; register the set again to start at 0)");
+                PercPlan    S;
+                std::string err;
+                if (const int rc = perc_plan_queries(queries, nq, B.next_id, B.nterms, B.term_cost.empty() ? nullptr : B.term_cost.data(), S, err))
+                        return fail(c, rc, "trn_percolator_add: " + err);
+                if (B.nentries + S.covers.size() >= c->perc_max_entries || B.cov_used + S.covers.size() >= (1ull << 32) ||
+                    B.ops_used + S.ops.size() >= (1ull << 32) || B.pt_used + S.phrase_terms.size() >= (1ull << 32))
+                        return fail(c, TRN_ERR_CAPACITY, "trn_percolator_add: the registry's anchor entries or program words would reach its limit (" +
+                                                             std::to_string(B.nentries + S.covers.size()) + " anchor entries)");
+                // rebase the slice onto the used program storage
+                for (PercQuery &Q : S.queries) {
+                        Q.op_begin += uint32_t(B.ops_used);
+                        Q.cover_begin += uint32_t(B.cov_used);
+                }
+                for (PercOp &o : S.ops)
+                        if (o.op == PERC_PHRASE)
+                                o.term += uint32_t(B.pt_used);
+                const uint64_t nentries = B.nentries + S.covers.size();
+                const uint32_t nun      = B.nunanchored + uint32_t(S.unanchored.size());
+                if (const int rc = perc_update(c, fn, &S, nullptr, false, nentries, nun))
+                        return rc;
+                for (uint32_t q = 0; q < nq; ++q)
+                        B.sizes.push_back({S.queries[q].nops, S.npt[q], S.queries[q].ncover, S.status[q]});
+                B.next_id += nq;
+                B.removed.resize((size_t(B.next_id) + 31u) / 32u, 0u);
+                B.nlive += nq;
+                B.nnever += S.never;
+        }
+        if (first_id)
+                *first_id = first;
+        perc_refresh_info(B);
+        if (out)
+                *out = B.info;
+        return TRN_OK;
+}
+
+extern "C" int trn_percolator_remove(trn_ctx *c, const uint32_t *ids, uint32_t n, trn_percolator_info *out) {
+        static const char *fn = "trn_percolator_remove";
+        if (!c)
+                return TRN_ERR_ARG;
+        if (n && !ids)
+                return fail(c, TRN_ERR_ARG, "trn_percolator_remove: bad arguments");
+        auto &B = c->pq;
+        if (!B.have)
+                return fail(c, TRN_ERR_STATE, "trn_percolator_remove: no query set registered (trn_percolator_register)");
+        CK(cudaSetDevice(c->device));
+        if (n) {
+                std::vector<uint32_t> rem = B.removed;
+                uint64_t              nentries = B.nentries, dead = B.dead_words;
+                uint32_t              nun = B.nunanchored, nnever = B.nnever;
+                for (uint32_t i = 0; i < n; ++i) {
+                        const uint32_t q = ids[i];
+                        if (q >= B.next_id)
+                                return fail(c, TRN_ERR_ARG, "trn_percolator_remove: id " + std::to_string(q) + " was never issued (next id " + std::to_string(B.next_id) + ")");
+                        if (rem[q >> 5] >> (q & 31u) & 1u)
+                                return fail(c, TRN_ERR_ARG, "trn_percolator_remove: id " + std::to_string(q) +
+                                                                (B.removed[q >> 5] >> (q & 31u) & 1u ? " was already removed" : " appears twice"));
+                        rem[q >> 5] |= 1u << (q & 31u);
+                        const auto &z = B.sizes[q];
+                        if (z.status == PERC_ANCHORED)
+                                nentries -= z.ncover;
+                        nun -= z.status == PERC_UNANCHORED;
+                        nnever -= z.status == PERC_NEVER;
+                        dead += 2ull * z.nops + z.npt + z.ncover;
+                }
+                // compact when the removed queries' program words outnumber the live ones
+                const uint64_t words   = 2ull * B.ops_used + B.pt_used + B.cov_used;
+                const bool     compact = dead > words - dead;
+                if (const int rc = perc_update(c, fn, nullptr, &rem, compact, nentries, nun))
+                        return rc;
+                B.removed    = std::move(rem);
+                B.dead_words = compact ? 0 : dead;
+                B.nlive -= n;
+                B.nnever = nnever;
+        }
+        perc_refresh_info(B);
+        if (out)
+                *out = B.info;
+        return TRN_OK;
+}
+
+extern "C" int trn_percolator_last_update(trn_ctx *c, float *device_ms, float *host_ms) {
+        if (!c)
+                return TRN_ERR_ARG;
+        if (device_ms)
+                *device_ms = c->pq.update_ms;
+        if (host_ms)
+                *host_ms = c->pq.update_host_ms;
+        return TRN_OK;
+}
+
+extern "C" int trn_debug_percolator_registry(trn_ctx *c, uint32_t *csr_off, uint32_t *csr, uint64_t cap, uint32_t *unanchored, uint64_t ucap,
+                                             uint32_t *nterms, uint64_t *nentries, uint64_t *nunanchored) {
+        if (!c)
+                return TRN_ERR_ARG;
+        auto &B = c->pq;
+        if (!B.have)
+                return fail(c, TRN_ERR_STATE, "trn_debug_percolator_registry: no query set registered (trn_percolator_register)");
+        if (nterms)
+                *nterms = B.nterms;
+        if (nentries)
+                *nentries = B.nentries;
+        if (nunanchored)
+                *nunanchored = B.nunanchored;
+        if ((csr && cap < B.nentries) || (unanchored && ucap < B.nunanchored))
+                return fail(c, TRN_ERR_CAPACITY, "trn_debug_percolator_registry: " + std::to_string(B.nentries) + " entries and " +
+                                                     std::to_string(B.nunanchored) + " unanchored ids do not fit");
+        CK(cudaSetDevice(c->device));
+        if (csr_off)
+                CK(cudaMemcpyAsync(csr_off, B.d_csr_off.p, (size_t(B.nterms) + 1) * 4, cudaMemcpyDeviceToHost, c->stream));
+        if (csr && B.nentries)
+                CK(cudaMemcpyAsync(csr, B.d_csr.p, B.nentries * sizeof(PercEntry), cudaMemcpyDeviceToHost, c->stream));
+        if (unanchored && B.nunanchored)
+                CK(cudaMemcpyAsync(unanchored, B.d_unanch.p, size_t(B.nunanchored) * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
         return TRN_OK;
 }
 

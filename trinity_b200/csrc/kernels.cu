@@ -966,6 +966,7 @@ __global__ void __launch_bounds__(kThreads) k_topk_merge(const uint32_t *docids,
 #include "collect.cuh"
 #include "intersect.cuh"
 #include "percolate.cuh"
+#include "percolate_update.cuh"
 #include "index_docs.cuh"
 #include "merge.cuh"
 

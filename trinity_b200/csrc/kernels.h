@@ -51,6 +51,21 @@ cudaError_t launch_isect_carry(const IsectParams &P, unsigned long long *carry, 
 // percolator (percolate.cuh): the count (write false) and write passes of trn_percolate over one launch's documents
 size_t      perc_smem_bytes(uint32_t max_len, uint32_t max_hash, bool write);
 cudaError_t launch_perc(const PercParams &P, bool write, int num_sms, cudaStream_t stream);
+// percolator registry updates (percolate_update.cuh): the keep flags of the old index / unanchored list, the index and unanchored rebuilds, and
+// the program-storage compaction of trn_percolator_add / trn_percolator_remove
+cudaError_t launch_perc_upd_keep(const PercEntry *csr, uint64_t n, const uint32_t *removed, uint32_t *keep, cudaStream_t stream);
+cudaError_t launch_perc_upd_keep(const uint32_t *ids, uint64_t n, const uint32_t *removed, uint32_t *keep, cudaStream_t stream);
+cudaError_t launch_perc_upd_csr(const PercEntry *csr, const uint32_t *csr_off, uint32_t nterms, uint64_t nold, const uint32_t *keep,
+                                const unsigned long long *kscan, const PercEntry *new_e, const uint32_t *new_terms, uint32_t nnew, uint32_t *cnt,
+                                unsigned long long *partials, unsigned long long *off, PercEntry *out, uint32_t *out_off, cudaStream_t stream);
+cudaError_t launch_perc_upd_unanch(const uint32_t *old, uint64_t nold, const uint32_t *keep, const unsigned long long *kscan, const uint32_t *add,
+                                   uint32_t nadd, uint32_t *out, cudaStream_t stream);
+cudaError_t launch_perc_upd_prog_sizes(const PercQuery *queries, const PercOp *ops, uint32_t nq, const uint32_t *removed, uint32_t *nops, uint32_t *npt,
+                                       uint32_t *ncov, cudaStream_t stream);
+cudaError_t launch_perc_upd_prog_scatter(const PercQuery *queries, const PercOp *ops, const uint32_t *pterms, const uint32_t *covers, uint32_t nq,
+                                         const uint32_t *removed, const unsigned long long *ops_at, const unsigned long long *pt_at,
+                                         const unsigned long long *cov_at, PercQuery *out_q, PercOp *out_ops, uint32_t *out_pt, uint32_t *out_cov,
+                                         cudaStream_t stream);
 // indexer (index_docs.cuh): document ranks, sort keys, one pass of the keys-only radix sort, the postings pass of trn_index_documents
 cudaError_t launch_index_doc_keys(const uint32_t *docids, uint32_t ndocs, unsigned long long *keys, cudaStream_t stream);
 cudaError_t launch_index_doc_ranks(const unsigned long long *keys, uint32_t ndocs, uint32_t *rank_of, uint32_t *docid_of, unsigned long long *errors,

@@ -32,6 +32,7 @@ struct PercPlan {
         std::vector<uint32_t>  csr_off; // nterms + 1
         std::vector<PercEntry> csr;
         std::vector<uint32_t>  unanchored;
+        std::vector<uint32_t>  npt; // per query: its phrase terms (consecutive in phrase_terms, in the order of its PHRASE ops)
         uint32_t               never{0};
 };
 
@@ -161,14 +162,18 @@ struct Builder {
 };
 } // namespace percplan_detail
 
+// The per-query part of the plan: queries[0 .. nq) get the ids first_id .. first_id + nq - 1 and their programs, covers and statuses are
+// appended to P (offsets relative to P's own arrays; P.unanchored holds ids).  A query's program, cover and status depend only on its tree,
+// nterms and term_cost, so planning a set in slices and concatenating them gives what planning it whole gives (trn_percolator_add).
 // Returns TRN_OK, or TRN_ERR_ARG (a malformed tree, a phrase of more than 16 terms, a term id >= nterms other than kEmptyTerm) /
 // TRN_ERR_UNSUPPORTED (a program that needs more than kPercStack pending operands) / TRN_ERR_CAPACITY (2^32 anchor entries), naming the
-// query in err.
-inline int perc_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, PercPlan &P, std::string &err) {
-        P = PercPlan{};
-        P.queries.resize(nq);
-        P.status.resize(nq);
-        std::vector<std::vector<uint32_t>> cov(nq);
+// query by its index in `queries` in err.
+inline int perc_plan_queries(const trn_query *queries, uint32_t nq, uint32_t first_id, uint32_t nterms, const uint32_t *term_cost, PercPlan &P,
+                             std::string &err) {
+        const size_t q0 = P.queries.size();
+        P.queries.resize(q0 + nq);
+        P.status.resize(q0 + nq);
+        P.npt.resize(q0 + nq);
         for (uint32_t q = 0; q < nq; ++q) {
                 const trn_query &Q   = queries[q];
                 const std::string who = "query " + std::to_string(q) + ": ";
@@ -179,20 +184,22 @@ inline int perc_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, con
                         return TRN_ERR_ARG;
                 }
                 percplan_detail::Builder b{Q.nodes, term_cost, P};
-                PercQuery &              R = P.queries[q];
-                R.op_begin                 = uint32_t(P.ops.size());
-                percplan_detail::Cover c   = b.node(Q.root);
-                R.nops                     = uint32_t(P.ops.size()) - R.op_begin;
+                PercQuery &              R  = P.queries[q0 + q];
+                const size_t             pt = P.phrase_terms.size();
+                R.op_begin                  = uint32_t(P.ops.size());
+                percplan_detail::Cover c    = b.node(Q.root);
+                R.nops                      = uint32_t(P.ops.size()) - R.op_begin;
                 if (b.max_depth > kPercStack) {
                         err = who + "its program needs " + std::to_string(b.max_depth) + " pending operands (at most " + std::to_string(kPercStack) + ")";
                         return TRN_ERR_UNSUPPORTED;
                 }
-                P.status[q]   = c.kind;
-                R.cover_begin = uint32_t(P.covers.size());
-                R.ncover      = uint32_t(c.terms.size());
+                P.status[q0 + q] = c.kind;
+                P.npt[q0 + q]    = uint32_t(P.phrase_terms.size() - pt);
+                R.cover_begin    = uint32_t(P.covers.size());
+                R.ncover         = uint32_t(c.terms.size());
                 P.covers.insert(P.covers.end(), c.terms.begin(), c.terms.end());
                 if (c.kind == PERC_UNANCHORED)
-                        P.unanchored.push_back(q);
+                        P.unanchored.push_back(first_id + q);
                 else if (c.kind == PERC_NEVER)
                         ++P.never;
                 if (P.covers.size() >= (1ull << 32)) {
@@ -200,6 +207,15 @@ inline int perc_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, con
                         return TRN_ERR_CAPACITY;
                 }
         }
+        return TRN_OK;
+}
+
+// The whole registration: the per-query part over every query (ids 0 .. nq - 1), then the term -> (query, ordinal) CSR, ascending query id
+// within every term.  The refusals of perc_plan_queries.
+inline int perc_plan(const trn_query *queries, uint32_t nq, uint32_t nterms, const uint32_t *term_cost, PercPlan &P, std::string &err) {
+        P = PercPlan{};
+        if (const int rc = perc_plan_queries(queries, nq, 0, nterms, term_cost, P, err))
+                return rc;
         P.csr_off.assign(size_t(nterms) + 1u, 0u);
         for (const uint32_t t : P.covers)
                 ++P.csr_off[t + 1u];
